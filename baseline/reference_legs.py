@@ -1,7 +1,6 @@
 #!/usr/bin/env python
 """The UNMODIFIED reference (traceopt-ai/traceml 0.2.15, installed into the git-ignored
-``baseline/_ref`` by ``python -m pip install --no-index --no-build-isolation --no-deps
---target baseline/_ref <copy of /root/reference>``) timed on this box's host cores.
+``oracle/_ref`` by ``oracle/install_reference.py``) timed on the host's cores.
 
 This file never imports the engine (``traceml_b200.engine`` / ``_abi`` / any ``.so`` of this
 repository): ``bench.py --impl reference`` runs it as a separate process so that the
@@ -35,7 +34,7 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.path.join(HERE, "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def _paths():
@@ -49,7 +48,7 @@ def _paths():
 
 def _envelope(sampler, rank, world, rows):
     return {"rank": rank, "global_rank": rank, "local_rank": rank, "world_size": world,
-            "local_world_size": world, "node_rank": 0, "hostname": "b200-box", "pid": 1000 + rank,
+            "local_world_size": world, "node_rank": 0, "hostname": "bench-host", "pid": 1000 + rank,
             "sampler": sampler, "timestamp": 0.0, "tables": {"t": rows}}
 
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the reference's headline metric on B200.
+"""bench.py -- the reference's headline metric on H100.
 
 BASELINE.json metric: "per-step profiling overhead (us) at 1/2/4/8 ranks;
 cross-rank reduce GB/s".  One invocation measures both legs:
@@ -16,19 +16,19 @@ cross-rank reduce GB/s".  One invocation measures both legs:
       pinned == to the row-level oracle, pinned == to the unmodified reference) on the same
       seed, outside the timed region.  default_window = the reference's default W = 10^4 on
       the same seed in BOTH arms: this engine's time next to the UNMODIFIED reference's
-      (baseline/_ref, separate process), and their summaries compared field by field.
+      (oracle/_ref, separate process), and their summaries compared field by field.
   step leg     (``step_overhead``)
       BASELINE config 2: synthetic ResNet-18 (batch 64x3x224x224, DDP when N > 1)
       and the isolated tiny-MLP micro-harness; per-step wall of untraced vs traced
       (this engine, auto mode); the reference's real ``traceml.trace_step`` is timed by
       baseline/reference_legs.py in its own process (rank 0).
 
-``--impl reference`` runs the UNMODIFIED reference (``baseline/_ref``: ``pip install --target``
-of /root/reference, git-ignored, travels with the snapshot) in a separate process that maps none
+``--impl reference`` runs the UNMODIFIED reference (``oracle/_ref``, git-ignored, installed by
+``oracle/install_reference.py``) in a separate process that maps none
 of this repository's native code: its own SQLite projection writers + its three summary
 sections on a bounded sample of the same workload (K timed steps, W warm-up; the sample per step is
 sized from K so that the whole run costs ~100 s of reference time, never above --sample rows), the default-window
-line at full size, and the real ``traceml.trace_step`` overhead leg.  If ``baseline/_ref`` is
+line at full size, and the real ``traceml.trace_step`` overhead leg.  If ``oracle/_ref`` is
 missing it falls back to the oracle port and says so (``cpu_baseline.kind: "port"``).
 
 Launch: ``python bench.py --gpus N --steps K --warmup W`` (N = 1) or under
@@ -85,7 +85,7 @@ def max_over_ranks(x: float, world: int, device) -> float:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -337,11 +337,11 @@ DEFAULT_PROC_ROWS = 2_000
 
 
 def ref_available() -> bool:
-    return os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "traceml"))
+    return os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "traceml"))
 
 
 def ref_leg(argv, timeout=1500) -> dict:
-    """Run baseline/reference_legs.py (the UNMODIFIED reference from baseline/_ref) in its own
+    """Run baseline/reference_legs.py (the UNMODIFIED reference from oracle/_ref) in its own
     process -- no module of this repository's engine is imported there -- and parse its JSON."""
     env = {k: v for k, v in os.environ.items()
            if k not in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "LOCAL_WORLD_SIZE", "GROUP_RANK", "MASTER_ADDR",
@@ -358,7 +358,7 @@ def ref_leg(argv, timeout=1500) -> dict:
 
 
 def oracle_reduce_sample(R: int, W: int, seed: int = 1):
-    """Fallback only (no baseline/_ref): the oracle port of the reference's CPU reduce."""
+    """Fallback only (no oracle/_ref): the oracle port of the reference's CPU reduce."""
     import replay
     from helpers import oracle_mem_rows, oracle_proc_rows, oracle_time_rows
     from oracle import process_oracle, step_memory_oracle, step_time_oracle
@@ -453,7 +453,7 @@ def run_reference(args, rank, world):
             "value": val, "ms_per_step": t * 1e3,
             "cpu_baseline": {
                 "value": val, "unit": "GB/s", "cores": 1, "kind": "reference",
-                "sample": f"each step = the UNMODIFIED reference (baseline/_ref, own process): "
+                "sample": f"each step = the UNMODIFIED reference (oracle/_ref, own process): "
                           f"StepTime/StepMemory/Process SummarySection.build(db) on R={R} ranks x {Ws} rows of the "
                           f"workload, SQLite written by the reference's own projection writers; "
                           f"{red['us_per_row']:.1f} us/row, single-threaded Python (1 of {os.cpu_count()} cores)",
@@ -483,7 +483,7 @@ def run_reference(args, rank, world):
         line.update({
             "value": val, "ms_per_step": t * 1e3,
             "cpu_baseline": {"value": val, "unit": "GB/s", "cores": 1, "kind": "port",
-                             "sample": f"baseline/_ref missing: oracle port, R={R} x W={Ws} rows pre-parsed"},
+                             "sample": f"oracle/_ref missing: oracle port, R={R} x W={Ws} rows pre-parsed"},
             "e2e": {"value": val, "unit": "GB/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}})
     print(json.dumps(line))
 
@@ -654,12 +654,61 @@ def default_window_leg(rank, local, world, device, comm):
                 out["reference"] = dw
             else:
                 out["reference"] = {"ms": dw["s_per_step_median"] * 1e3, "us_per_row": dw["us_per_row"],
-                                    "kind": "unmodified reference, baseline/_ref, separate process, 1 core"}
+                                    "kind": "unmodified reference, oracle/_ref, separate process, 1 core"}
                 out["speedup_vs_reference"] = dw["s_per_step_median"] * 1e3 / ms
                 out["parity_vs_reference"] = compare_digests(out["summary"], summary_digest(dw["summary"]))
     barrier(world)
     eng.close()
     return out
+
+
+# ----------------------------------------------------------------------------- --dump-outputs
+DUMP_SERIES_COLS = 1 << 17  # sampled steps per series over all ranks: 16 x 2^17 float64 = 16 MB
+
+
+def _flatten_numbers(obj, vals):
+    """Every numeric leaf of a section dict, in sorted-key order (strings are labels and None marks
+    a value the section does not have: both skipped)."""
+    if isinstance(obj, dict):
+        for k in sorted(obj, key=str):
+            _flatten_numbers(obj[k], vals)
+    elif isinstance(obj, (list, tuple)):
+        for v in obj:
+            _flatten_numbers(v, vals)
+    elif isinstance(obj, (bool, int, float, np.integer, np.floating)):
+        vals.append(float(obj))
+
+
+def capture_outputs(res, world: int, seed: int = 0) -> dict:
+    """What one ``SummaryEngine.build`` handed its caller, as float64 host arrays: the numbers of
+    the three sections and the per-step median / worst series (a fixed, seeded sample of the
+    steps when the window is larger than DUMP_SERIES_COLS, with the sampled step indices).  Each of
+    the ``world`` ranks samples its own shard, DUMP_SERIES_COLS / world steps of it, so that the
+    files of all ranks together stay within the same size."""
+    out = {}
+    for name in ("step_time", "step_memory", "process"):
+        vals = []
+        _flatten_numbers(res.get(name), vals)
+        out[name] = np.asarray(vals, dtype=np.float64)
+    seen = set()
+    for kind in ("time", "mem"):
+        k = getattr(res["reduce"], kind)
+        if k.series is None or not k.n_common or k.series.data_ptr() in seen:
+            continue
+        seen.add(k.series.data_ptr())
+        lo, hi = k.shard if k.shard[1] > k.shard[0] else (0, int(k.n_common))
+        take = min(hi - lo, max(1, DUMP_SERIES_COLS // world))
+        cols = lo + np.sort(np.random.default_rng(seed).choice(hi - lo, take, replace=False))
+        idx = torch.from_numpy(cols).to(k.series.device)
+        out[f"{kind}_series"] = k.series[:, idx].double().cpu().numpy()
+        out[f"{kind}_series_steps"] = cols.astype(np.float64)
+    return out
+
+
+def write_outputs(outdir: str, arrays: dict, rank: int, world: int) -> None:
+    os.makedirs(outdir, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(outdir, f"{name}.npy" if world == 1 else f"{name}_rank{rank}.npy"), arr)
 
 
 # ----------------------------------------------------------------------------- main arm
@@ -675,7 +724,11 @@ def main():
     ap.add_argument("--no-overhead", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(3, args.warmup) if args.impl == "b200" else args.warmup
 
     if args.impl == "reference":
@@ -729,6 +782,8 @@ def main():
     e1.record()
     torch.cuda.synchronize(device); barrier(world)
     launches = eng.launch_count - l0
+    # the series are views of the engine's workspace: copy them out before the next build
+    dumped = capture_outputs(res, world) if args.dump_outputs else None
     # stage breakdown (a diagnostic, outside the timed region: it adds a dozen torch events
     # per step).  The two kernels' own times (k3a, k4) above come from the timed steps.
     for _ in range(max(3, args.steps // 2)):
@@ -770,7 +825,7 @@ def main():
 
     # ---- roofline of the dominant kernels (per launch, this rank)
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    peak, peak_src = 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3"
     if os.path.exists(peaks_path):
         with open(peaks_path) as fh:
             peak = float(json.load(fh)["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst)"
@@ -790,25 +845,16 @@ def main():
         kernels = {"k_window_fused": {"ms": med.get("k3a"), "bytes": fb,
                                       "GBps": fb / (med["k3a"] * 1e-3) / 1e9 if med.get("k3a") else None}}
     if R > 1 and med.get("k4"):
-        # step-sharded K4 loads (R-1)/R of its rows from peer HBM: NVLink 5 is its bound, not the
-        # local HBM.  Denominator: the measured peer copy of 770 GB/s per direction per GPU
-        # (B200_PROFILING.md; 900 nominal)
+        # step-sharded K4 loads (R-1)/R of its rows from peer HBM: NVLink 4 is its bound, not the
+        # local HBM.  Denominator: the H100 SXM data sheet's 900 GB/s per GPU, 450 per direction
         nv = (R - 1) * n_shard * 64.0
         kernels["k_window_reduce"]["nvlink"] = {
-            "bytes_in": nv, "GBps": nv / (med["k4"] * 1e-3) / 1e9, "peak": 770.0, "nominal": 900.0,
-            "frac": nv / (med["k4"] * 1e-3) / 1e9 / 770.0,
-            "peak_source": "measured peer copy, B200_PROFILING.md"}
+            "bytes_in": nv, "GBps": nv / (med["k4"] * 1e-3) / 1e9, "peak": 450.0, "nominal": 900.0,
+            "frac": nv / (med["k4"] * 1e-3) / 1e9 / 450.0,
+            "peak_source": "H100 SXM data sheet, NVLink 4, one direction"}
     dom = max(kernels, key=lambda k: kernels[k]["ms"] or 0.0)
-    traffic = None
-    try:  # DRAM traffic per launch from the committed ncu capture, if it is this workload
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            tj = json.load(fh)
-        if tj.get("window") == W and tj.get("ranks") == R and dom in tj:
-            traffic = tj[dom]["dram_read_bytes"] + tj[dom]["dram_write_bytes"]
-    except Exception:
-        traffic = None
     roofline = {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["GBps"], "peak": peak,
-                "unit": "GB/s", "frac": (kernels[dom]["GBps"] or 0.0) / peak, "traffic": traffic,
+                "unit": "GB/s", "frac": (kernels[dom]["GBps"] or 0.0) / peak, "traffic": None,
                 "peak_source": peak_src, "kernels": kernels, "stage_ms": med}
 
     # ---- (2) end to end from HOST buffers: H2D + reduce + results on the host
@@ -871,7 +917,7 @@ def main():
                 cpu = {"value": b_reduce(1, args.sample) / t / 1e9, "unit": "GB/s", "cores": 1, "kind": "reference",
                        "sample": f"R=1 x W={args.sample} rows of the same workload ({t:.2f} s/step, "
                                  f"{red['us_per_row']:.1f} us/row): the UNMODIFIED reference's three summary sections "
-                                 "over SQLite written by its own projection writers (baseline/_ref, own process)",
+                                 "over SQLite written by its own projection writers (oracle/_ref, own process)",
                        "host_cores": os.cpu_count(), "sqlite_projection": red["sqlite_projection"]}
             else:
                 cpu = {"error": red["error"], "kind": "reference"}
@@ -900,6 +946,8 @@ def main():
             "diagnosis": diagnosis, "bench_wall_s": time.perf_counter() - t_bench0,
         }
         print(json.dumps(line))
+    if dumped is not None:
+        write_outputs(args.dump_outputs, dumped, rank, world)
     if world > 1:
         torch.distributed.destroy_process_group()
 

@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """BASELINE config 5 on this engine: the reference's ``examples/huggingface_trainer_minimal.py``
 (TinyMLP, 200 steps, synthetic data) through the KEPT, UNMODIFIED ``TraceMLTrainer`` of the
-reference package (``baseline/_ref/traceml/integrations/huggingface.py:22-83``: a
+reference package (``oracle/_ref/traceml/integrations/huggingface.py:22-83``: a
 ``transformers.Trainer`` subclass whose ``training_step`` runs inside the reference's own
 ``trace_step``), bound to this engine by ``traceml_b200.shim`` (INTEGRATION.md option B), bf16, one
 rank per GPU.
 
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 \\
-        examples/hf_trainer_minimal.py --session-root profiles/r02_config5
+        examples/hf_trainer_minimal.py --session-root /tmp/traceml_config5
 
 ``transformers.Trainer`` needs the ``accelerate`` package (transformers >= 4.x raises ImportError in
 ``Trainer.__init__`` without it) and this image has none.  The script first tries the real
@@ -30,7 +30,7 @@ from torch.utils.data import DataLoader, Dataset
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "baseline", "_ref"))   # the installed reference package
+sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))   # the installed reference package
 os.environ.setdefault("TRACEML_LOGS_DIR", "/tmp/traceml_ref_logs")
 import traceml  # noqa: E402  -- the REFERENCE's package: its API, patches and integrations, unmodified
 import traceml_b200  # noqa: E402

@@ -4,7 +4,7 @@ seq 1024, batch 8 per rank) with process telemetry sampled at 1 kHz by the nativ
 ``--seconds`` (default 60), then the cross-rank reduce.
 
     python -m torch.distributed.run --nproc-per-node 8 --master-addr 127.0.0.1 \\
-        examples/transformer_1khz_ddp.py --seconds 60 --session-root profiles/r02_config4
+        examples/transformer_1khz_ddp.py --seconds 60 --session-root /tmp/traceml_config4
 
 The traced loop is the stock drop-in (``traceml.init(mode="auto")``, ``with traceml.trace_step(model)``,
 ``traceml.final_summary()``).  Rank 0 prints one JSON line with what was measured: steps, step

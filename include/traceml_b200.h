@@ -1,5 +1,5 @@
 /*
- * traceml_b200.h -- C-ABI of libtraceml_b200.so, the B200-native telemetry engine.
+ * traceml_b200.h -- C-ABI of libtraceml_b200.so, the GPU-native telemetry engine (H100, sm_90a).
  *
  * The reference (traceopt-ai/traceml v0.2.15) is pure Python and has no FFI;
  * its "operator API" for this path is the set of Python seams listed in

@@ -3,7 +3,7 @@ Step-Time and Step-Memory sections restated with numpy.  TEST INFRASTRUCTURE ONL
 (tests/, __graft_entry__.smoke(), bench.py's parity + cpu_baseline legs).
 
 The row-level restatement (``step_time_oracle.py`` / ``step_memory_oracle.py``) walks every row
-in Python (~70 us/row): fine up to ~2*10^5 rows, hopeless at bench.py's W = 4*10^6.  This module
+in Python: fine up to ~2*10^5 rows, hopeless at bench.py's W = 4*10^6.  This module
 vectorises exactly the O(R*W) stages and then hands over to the SAME downstream functions
 (``step_time_oracle.diagnose_summary / global_points / overview``,
 ``step_memory_oracle.diagnose_summary / rollup_points``), so labels, rank ids and strings come
@@ -12,7 +12,7 @@ equality (``==`` on floats) with the row-level oracle on every step golden case 
 random windows, which in turn is pinned ``==`` against the unmodified reference
 (``tests/golden/make_golden.py``).
 
-What keeps it bit-exact with the reference (file:line = /root/reference/src/traceml/...):
+What keeps it bit-exact with the reference (file:line = the reference's src/traceml/...):
   * ns -> ms is IEEE division ``ns / 1e6`` (the wire rows carry ``duration_ms`` computed that way);
   * per-rank window sums are the reference's plain ``s += x`` loops over rows in DESCENDING step
     order (reporting/sections/step_time/model.py:241-268, loader.py ``ORDER BY step DESC``;

@@ -1,6 +1,6 @@
 """Workload for an ncu capture of K4 under REAL peer loads: torchrun, one rank per GPU, every rank
 holds W step records, the native driver reduces with the fused NVLink peer-load exchange ("p2p").
-Launch through profiles/ncu_rank0.sh so that only rank 0 runs under ncu.
+Launch it under torchrun with the profiler wrapping rank 0 only.
 Usage: ... profiles/run_reduce_p2p.py [W] [reps]"""
 import os
 import sys

@@ -2,7 +2,7 @@
 
 ``-m "not gpu"``: oracle vs golden vectors, host logic, C-ABI symbol checks,
 world_size-2 gloo runs -- no CUDA device needed.
-``-m gpu``: parity tests proper, through the C-ABI on a real B200.
+``-m gpu``: parity tests proper, through the C-ABI on a real H100.
 """
 import os
 import sys
@@ -13,13 +13,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_sessionstart(session):
     """Build the native library in-tree if it is missing (a fresh checkout has no .so: they
-    are git-ignored).  nvcc cross-compiles without a GPU; on the GPU box the prebuilt library
-    travels with the snapshot and this is a no-op."""
+    are git-ignored).  nvcc cross-compiles without a GPU; after build() this is a no-op."""
     try:
         import __graft_entry__ as entry
 

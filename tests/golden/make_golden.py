@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Generate tests/golden/*.json from the UNMODIFIED reference.
 
-Run in the build container only (needs /root/reference):
+Needs the unmodified reference installed into oracle/_ref (oracle/install_reference.py):
 
     python tests/golden/make_golden.py
 
@@ -14,8 +14,8 @@ For every case it
      oracle's parity pin -- and
   5. writes inputs' digest + the reference outputs as the golden vector.
 
-The golden files are what the GPU parity tests compare against on the GPU
-box, where /root/reference does not exist.
+The golden files are what the tests compare against wherever the reference
+is not installed.
 """
 
 from __future__ import annotations
@@ -32,7 +32,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, "/root/reference/src")
+sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
 
 import numpy as np  # noqa: E402
 

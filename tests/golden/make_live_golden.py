@@ -2,7 +2,7 @@
 """Generate tests/golden/live/*.json from the UNMODIFIED reference's live
 Step-Time computer (renderers/step_time/compute.py, StepCombinedComputer).
 
-Build container only (needs /root/reference):
+Needs the unmodified reference installed into oracle/_ref:
 
     python tests/golden/make_live_golden.py
 

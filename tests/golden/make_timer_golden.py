@@ -6,7 +6,7 @@ Runs the SAME scripted training loop (fake deterministic clock) through
       traceml.sdk.instrumentation.trace_step, StepTimeSampler / StepMemorySampler;
   (2) oracle.timer_oracle.ReferenceTimerPath
 and asserts the emitted wire rows are identical; writes them to
-tests/golden/timer_rows.json.  CPU only (the build container has no GPU), so
+tests/golden/timer_rows.json.  CPU only, so
 this pins the host-clock half: step numbering, accumulate-by-name, n_calls,
 dataloader_next flushed with the following step, failed-step flush under the
 old id, NULL memory on CPU.
@@ -18,7 +18,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference/src")
+sys.path.insert(0, os.path.join(ROOT, "oracle", "_ref"))
 
 import time  # noqa: E402
 

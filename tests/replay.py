@@ -33,7 +33,7 @@ from traceml_b200.records import (
 
 GIB = 1024 ** 3
 MIB = 1024 ** 2
-GPU_TOTAL_BYTES = 183_359 * MIB  # B200: nvidia-smi reports 183,359 MiB
+GPU_TOTAL_BYTES = 183_359 * MIB  # a synthetic device total; the golden vectors were made with it
 
 STEP_SCENARIOS = (
     "balanced", "input_straggler", "compute_straggler", "straggler",

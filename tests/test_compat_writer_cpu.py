@@ -1,4 +1,4 @@
-"""CPU, build container only: a database written by traceml_b200.compat.SQLiteCompatWriter
+"""CPU, where the reference is installed in oracle/_ref: a database written by traceml_b200.compat.SQLiteCompatWriter
 is consumed by the reference's OWN final-report sections and yields the golden payloads
 (the kept consumers keep working on our output)."""
 import os
@@ -6,7 +6,7 @@ import sys
 
 import pytest
 
-REF_SRC = "/root/reference/src"
+REF_SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 if os.path.isdir(REF_SRC) and REF_SRC not in sys.path:
     sys.path.append(REF_SRC)
 pytest.importorskip("traceml.reporting.sections.step_time", reason="reference not importable here")

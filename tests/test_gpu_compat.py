@@ -1,6 +1,6 @@
 """GPU, f1: records produced by the KERNELS on a real training loop are drained into the
 compatibility SQLite (traceml_b200/compat.py) and consumed by the UNMODIFIED reference
-(baseline/_ref): its three summary sections, its FinalReportGenerator (``final_summary.json`` of the
+(oracle/_ref): its three summary sections, its FinalReportGenerator (``final_summary.json`` of the
 aggregator path) and ``traceml compare`` -- next to this engine's own in-process summary of the
 same records (aggregator/sqlite_writers/step_time.py:172-187, database/database_sender.py:49-66)."""
 import json
@@ -14,14 +14,14 @@ from helpers import plain
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 def test_reference_consumers_read_device_fed_database(tmp_path):
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     if not os.path.isdir(os.path.join(REF, "traceml")):
-        pytest.skip("baseline/_ref (the installed reference) is not present")
+        pytest.skip("oracle/_ref (the installed reference) is not present")
     os.environ.setdefault("TRACEML_LOGS_DIR", "/tmp/traceml_ref_logs")
     if REF not in sys.path:
         sys.path.insert(0, REF)

@@ -1,6 +1,6 @@
 """GPU, f4: deep profile -- per-layer forward / backward device timers and activation sizes
 (K1 / K2 with a layer id) next to CUDA events around the same layers, and next to the
-reference's own layer hooks when baseline/_ref is present."""
+reference's own layer hooks when oracle/_ref is present."""
 import os
 import sys
 
@@ -10,7 +10,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 @pytest.fixture()
@@ -115,7 +115,7 @@ def test_layer_times_next_to_the_reference_hooks(deep):
     """The UNMODIFIED reference's layer forward timing hooks (CUDA events resolved by its sampler
     helper) on the same model in the same steps."""
     if not os.path.isdir(os.path.join(REF, "traceml")):
-        pytest.skip("baseline/_ref is not present")
+        pytest.skip("oracle/_ref is not present")
     os.environ.setdefault("TRACEML_LOGS_DIR", "/tmp/traceml_ref_logs")
     if REF not in sys.path:
         sys.path.insert(0, REF)

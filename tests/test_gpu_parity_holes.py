@@ -10,7 +10,6 @@
 (d) a1: stamp durations bracketed by CUDA events on both sides, SURVEY 8d tolerance
     (2 us + 1 %), and next to the reference's own CUDA-event timer path.
 """
-import json
 import os
 import sys
 import time
@@ -23,7 +22,7 @@ from helpers import assert_struct, plain, strip_device
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 
 @pytest.fixture(scope="module")
@@ -186,7 +185,7 @@ def test_step_memory_peaks_are_torch_exact(cuda):
 # ------------------------------------------------------------------------------------ (c)
 def _reference():
     if not os.path.isdir(os.path.join(REF, "traceml")):
-        pytest.skip("baseline/_ref (the installed reference) is not present")
+        pytest.skip("oracle/_ref (the installed reference) is not present")
     if REF not in sys.path:
         sys.path.insert(0, REF)
     os.environ.setdefault("TRACEML_LOGS_DIR", "/tmp/traceml_ref_logs")
@@ -296,7 +295,7 @@ def test_stamp_bracketed_by_cuda_events(cuda):
 
     The stamp kernels and the CUDA events are all in-stream timestamps; an event recorded
     OUTSIDE the stamp pair must see at least the stamp duration, one recorded INSIDE at most.
-    The measured deltas are written to gpurun_out/ (committed under profiles/)."""
+    The measured deltas travel in the assertion messages."""
     from traceml_b200.engine import Engine
 
     eng = Engine(device=0, ring_slots=1024)
@@ -329,9 +328,6 @@ def test_stamp_bracketed_by_cuda_events(cuda):
             "stamp_minus_inner": np.percentile(stamp - inner, [0, 5, 50, 95, 99, 100]).tolist(),
             "outer_minus_inner": np.percentile(outer - inner, [0, 5, 50, 95, 99, 100]).tolist(),
             "stamp_us": np.percentile(stamp, [0, 50, 100]).tolist(), "percentiles": [0, 5, 50, 95, 99, 100]}
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "timer_delta_hist.json"), "w") as fh:
-        json.dump(hist, fh, indent=1)
     assert (stamp <= outer + tol).all(), hist
     assert (stamp >= inner - tol).all(), hist
     # means over >= 100 steps: the stamp mean lies inside the bracket means, 0.5 %

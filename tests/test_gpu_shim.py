@@ -14,7 +14,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 SCRIPT = r"""
 import os, sys
@@ -27,7 +27,7 @@ import traceml                                   # the reference
 from traceml.runtime.state import reset_trace_session_state
 from traceml_b200 import runtime, shim
 
-assert "baseline/_ref" in traceml.__file__.replace(os.sep, "/")
+assert "oracle/_ref" in traceml.__file__.replace(os.sep, "/")
 patched = shim.install()
 assert "traceml.sdk.instrumentation.timed_region" in patched
 reset_trace_session_state(0)
@@ -68,6 +68,6 @@ def test_reference_trace_step_records_through_the_c_abi():
     if not torch.cuda.is_available():
         pytest.skip("no CUDA device")
     if not os.path.isdir(os.path.join(REF, "traceml")):
-        pytest.skip("baseline/_ref (the installed reference) is not present")
+        pytest.skip("oracle/_ref (the installed reference) is not present")
     p = subprocess.run([sys.executable, "-c", SCRIPT, ROOT, REF], capture_output=True, text=True, timeout=300)
     assert p.returncode == 0 and "SHIM_OK" in p.stdout, (p.stdout[-2000:], p.stderr[-3000:])

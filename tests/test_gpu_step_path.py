@@ -341,7 +341,7 @@ def test_final_summary_public_api(cuda):
     out = traceml.final_summary(print_text=False)
     assert out is not None and out["schema_version"] == 1.2
     st = out["step_time"]
-    if "data" in st:   # reference not installed on this box: native envelope
+    if "data" in st:   # reference not installed: native envelope
         assert st["data"]["training_steps"] == 65
         assert st["data"]["aligned_window"]["steps_analyzed"] == 64
         assert st["data"]["aligned_window"]["start_step"] == 1

@@ -1,7 +1,7 @@
 """The KEPT live renderers fed from this package (SURVEY 8b down-facing seam, 8f-2): the
 reference's own ``StepCombinedRenderer`` / ``StepMemoryRenderer`` render the same panel text
 whether their computer reads the reference's SQLite (the reference path) or is replaced by
-``traceml_b200.live`` over the engine double.  Needs the reference importable (build container)."""
+``traceml_b200.live`` over the engine double.  Needs the reference installed in oracle/_ref."""
 import io
 import os
 import sys
@@ -10,7 +10,7 @@ import tempfile
 import pytest
 import torch
 
-REF_SRC = "/root/reference/src"
+REF_SRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 if os.path.isdir(REF_SRC) and REF_SRC not in sys.path:
     sys.path.insert(0, REF_SRC)
 pytest.importorskip("traceml.renderers.step_time.renderer", reason="reference not importable here")

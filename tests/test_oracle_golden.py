@@ -1,5 +1,5 @@
 """CPU: the oracle against the committed golden vectors (the reference's own
-outputs, produced by tests/golden/make_golden.py in the build container)."""
+outputs, produced by tests/golden/make_golden.py)."""
 import pytest
 
 from oracle import process_oracle, step_memory_oracle, step_time_oracle

@@ -1,4 +1,4 @@
-"""CPU, build container only (needs the reference importable): the bridge to the KEPT
+"""CPU, where the reference is installed in oracle/_ref: the bridge to the KEPT
 payload builders.  Section dicts in the product's format (numbers from the oracle,
 diagnoses from the native C++ engines) -> traceml_b200.reporting.to_reference_* ->
 the reference's own build_*_payload / formatters == the golden payload JSON + card text."""
@@ -7,16 +7,12 @@ import sys
 
 import pytest
 
-REF_SRC = "/root/reference/src"
-if os.path.isdir(REF_SRC) and REF_SRC not in sys.path:
-    sys.path.append(REF_SRC)
-
 from helpers import (assert_struct, golden_cases, oracle_mem_rows, oracle_time_rows, plain,
                      proc_replay_for, step_replay_for)
 
 reporting = pytest.importorskip("traceml_b200.reporting")
 if not reporting.reference_available():
-    pytest.skip("reference package not importable on this box", allow_module_level=True)
+    pytest.skip("the reference is not installed in oracle/_ref", allow_module_level=True)
 
 from oracle import step_memory_oracle, step_time_oracle  # noqa: E402
 from test_native_diag_cpu import _agg_from_records  # noqa: E402

@@ -1,8 +1,12 @@
 """CPU: SDK policy and host-side semantics (mirrors the intent of the reference's
 tests/sdk/test_init_and_wrappers.py:34-417 and tests/runtime/test_trace_session_state.py)."""
+import os
+
 import pytest
 import torch
 import torch.nn as nn
+
+REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref")
 
 
 @pytest.fixture()
@@ -139,13 +143,12 @@ def test_kept_huggingface_integration_imports_against_this_package(monkeypatch):
     this package: it must import (TRACEML_DISABLED: no engine needed), expose ``TraceMLTrainer``
     on top of transformers' Trainer, and its bypass path must not touch the engine."""
     import importlib.util
-    import os
     import sys
     import types
 
-    ref = "/root/reference/src/traceml/integrations/huggingface.py"
+    ref = os.path.join(REF, "traceml", "integrations", "huggingface.py")
     if not os.path.exists(ref):
-        pytest.skip("reference not present on this box")
+        pytest.skip("the reference is not installed in oracle/_ref")
     pytest.importorskip("transformers")
     monkeypatch.setenv("TRACEML_DISABLED", "1")
     from traceml_b200 import runtime
@@ -175,13 +178,12 @@ def test_kept_lightning_callback_imports_against_this_package(monkeypatch):
     seam modules (same module paths, same names): it must import and define its callback.
     (Lightning itself is stubbed: only ``Callback`` is needed at import time; the hook sequence
     is exercised on the GPU by test_gpu_step_path.py::test_lightning_style_seam_sequence.)"""
-    import os
     import sys
     import types
 
-    ref = "/root/reference/src/traceml/integrations/lightning.py"
+    ref = os.path.join(REF, "traceml", "integrations", "lightning.py")
     if not os.path.exists(ref):
-        pytest.skip("reference not present on this box")
+        pytest.skip("the reference is not installed in oracle/_ref")
     src = open(ref).read()
     wanted = ["from traceml.runtime.state import", "from traceml.utils.flush_buffers import",
               "from traceml.utils.step_memory import", "from traceml.utils.timing import"]

@@ -7,7 +7,7 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CANDIDATES = [os.path.join(ROOT, "baseline", "_ref"), "/root/reference/src"]
+CANDIDATES = [os.path.join(ROOT, "oracle", "_ref")]
 
 
 @pytest.fixture()

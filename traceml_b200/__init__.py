@@ -1,4 +1,4 @@
-"""traceml_b200 -- B200-native per-step telemetry + cross-rank diagnostics engine.
+"""traceml_b200 -- GPU-native (H100) per-step telemetry + cross-rank diagnostics engine.
 
 Drop-in for the hot path of traceopt-ai/traceml (v0.2.15): the per-step phase
 timers, the step/process memory samplers and the cross-rank step-alignment /

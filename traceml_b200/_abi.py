@@ -238,7 +238,7 @@ def lib() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"traceml_b200: native extension not found at {LIB_PATH}. Build it with "
-            "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). "
+            "`python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). "
             "There is no CPU fallback."
         )
     handle = C.CDLL(LIB_PATH)

@@ -1,4 +1,4 @@
-// tml_engine.cu -- kernels + C-ABI of the B200-native telemetry engine (sm_100a).
+// tml_engine.cu -- kernels + C-ABI of the GPU-native telemetry engine (H100, sm_90a).
 //
 // Kernel map (DESIGN.md section 4):
 //   K1  k_stamp_begin / k_stamp_end   %globaltimer phase stamps on the training stream
@@ -161,10 +161,9 @@ __global__ void k_stamp_end(DevState* st, u32 slot, u32 phase, u32 epoch) {
 // 6 warps: warp p owns phase p's running statistics; warp 0 also assembles the
 // 128-B record in shared memory and writes it as 8 x 16-B coalesced stores.
 
-// Nothing in here leaves the GPU: round 1 also wrote the record and the live statistics into
-// host-mapped memory and closed with __threadfence_system -- 7.6 us of the TRAINING stream per step
-// (r01 launch list) for the benefit of a sampler that looks twice a second.  The sampler now
-// fetches what it needs itself (k_mirror, on its own stream, tml_drain / tml_live).
+// Nothing in here leaves the GPU: writing the record and the live statistics into host-mapped
+// memory and closing with __threadfence_system would cost the TRAINING stream time every step for
+// the benefit of a sampler that looks twice a second.  The sampler instead fetches what it needs itself (k_mirror, on its own stream, tml_drain / tml_live).
 __global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* ring, u32 ring_slots,
                                                  CommitArgs a) {
   __shared__ __align__(16) u64 rec[16];
@@ -176,8 +175,8 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* r
 
   // ONE global round trip on the critical path: the phase accumulator and the 256-bin histogram
   // (8 bins per lane) are fetched together; the +1 of this step is applied in registers and
-  // written back without being waited for.  (r01: accumulator -> histogram RMW -> histogram
-  // re-read -> head read, four dependent round trips, 5.3-7.6 us.)
+  // written back without being waited for (instead of accumulator -> histogram RMW -> histogram
+  // re-read -> head read: four dependent round trips).
   u32* h = st->hist[warp];
   u32 c[8];
 #pragma unroll
@@ -422,8 +421,8 @@ __global__ void k_finalize(const double* __restrict__ partials, int nblk, int nc
 // Ring (128-B AoS records) -> WindowRow[] (64 B), step ids, row flags, bounds, sums.
 //   * tiles are fetched with cp.async (LDGSTS, 16 B per lane per copy, fully coalesced)
 //     into XOR-swizzled shared buffers, two per warp, so tile i+1 is in flight while
-//     tile i is converted -- the kernel was HBM-latency-bound before (ncu r01 v1:
-//     long-scoreboard stalls, 25 % occupancy, 1.97 TB/s);
+//     tile i is converted -- without it the kernel is HBM-latency-bound (long-scoreboard
+//     stalls);
 //   * the swizzle makes the per-lane 128-B record read bank-conflict-free;
 //   * rows leave through a swizzled staging buffer as coalesced 16-B stores;
 //   * integer side results live in registers for the whole persistent loop.
@@ -483,8 +482,7 @@ __device__ __forceinline__ void wr_issue_warp(uint4* buf, const uint4* __restric
 // 32-record tiles (cp.async double buffer -> XOR-swizzled smem -> registers -> swizzled
 // smem -> coalesced 16-B stores) and synchronises only with __syncwarp; neighbour step
 // ids come from warp shuffles (tile edges: two 8-B global reads).  No block barrier in
-// the loop (ncu r01 v2 showed barrier + wait stalls dominating once the loads were
-// asynchronous).
+// the loop (block barriers and waits dominate once the loads are asynchronous).
 __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
     tml_window_row* __restrict__ rows, u64* __restrict__ steps, u8* __restrict__ flags,
@@ -722,8 +720,8 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // ------------------------------------------------------------------ K3a+K4 fused (single rank)
 // With ONE rank the cross-rank median and worst of a step are the rank's own value, so the
 // per-step series can be written straight from the ring records: 128 B in, 128 B out per step, and
-// the 64-B WindowRows -- written by K3a only to be re-read by K4 (r01: 256 MB each way at
-// W = 4e6, 1481 MB of DRAM traffic for 1024 MB of payload) -- never exist.  Same warp-private
+// the 64-B WindowRows -- written by K3a only to be re-read by K4 (256 MB each way at
+// W = 4e6) -- never exist.  Same warp-private
 // cp.async pipeline as k_window_rows; lane = record, so each of the 16 series receives 32
 // consecutive doubles per tile: 256-B fully coalesced stores, no staging buffer.  Bounds, counters,
 // tree sums and maxima are produced exactly as in k_window_rows; the host accepts the series only
@@ -1180,7 +1178,7 @@ __global__ void __launch_bounds__(RD_THREADS, (R <= 2 ? 8 : R <= 4 ? 5 : 3)) k_w
   double* __restrict__ S = p.series;
   const bool do_time = (p.mask & TML_MASK_TIME) != 0u, do_mem = (p.mask & TML_MASK_MEM) != 0u;
   // Tiles are handed out by a ticket counter, not by a fixed stride: beside K3e only part of the
-  // grid is resident at first (the compose CTAs hold most of every SM for ~0.1 ms), and with a
+  // grid is resident at first (the compose CTAs hold most of every SM for a while), and with a
   // fixed stride the CTAs that get in late would still have their whole share to do -- the kernel
   // would last until the last of them is done.  With tickets whoever is resident pulls work, late
   // CTAs find none.  Thread 0 draws the next ticket at the top of a trip (its latency hides under
@@ -1478,7 +1476,7 @@ extern "C" int tml_set_error_(int code, const char* fmt, ...) {
 
 struct tml_ctx {
   int device = 0, rank = 0, world = 1;
-  int n_sms = 148;
+  int n_sms = 132;
   u32 ring_slots = 0, proc_slots = 0, mirror_slots = 0, pmirror_slots = 0;
   DevState* d_state = nullptr;
   tml_step_record* d_ring = nullptr;
@@ -1690,7 +1688,7 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   c->pmirror_slots = proc_slots < 16384u ? proc_slots : 16384u;
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  c->n_sms = sms > 0 ? sms : 148;
+  c->n_sms = sms > 0 ? sms : 132;
   CK(cudaMalloc(&c->d_state, sizeof(DevState)));
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   CK(cudaMalloc(&c->d_ring, (size_t)ring_slots * sizeof(tml_step_record)));
@@ -2577,7 +2575,7 @@ int tml_peer_close(tml_ctx* c, void* peer_ptr) {
 
 template <int R>
 static void launch_reduce(int grid, cudaStream_t s, const ReduceParams& p) {
-  constexpr int U = 1;  // measured on B200: U = 4 (R = 1) was 5-8 % slower than U = 1 at full occupancy
+  constexpr int U = 1;  // one row in flight per thread; occupancy hides the latency
   k_window_reduce<R, U><<<grid, RD_THREADS, 0, s>>>(p);
 }
 
@@ -2601,11 +2599,12 @@ int tml_win_reduce(tml_ctx* c, const tml_reduce_args* a, void* stream) {
   // A multiple of the SM count; the CTAs pull tiles from a ticket counter.  One rank: 8 CTAs/SM
   // (29 regs), HBM-bound.  Several ranks: NVLink-bound -- two CTAs of 256 threads x R loads already
   // keep several bandwidth-delay products in flight per SM -- and K3e runs beside it on the side
-  // stream, so the cap leaves the registers of one walk CTA free on every SM (r02 timeline on 8
-  // ranks before this: the persistent K4 CTAs held every SM, the walk started when K4 had finished).
+  // stream, so the cap leaves the registers of one walk CTA free on every SM (without it the
+  // persistent K4 CTAs hold every SM and the walk starts only when K4 has finished).
   u64 need = ((a->shard_hi - a->shard_lo) * 4 + RD_THREADS - 1) / RD_THREADS;
   static const int env_ctas = [] { const char* e = getenv("TML_K4_CTAS"); return e ? atoi(e) : 0; }();
   // registers decide what fits beside K3e's walk (16 K): R = 2: 6 x 8 K, R = 3..4: 4 x 12 K, R >= 5: 2 x 20 K
+  // (re-measured on the H100: DESIGN.md, "Launch shapes on the H100")
   const u64 per_sm = env_ctas > 0 ? (u64)env_ctas
                      : (a->n_ranks >= 5 ? 2ull : a->n_ranks >= 3 ? 4ull : a->n_ranks > 1 ? 6ull : 8ull);
   const u64 cap = (u64)c->n_sms * per_sm;

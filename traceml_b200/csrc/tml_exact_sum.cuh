@@ -278,10 +278,9 @@ __global__ void __launch_bounds__(1024) k_xs_bscan(XsWork w, int nblocks) {
 // derived ONCE and parked in shared memory, chain by chain.  Phase B: lane = (g, k), row quarter
 // g = lane >> 3 (64 consecutive rows), chain k = lane & 7 (k == 7 idles): a lane walks its 64 rows
 // serially for ITS chain -- one LDS, one branch-free FPU element map, one branch-free compose per
-// row -- and the four quarters of a chain are joined by two shuffle levels.  ncu history (W = 4e6,
-// 28 M element maps): v1 lane = 8 rows x 7 chains from global memory, 95 M warp instructions, 217 us;
-// v3 lane = (g, k) deriving all seven addends per lane, 209 M, 197 us; v5 shared-memory staging,
-// flag -> row loads one after the other, 100 us; this version 88 us (profiles/r02_summary.md).
+// row -- and the four quarters of a chain are joined by two shuffle levels.  Deriving the addends
+// once in shared memory, instead of every lane deriving all seven from global memory, cuts the
+// warp instructions several-fold.
 #define XS_CW 2                    // warps (chunks in flight) per compose CTA
 #define XS_SG 65                   // doubles per row quarter (64 + 1: quarters in different banks)
 #define XS_SK (4 * XS_SG + 8)      // doubles per chain
@@ -517,7 +516,7 @@ __device__ __forceinline__ void xs_walk_rows(const tml_window_row* rows, const X
 }
 
 // <= 64 registers: a walk CTA (16 K registers) must fit on an SM beside the resident K4 CTAs -- at
-// 128 it did not, and on 8 ranks the walk started only when K4 had finished (r02 timeline)
+// 128 it does not, and on 8 ranks the walk then starts only when K4 has finished
 __global__ void __launch_bounds__(256, 4) k_xs_walk(const XsSrc s, long long n, long long nchunks, long long ngroups,
                                                  XsWork w, int planned, double* __restrict__ out,
                                                  unsigned long long* __restrict__ stats /* [7]: rows added one by one */) {

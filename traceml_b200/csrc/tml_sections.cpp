@@ -3,7 +3,7 @@
 // The native counterpart of traceml_b200/sections.py (build_step_time / build_step_memory /
 // build_process + the O(R) public rollups): it consumes tml_reduce_run's output, runs the
 // three rule engines (tml_diag_*) and emits exactly the objects sections.py builds, so the
-// host does one JSON parse per final_summary() instead of ~0.3-0.5 ms of interpreter work.
+// host does one JSON parse per final_summary() instead of interpreter work per section.
 // Reference arithmetic followed (file:line under src/traceml/):
 //   RankStepSummary from sums        reporting/sections/step_time/model.py:108-120,270-281
 //   closest_rank_to_median           reporting/sections/step_time/model.py:77-105

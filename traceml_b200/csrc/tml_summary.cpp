@@ -6,8 +6,8 @@
 // the single-GPU parity tests use, and as the executable specification of this file.
 //
 // Why native: at R >= 2 the reduce is latency-bound (three small exchanges + five
-// kernel launches around two ~0.15 ms bandwidth kernels); the interpreter between the
-// stages cost more than the kernels (profiles/r01_summary.md).  Here an exchange is
+// kernel launches around two short bandwidth kernels); the interpreter between the
+// stages cost more than the kernels.  Here an exchange is
 // pinned-buffer H2D + ncclAllGather + D2H + one stream sync.
 //
 // NCCL is resolved at run time from the copy the process already has loaded (the one
@@ -122,9 +122,8 @@ struct RunWs {
 
 // ------------------------------------------------------------------ host mailbox
 // The small exchanges carry HOST data (bounds, counts, sums: a few hundred bytes per rank that
-// the stage before has just synchronised onto the host).  Round 1 sent them through the GPU and
-// back -- pinned H2D, ncclAllGather, D2H, stream sync: ~70 us each, three per reduce, a fifth of
-// the N = 8 step.  All ranks of this engine's scope live on one node, so they meet in a POSIX
+// the stage before has just synchronised onto the host).  Through the GPU and back each would be
+// a pinned H2D, ncclAllGather, D2H and stream sync, three per reduce.  All ranks of this engine's scope live on one node, so they meet in a POSIX
 // shared-memory segment instead: rank p writes its vector into slot p of a double-buffered
 // mailbox and publishes a sequence number with release semantics; everybody spins (acquire) until
 // all R slots carry the current number.  A few microseconds, no GPU work, no stream sync.
@@ -366,7 +365,7 @@ bool trend_layout(u64 n, u64 min_points, double warmup_frac, u64 lo[3], u64 hi[3
 
 // ------------------------------------------------------------------ the run
 constexpr u64 TML_FUSED_MIN_ROWS = 1u << 17;  // == TML_EXACT_SUM_MAX: below it the staged path gives reference-order sums
-constexpr u64 P2P_MIN_ROWS = 1000000;  // reduce.py: one-shot IPC mapping (44-65 ms at R = 8) pays above this
+constexpr u64 P2P_MIN_ROWS = 1000000;  // reduce.py: the one-shot IPC mapping pays above this
 
 struct KindState {
   tml_kind_result* res;
@@ -601,7 +600,6 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
   // ---- stage 1: local window + bounds; process aggregates and the speculative alignment ride along
   // K6 on the side stream: three tiny kernels that would otherwise sit in front of K3a;
   // tml_proc_reduce_collect waits on their own event
-  // (measured on one box, A/B: 0.523 vs 0.537 ms/step at N = 1)
   if (args->proc_rows) {
     CKC(cudaEventRecord(r.w->side_gate, r.s));
     CKC(cudaStreamWaitEvent(r.w->side, r.w->side_gate, 0));

@@ -1,6 +1,6 @@
 """Per-GPU engine handle: a thin object wrapper over the C-ABI context.
 
-One ``Engine`` per (process, GPU) -- the B200-native replacement for the
+One ``Engine`` per (process, GPU) -- the GPU-native replacement for the
 reference's per-rank ``TraceMLRuntime`` + queues + samplers
 (``src/traceml/runtime/runtime.py:33-193``).  Tests may create several engines
 on one GPU to play several ranks.

@@ -1,4 +1,4 @@
-"""Live tick: the B200 twin of the reference's ``StepCombinedComputer``.
+"""Live tick: the GPU twin of the reference's ``StepCombinedComputer``.
 
 The reference's live CLI / dashboard recompute, every render tick, the combined
 step-time view from SQLite (``src/traceml/renderers/step_time/compute.py:38-315``):

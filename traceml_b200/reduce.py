@@ -1,4 +1,4 @@
-"""Cross-rank window reduce: the B200-native final-summary path.
+"""Cross-rank window reduce: the GPU-native final-summary path.
 
 Replaces, for the Step-Time / Step-Memory / Process sections, the reference's
 TCP -> SQLite -> single-core Python chain
@@ -636,9 +636,9 @@ class WindowReducer:
 
     # ------------------------------------------------------------------ exchange
     # One-shot cost of the fused peer-load exchange is the CUDA-IPC mapping of R-1 peer
-    # allocations (measured on 8 x B200: 44-65 ms the first time, 0 once cached), so it
+    # allocations (tens of ms the first time, 0 once cached), so it
     # pays only for large or repeated windows.  Below this many aligned rows per rank the
-    # step-sharded NCCL all-to-all (2.7-7 ms one-shot at R = 8) is the default.
+    # step-sharded NCCL all-to-all is the default.
     P2P_MIN_ROWS = 1_000_000
 
     def _exchange_mode(self, n_common: Optional[int] = None) -> str:

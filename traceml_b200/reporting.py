@@ -37,7 +37,7 @@ _REF_TRIED = False
 def reference_available() -> bool:
     """Is the KEPT reporting layer (the reference package ``traceml``) importable?  Looked for on
     ``sys.path`` first, then under ``$TRACEML_REFERENCE_PATH`` and the in-tree install
-    ``<repo>/baseline/_ref`` (appended to ``sys.path``, never put in front of anything)."""
+    ``<repo>/oracle/_ref`` (appended to ``sys.path``, never put in front of anything)."""
     global _REF_TRIED
     try:
         import traceml.reporting.sections.step_time.builder  # noqa: F401
@@ -51,7 +51,7 @@ def reference_available() -> bool:
     import sys
 
     here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for cand in (os.environ.get("TRACEML_REFERENCE_PATH"), os.path.join(here, "baseline", "_ref")):
+    for cand in (os.environ.get("TRACEML_REFERENCE_PATH"), os.path.join(here, "oracle", "_ref")):
         if cand and os.path.isdir(os.path.join(cand, "traceml")) and cand not in sys.path:
             sys.path.append(cand)
             os.environ.setdefault("TRACEML_LOGS_DIR", os.path.join("/tmp", "traceml_ref_logs"))

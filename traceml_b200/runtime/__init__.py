@@ -63,7 +63,7 @@ def get_engine(device: Optional[int] = None):
     """The process's engine, created on first use on the current CUDA device.
 
     Raises if there is no CUDA device or the native library is missing: the
-    B200 engine has no CPU fallback.
+    GPU engine has no CPU fallback.
     """
     global _ENGINE, _ENGINE_DEVICE
     if _ENGINE is not None and (device is None or device == _ENGINE_DEVICE):
@@ -75,7 +75,7 @@ def get_engine(device: Optional[int] = None):
 
         if not torch.cuda.is_available():
             raise RuntimeError(
-                "traceml_b200: no CUDA device is visible. The B200-native telemetry engine "
+                "traceml_b200: no CUDA device is visible. The GPU-native telemetry engine "
                 "records through CUDA kernels and has no CPU fallback.")
         from ..engine import Engine
 

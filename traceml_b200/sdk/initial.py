@@ -71,7 +71,7 @@ def _require_engine() -> None:
 
     if not torch.cuda.is_available():
         raise RuntimeError(
-            "traceml_b200.init(): no CUDA device is visible. The B200-native engine records "
+            "traceml_b200.init(): no CUDA device is visible. The GPU-native engine records "
             "through CUDA kernels and has no CPU fallback; set TRACEML_DISABLED=1 to run untraced.")
 
 

@@ -1,6 +1,6 @@
 """Step-Time / Step-Memory / Process sections from the device-side reduce.
 
-The B200-native counterpart of
+The GPU-native counterpart of
 ``src/traceml/reporting/sections/{step_time,step_memory,process}/__init__.py``
 (``load -> to_diagnosis_input -> diagnose``): ``load`` is the cross-rank window
 reduce on the GPUs (``reduce.WindowReducer``), ``diagnose`` is the C++ rule

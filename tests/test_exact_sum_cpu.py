@@ -1,7 +1,8 @@
 """K3e arithmetic (csrc/tml_exact_sum.h) on the CPU: the reference's sequential ``s += x`` sums
 reproduced BIT FOR BIT from composed integer maps -- plan, chunk / group composition, verified
 application, 32-row tile fallback -- fuzzed against a plain sequential loop through the host
-emulation ``tml_xs_host_sum`` (the kernels share the header; GPU runs: test_gpu_parity_holes.py)."""
+emulation ``tml_xs_host_sum`` (the kernels share the header; GPU runs: test_gpu_exact_sums.py,
+test_gpu_parity_holes.py)."""
 import ctypes as C
 
 import numpy as np
@@ -38,10 +39,20 @@ def make(kind, n, rng):
         return rng.integers(0, 2 ** 20, n).astype(np.float64) * 2.0 ** -30 + 1.0
     if kind == 6:
         return np.concatenate([[1e18], rng.uniform(0, 1e3, n)])                 # one giant, then dust
+    if kind == 8:  # stalled just below 2^e: every chunk lies inside the plan's 1e-6 margin band
+        e = int(rng.integers(-10, 60))
+        return np.concatenate([[2.0 ** e * (1.0 - 3.0e-7)], rng.uniform(1, 2, n) * 2.0 ** (e - 45)])
+    if kind == 9:  # multiples of 1/64 near 2^40: past 2^47 every odd addend is an exact tie
+        return rng.integers(2 ** 45, 2 ** 47, n).astype(np.float64) * 2.0 ** -6
+    if kind == 10:  # giants inside 32-row tiles: the sum jumps several binades mid-tile
+        x = rng.uniform(1, 3, n)
+        for j, t in enumerate(sorted(rng.choice(max(1, n // 32), 3, replace=True))):
+            x[min(n - 1, 32 * int(t) + 13)] = 10.0 ** (3 * j + 4)
+        return x
     return rng.lognormal(2, 3, n)
 
 
-@pytest.mark.parametrize("kind", range(8))
+@pytest.mark.parametrize("kind", range(11))
 def test_bit_exact_against_sequential_loop(kind):
     rng = np.random.default_rng(100 + kind)
     for _ in range(40):

@@ -51,6 +51,7 @@ def _engines(records, ring=None):
     ("balanced", 2, 131_072, 131_072), ("balanced", 2, 131_073, 131_073), ("balanced", 4, 200_000, 200_000),
     ("balanced", 2, 1_000_000, 1_000_000), ("input_straggler", 4, 140_000, 135_000),
     ("balanced", 8, 300_001, 300_001), ("balanced", 2, 60_000, 10_000), ("balanced", 6, 150_000, 140_000),
+    ("ragged", 4, 150_000, 140_000), ("ragged", 2, 131_073, 131_073),   # offset + holey ranks: aligned K3e
 ])
 def test_large_window_vs_numpy_oracle(cuda, scenario, R, S, W):
     import replay

@@ -1,0 +1,192 @@
+"""Where the time of one single-rank summary build goes, next to what the HBM can do.
+
+Builds the workload ``bench.py --gpus 1`` times (same replay kinds and seed, ``Engine(ring_slots=W)``,
+steps loaded from pinned memory with ``load_steps_ptr``, 60 000 process samples) and prints one JSON
+line:
+
+  * ``build_ms``: CUDA events around K back-to-back ``SummaryEngine.build`` calls, per call;
+  * ``build_wall_ms``: host clock around one call (it ends in a stream synchronise), median;
+  * ``stage_ms``: the native driver's own stage times and ``k3a`` (the fused pass), medians;
+  * ``sections_json_ms``: the host time of ``tml_sections_json`` alone, and ``python_rest_ms``,
+    what is left of the wall time after the native driver and the JSON emitter;
+  * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved, the fused pass's
+    bytes at W = 4e6), CUDA events, median of 25 after warm-up; the fused pass against it;
+  * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
+
+``--alternate N`` runs N rounds of the chained sequence and the three-wait sequence
+(``TML_FUSED_CHAIN=0``), each arm in a child process of its own (the switch is read once per
+process), in ABBA order, and prints every child's line plus a comparison line.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PROC_ROWS = 60_000
+ARMS = {"chain": "1", "three_wait": "0"}
+
+
+def gpu_info(index: int = 0) -> dict:
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout
+        name, power, clk = [x.strip() for x in out.strip().split(",")]
+        return {"name": name, "power_limit": power, "clocks_max_sm": clk}
+    except Exception as exc:  # noqa: BLE001 -- reported, not hidden
+        return {"error": f"{type(exc).__name__}: {exc}"[:200]}
+
+
+def copy_ceiling(torch, nbytes: int = 512_000_000, reps: int = 25) -> dict:
+    src = torch.empty(nbytes, dtype=torch.uint8, device="cuda").random_(0, 255)
+    dst = torch.empty_like(src)
+    for _ in range(3):
+        dst.copy_(src)
+    torch.cuda.synchronize()
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
+    for a, b in ev:
+        a.record()
+        dst.copy_(src)
+        b.record()
+    torch.cuda.synchronize()
+    ms = statistics.median(a.elapsed_time(b) for a, b in ev)
+    del src, dst
+    torch.cuda.empty_cache()
+    return {"bytes_moved": 2 * nbytes, "ms": ms, "GBps": 2 * nbytes / (ms * 1e-3) / 1e9}
+
+
+def measure(steps: int, window: int, warmup: int) -> dict:
+    sys.path.insert(0, ROOT)
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import numpy as np
+    import torch
+
+    import replay
+    from traceml_b200 import sections
+    from traceml_b200.engine import Engine
+    from traceml_b200.reduce import LocalComm
+
+    assert torch.cuda.is_available(), "single_rank_build.py needs a CUDA device"
+    torch.cuda.set_device(0)
+    W = int(window)
+    recs = replay.make_step_replay("balanced", 1, W, seed=1, only_ranks=[0])[0]
+    procs = replay.make_proc_replay("normal", 1, PROC_ROWS, seed=1, only_ranks=[0])[0]
+    host = torch.empty(W * 128, dtype=torch.uint8).pin_memory()
+    host.numpy()[:] = recs.view(np.uint8).reshape(-1)
+    eng = Engine(device=0, rank=0, world=1, ring_slots=W, proc_slots=65_536)
+    eng.load_procs(procs)
+    stream = torch.cuda.current_stream()
+    eng.load_steps_ptr(host.data_ptr(), W, stream.cuda_stream)
+    torch.cuda.synchronize()
+    summ = sections.SummaryEngine([eng], LocalComm(), ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1)
+
+    for _ in range(warmup):
+        res = summ.build(W, PROC_ROWS)
+    torch.cuda.synchronize()
+    # (1) back-to-back builds between two events, as bench.py times them
+    l0 = eng.launch_count
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    stage: dict = {}
+    e0.record()
+    for _ in range(steps):
+        res = summ.build(W, PROC_ROWS)
+        for k, v in res["reduce"].timings_ms.items():
+            stage.setdefault(k, []).append(v)
+    e1.record()
+    torch.cuda.synchronize()
+    build_ms = e0.elapsed_time(e1) / steps
+    launches = (eng.launch_count - l0) / steps
+    fused = bool(getattr(res["reduce"], "fused_rows", False))
+    # (2) host clock around single builds, and the JSON emitter alone on a fresh result
+    wall = []
+    for _ in range(steps):
+        t0 = time.perf_counter()
+        summ.build(W, PROC_ROWS)
+        wall.append((time.perf_counter() - t0) * 1e3)
+    o = summ.reducer.run_native(W, PROC_ROWS)
+    sj = []
+    for _ in range(steps):
+        t0 = time.perf_counter()
+        eng.sections_json(o, replay.PROC_RAM_TOTAL_BYTES, 1, W, PROC_ROWS)
+        sj.append((time.perf_counter() - t0) * 1e3)
+    eng.close()
+    del host, recs
+    med = {k: statistics.median(v) for k, v in stage.items() if not k.startswith("host_")}
+    wall_ms, sj_ms = statistics.median(wall), statistics.median(sj)
+    ceil = copy_ceiling(torch)
+    fused_bytes = W * 256.0
+    k3a = med.get("k3a") or 0.0
+    fused_gbps = fused_bytes / (k3a * 1e-3) / 1e9 if k3a else None
+    return {
+        "chain_env": os.environ.get("TML_FUSED_CHAIN"), "window": W, "steps": steps, "fused_rows": fused,
+        "build_ms": build_ms, "build_wall_ms": wall_ms, "launches_per_build": launches,
+        "stage_ms": med, "sections_json_ms": sj_ms,
+        "python_rest_ms": wall_ms - med.get("total", 0.0) - sj_ms,
+        "native_minus_fused_ms": med.get("total", 0.0) - k3a,
+        "copy_ceiling": ceil,
+        "fused_pass": {"bytes": fused_bytes, "ms": k3a, "GBps": fused_gbps,
+                       "of_copy_ceiling": (fused_gbps / ceil["GBps"]) if fused_gbps else None,
+                       "of_datasheet_3350": (fused_gbps / 3350.0) if fused_gbps else None},
+        "gpu": gpu_info(0),
+    }
+
+
+def alternate(args) -> None:
+    runs = {a: [] for a in ARMS}
+    order = list(ARMS)
+    for rnd in range(args.alternate):
+        for arm in (order if rnd % 2 == 0 else order[::-1]):
+            env = dict(os.environ, TML_FUSED_CHAIN=ARMS[arm])
+            cmd = [sys.executable, os.path.abspath(__file__), "--steps", str(args.steps),
+                   "--window", str(args.window), "--warmup", str(args.warmup)]
+            p = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=1800)
+            if p.returncode != 0:
+                sys.stderr.write(p.stderr[-4000:])
+                raise SystemExit(f"{arm} arm failed in round {rnd} (exit {p.returncode})")
+            line = json.loads(p.stdout.strip().splitlines()[-1])
+            line["arm"], line["round"] = arm, rnd
+            runs[arm].append(line)
+            print(json.dumps(line), flush=True)
+
+    def stats(xs):
+        return {"median": statistics.median(xs), "min": min(xs), "max": max(xs), "spread": max(xs) - min(xs),
+                "all": xs}
+
+    summary = {"compare": {}, "gpu": runs["chain"][0]["gpu"]}
+    for key in ("build_ms", "build_wall_ms"):
+        per = {a: stats([r[key] for r in runs[a]]) for a in ARMS}
+        d = per["three_wait"]["median"] - per["chain"]["median"]
+        summary["compare"][key] = dict(per, saving_ms=d, saving_frac=d / per["three_wait"]["median"],
+                                       beyond_spread=d > max(per["chain"]["spread"], per["three_wait"]["spread"]))
+    summary["stage_ms"] = {a: {k: statistics.median(r["stage_ms"][k] for r in runs[a]) for k in runs[a][0]["stage_ms"]}
+                           for a in ARMS}
+    summary["launches_per_build"] = {a: runs[a][0]["launches_per_build"] for a in ARMS}
+    summary["copy_ceiling_GBps"] = statistics.median(r["copy_ceiling"]["GBps"] for a in ARMS for r in runs[a])
+    summary["fused_of_copy_ceiling"] = {a: statistics.median(r["fused_pass"]["of_copy_ceiling"] for r in runs[a])
+                                        for a in ARMS}
+    print(json.dumps(summary), flush=True)
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--steps", type=int, default=1000, help="K: builds per timed loop")
+    ap.add_argument("--window", type=int, default=4_000_000, help="W: step records")
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--alternate", type=int, default=0, metavar="N",
+                    help="N rounds of both sequences, each arm in a child process")
+    args = ap.parse_args()
+    if args.steps < 1 or args.window < 1:
+        ap.error("--steps and --window must be at least 1")
+    if args.alternate > 0:
+        alternate(args)
+    else:
+        print(json.dumps(measure(args.steps, args.window, args.warmup)), flush=True)
+
+
+if __name__ == "__main__":
+    main()

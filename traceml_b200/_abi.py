@@ -293,7 +293,8 @@ def sections_json(run_out, ram_total: float, gpu_count: int, window: int, proc_r
         _SEC_BUF = C.create_string_buffer(len(_SEC_BUF) * 8)
         return sections_json(run_out, ram_total, gpu_count, window, proc_rows)
     check(rc, "tml_sections_json")
-    return Sections(_SEC_BUF.value)
+    # string_at: strlen + one copy; .value walks the 256 KB buffer byte by byte in Python's C loop
+    return Sections(C.string_at(_SEC_BUF))
 
 
 class Sections:

@@ -108,6 +108,25 @@ struct WinAcc {  // integer side results of k_window_rows (atomics; order-indepe
   u64 msum[2]; // exact sum of peak_alloc / peak_resv over the window rows (byte counts are integers;
                // the reference's mean is CPython's compensated sum = the correctly rounded exact sum)
 };
+#define WINACC_WORDS 15
+static_assert(sizeof(WinAcc) == WINACC_WORDS * sizeof(u64), "WinAcc is re-armed word by word");
+
+// The chained single-rank build (tml_win_fused_chain_launch_ / _finish_): everything the host
+// reads back, packed so that ONE device-to-host copy fetches it.  Bands and tails have slots of
+// their own: nothing here is shared with the staged path's d_final / d_partials.
+struct ChainOut {
+  double fin[16];       // k_finalize's columns of k_window_fused: 7 tree sums, 2 byte sums, 2 maxima
+  WinAcc acc;           // the pass's integer side results
+  double band_sum[48];  // k_bands: [series][band]
+  u64 band_cnt[48];
+  double tail[32];      // k_bands: [series][first, last]
+};
+// The chained pass's own accumulator and completion ticket, armed at context creation and
+// re-armed by the pass's last CTA, so no host copy sits in front of the kernel.
+struct ChainState {
+  WinAcc acc;
+  unsigned int ticket;
+};
 
 // ------------------------------------------------------------------ device helpers
 
@@ -399,15 +418,24 @@ __device__ __forceinline__ void block_sum(double (&v)[NV], double* out) {
 // out[c] = reduce over b of partials[b * ncols + c]; op per column: 0 sum, 1 max.
 // One warp per column: lane l folds blocks l, l+32, ... in order, then a fixed
 // shuffle tree -- deterministic for a given grid, and ~nblk/32 dependent loads deep.
-__global__ void k_finalize(const double* __restrict__ partials, int nblk, int ncols, u32 max_mask,
-                           double* __restrict__ out) {
-  const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (c >= ncols) return;
+// Shared by k_finalize and the last CTA of k_window_fused, so both give the same bits.  The
+// partials come from other CTAs of a running grid in the latter: L2 loads, never the nc path.
+__device__ __forceinline__ void finalize_column(const double* partials, int nblk, int ncols, u32 max_mask,
+                                                int c, int lane, double* out) {
   const bool is_max = (max_mask >> c) & 1u;
   double x = is_max ? -INFINITY : 0.0;
-  for (int b = lane; b < nblk; b += 32) {
-    double p = partials[(size_t)b * ncols + c];
-    x = is_max ? fmax(x, p) : (x + p);
+  // eight loads in flight before they are folded, still in block order: one L2 round trip per
+  // eight blocks instead of one per block (it is the tail of the chained pass)
+  for (int b0 = lane; b0 < nblk; b0 += 32 * 8) {
+    double p[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int b = b0 + 32 * k;
+      p[k] = b < nblk ? __ldcg(partials + (size_t)b * ncols + c) : 0.0;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k)
+      if (b0 + 32 * k < nblk) x = is_max ? fmax(x, p[k]) : (x + p[k]);
   }
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) {
@@ -415,6 +443,13 @@ __global__ void k_finalize(const double* __restrict__ partials, int nblk, int nc
     x = is_max ? fmax(x, y) : (x + y);
   }
   if (lane == 0) out[c] = x;
+}
+
+__global__ void k_finalize(const double* __restrict__ partials, int nblk, int ncols, u32 max_mask,
+                           double* __restrict__ out) {
+  const int c = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (c >= ncols) return;
+  finalize_column(partials, nblk, ncols, max_mask, c, lane, out);
 }
 
 // ------------------------------------------------------------------ K3a: window rows
@@ -727,12 +762,17 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // tree sums and maxima are produced exactly as in k_window_rows; the host accepts the series only
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
 // otherwise it falls back to the staged path.
+// CHAINED (the chained build): the CTAs count themselves out on the ticket and the last
+// one folds the partials with finalize_column and hands the accumulator over to chain_out, then
+// re-arms both -- no k_finalize launch behind the pass and no accumulator copy in front of it.
 #define WF_WARP_U4 (2 * 32 * 8)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
 
+template <bool CHAINED>
 __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
     const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
-    double* __restrict__ series, u64 n_ser, WinAcc* acc, double* partials) {
+    double* __restrict__ series, u64 n_ser, WinAcc* acc, double* partials, unsigned int* ticket,
+    ChainOut* chain_out) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint4* w_in0 = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
@@ -887,6 +927,24 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
       double x = -INFINITY;
       for (int w = 0; w < WR_THREADS / 32; ++w) x = fmax(x, s_mx[w][tid]);
       partials[(size_t)blockIdx.x * 11 + 9 + tid] = x;
+    }
+  }
+  if (CHAINED) {  // chained build: the last CTA to finish does k_finalize's work, in its order
+    __threadfence();  // this CTA's partials and accumulator atomics, before its ticket
+    int last = 0;
+    if (tid == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    // the vote rides the barrier: a 16-B __shared__ flag made the whole pass ~30 us slower on an
+    // H100 80GB HBM3 (400 W), measured; static shared memory stays at 704 B, as unchained
+    if (__syncthreads_or(last)) {
+      __threadfence();
+      for (int col = warp; col < 11; col += WR_WARPS)
+        finalize_column(partials, (int)gridDim.x, 11, (1u << 9) | (1u << 10), col, lane, chain_out->fin);
+      if (tid < WINACC_WORDS) {  // hand the accumulator over and re-arm it for the next pass
+        u64* a = reinterpret_cast<u64*>(acc);
+        reinterpret_cast<u64*>(&chain_out->acc)[tid] = __ldcg(a + tid);
+        a[tid] = tid < 2 ? ~0ull : 0ull;  // lo[0], lo[1] start at ~0, every other word at 0
+        if (tid == 0) *ticket = 0u;
+      }
     }
   }
 }
@@ -1547,8 +1605,12 @@ struct tml_ctx {
   cudaEvent_t xs_gate = nullptr, xs_done = nullptr;
   bool xs_defer = false, xs_pending = false;
   double* d_partials = nullptr;  // max(grid) * 16 doubles
-  double* d_final = nullptr;     // 64 doubles
+  double* d_final = nullptr;     // 64 doubles, then d_winacc, d_chain_out, d_chain_state
   u64* d_bandcnt = nullptr;
+  ChainOut* d_chain_out = nullptr;      // the chained single-rank build's results (one copy), in d_final's allocation
+  ChainState* d_chain_state = nullptr;  // ... and its pass's own accumulator + ticket (always armed)
+  u64 chain_n = 0, chain_window = 0;    // the chained pass in flight: retained rows, window
+  bool chain_pending = false;
   void* h_stage = nullptr;       // pinned 4 KB result staging
   std::unordered_map<std::string, void*> peers;
   void* comb[2] = {nullptr, nullptr};  // live step-combined workspaces, per kind (tml_combined.cuh)
@@ -1706,11 +1768,22 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   CK(cudaMalloc(&c->d_xs_out, 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_xs_stats, 8 * sizeof(u64)));
   CK(cudaMalloc(&c->d_partials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
-  CK(cudaMalloc(&c->d_final, 64 * sizeof(double) + sizeof(WinAcc)));
-  c->d_winacc = reinterpret_cast<WinAcc*>(c->d_final + 64);  // one D2H copy fetches both
+  // d_final | K3a's WinAcc (one D2H copy fetches both) | the chained build's ChainOut, ChainState
+  const size_t fin_bytes = 64 * sizeof(double) + sizeof(WinAcc);
+  static_assert((64 * sizeof(double) + sizeof(WinAcc)) % 8 == 0 && sizeof(ChainOut) % 8 == 0, "8-B aligned");
+  CK(cudaMalloc(&c->d_final, fin_bytes + sizeof(ChainOut) + sizeof(ChainState)));
+  c->d_winacc = reinterpret_cast<WinAcc*>(c->d_final + 64);
+  c->d_chain_out = reinterpret_cast<ChainOut*>((char*)c->d_final + fin_bytes);
+  c->d_chain_state = reinterpret_cast<ChainState*>((char*)c->d_final + fin_bytes + sizeof(ChainOut));
   CK(cudaMalloc(&c->d_ppartials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_pfinal, 32 * sizeof(double)));
   CK(cudaMalloc(&c->d_bandcnt, 64 * sizeof(u64)));
+  {  // armed once here; every chained pass re-arms it on its way out
+    ChainState armed;
+    memset(&armed, 0, sizeof(armed));
+    armed.acc.lo[0] = armed.acc.lo[1] = ~0ull;
+    CK(cudaMemcpy(c->d_chain_state, &armed, sizeof(armed), cudaMemcpyHostToDevice));
+  }
   CK(cudaHostAlloc(&c->h_stage, 4096, cudaHostAllocDefault));
   *out = c;
   return TML_OK;
@@ -2228,53 +2301,54 @@ int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_
   return TML_OK;
 }
 
-// Single-rank bulk path: ring -> per-step series in ONE pass (k_window_fused).  *ok = 1: the
-// window is dense and `series` ([16][n_window], device) plus `aligned` hold the result; 0: the
-// caller runs the staged path (tml_win_prepare ...).  Leaves no WindowRows behind.
-int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml_win_info* out,
-                  tml_align_info* aligned, uint32_t* ok) {
-  if (!c || !out || !aligned || !ok || !series || window == 0) return TML_ERR_ARG;
-  cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaSetDevice(c->device));
-  memset(out, 0, sizeof(*out));
-  memset(aligned, 0, sizeof(*aligned));
-  *ok = 0;
+// k_window_fused on stream s over the retained ring's last `window` rows (n > 0), between ev0 and
+// ev1.  chained: the pass finalises itself into d_chain_out from its own, always armed,
+// accumulator; otherwise d_winacc is armed by a copy in front and k_finalize runs behind.
+static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, bool chained) {
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
   const u64 t_start = n > window ? n - window : 0;
   const u64 n_win = n - t_start;
-  c->win_ready = false;
-  out->n_retained = n;
-  out->monotone = 1;
-  if (n == 0) return TML_OK;
   if (c->xs_pending) { CK(cudaStreamWaitEvent(s, c->xs_done, 0)); c->xs_pending = false; }
-  WinAcc init;
-  memset(&init, 0, sizeof(init));
-  init.lo[0] = init.lo[1] = ~0ull;
-  CK(cudaMemcpyAsync(c->d_winacc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+  if (!chained) {
+    WinAcc init;
+    memset(&init, 0, sizeof(init));
+    init.lo[0] = init.lo[1] = ~0ull;
+    CK(cudaMemcpyAsync(c->d_winacc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+  }
   static bool wf_attr = false;
   if (!wf_attr) {
-    CK(cudaFuncSetAttribute(k_window_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
     wf_attr = true;
   }
   int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
   if (grid > c->n_sms * 2) grid = c->n_sms * 2;
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   CK(cudaEventRecord(c->ev0, s));
-  k_window_fused<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
-                                                          c->d_winacc, c->d_partials);
+  if (chained)
+    k_window_fused<true><<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
+                                                            &c->d_chain_state->acc, c->d_partials,
+                                                            &c->d_chain_state->ticket, c->d_chain_out);
+  else
+    k_window_fused<false><<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
+                                                            c->d_winacc, c->d_partials, nullptr, nullptr);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
-  k_finalize<<<1, 32 * 11, 0, s>>>(c->d_partials, grid, 11, (1u << 9) | (1u << 10), c->d_final + 32);
-  CK(cudaPeekAtLastError());
-  c->launches += 2;
-  char* st = (char*)c->h_stage;
-  CK(cudaMemcpyAsync(st + 1024, c->d_final, 64 * sizeof(double) + sizeof(WinAcc), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  WinAcc acc;
-  memcpy(&acc, st + 1024 + 64 * sizeof(double), sizeof(acc));
-  double f[11];
-  memcpy(f, st + 1024 + 32 * sizeof(double), sizeof(f));
+  c->launches += 1;
+  if (!chained) {
+    k_finalize<<<1, 32 * 11, 0, s>>>(c->d_partials, grid, 11, (1u << 9) | (1u << 10), c->d_final + 32);
+    CK(cudaPeekAtLastError());
+    c->launches += 1;
+  }
+  return TML_OK;
+}
+
+// What tml_win_fused reports once the pass has finished: `acc` its accumulator, f[0..11) its
+// finalised columns.  *ok = 1 and `aligned` when the window is dense.
+static int fused_result(tml_ctx* c, u64 n, u64 window, const WinAcc& acc, const double* f, tml_win_info* out,
+                        tml_align_info* aligned, uint32_t* ok) {
+  const u64 n_win = n > window ? window : n;
   memcpy(out->t_sums, f, 7 * sizeof(double));
   out->latest_step = acc.latest_step;
   out->monotone = acc.violations == 0 ? 1u : 0u;
@@ -2309,6 +2383,90 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
     aligned->m_sums[2] = f[9]; aligned->m_sums[3] = f[10];
   }
   return TML_OK;
+}
+
+// Single-rank bulk path: ring -> per-step series in ONE pass (k_window_fused).  *ok = 1: the
+// window is dense and `series` ([16][n_window], device) plus `aligned` hold the result; 0: the
+// caller runs the staged path (tml_win_prepare ...).  Leaves no WindowRows behind.
+int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml_win_info* out,
+                  tml_align_info* aligned, uint32_t* ok) {
+  if (!c || !out || !aligned || !ok || !series || window == 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  memset(out, 0, sizeof(*out));
+  memset(aligned, 0, sizeof(*aligned));
+  *ok = 0;
+  const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
+  c->win_ready = false;
+  out->n_retained = n;
+  out->monotone = 1;
+  if (n == 0) return TML_OK;
+  int rc = fused_pass(c, window, series, s, false);
+  if (rc != TML_OK) return rc;
+  // d_final[32..43) tree sums + maxima | d_final[64..] WinAcc: one copy
+  char* st = (char*)c->h_stage;
+  CK(cudaMemcpyAsync(st + 1024, c->d_final, 64 * sizeof(double) + sizeof(WinAcc), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  WinAcc acc;
+  memcpy(&acc, st + 1024 + 64 * sizeof(double), sizeof(acc));
+  double f[11];
+  memcpy(f, st + 1024 + 32 * sizeof(double), sizeof(f));
+  return fused_result(c, n, window, acc, f, out, aligned, ok);
+}
+
+// The same pass as one device submission with the band sums chained behind it (tml_internal.h).
+int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
+                                void* stream) {
+  if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
+  if (n == 0) return set_err(TML_ERR_STATE, "chained window pass over an empty ring");
+  c->win_ready = false;
+  c->chain_n = n;
+  c->chain_window = window;
+  c->chain_pending = false;
+  int rc = fused_pass(c, window, series, s, true);
+  if (rc != TML_OK) return rc;
+  // k_bands exactly as tml_win_bands launches it, into the packed block's own slots
+  BandParams p;
+  p.series = series; p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
+  memcpy(p.lo, bands->band_lo, sizeof(p.lo));
+  memcpy(p.hi, bands->band_hi, sizeof(p.hi));
+  memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
+  char* co = (char*)c->d_chain_out;
+  k_bands<<<dim3(16, 4), 256, 0, s>>>(p, (double*)(co + offsetof(ChainOut, band_sum)),
+                                      (u64*)(co + offsetof(ChainOut, band_cnt)), (double*)(co + offsetof(ChainOut, tail)));
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  c->chain_pending = true;
+  return TML_OK;
+}
+
+int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
+                                tml_band_out* band_out, uint32_t* ok) {
+  if (!c || !out || !aligned || !band_out || !ok) return TML_ERR_ARG;
+  if (!c->chain_pending) return set_err(TML_ERR_STATE, "tml_win_fused_chain_finish_ without a launch");
+  c->chain_pending = false;
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  memset(out, 0, sizeof(*out));
+  memset(aligned, 0, sizeof(*aligned));
+  *ok = 0;
+  out->n_retained = c->chain_n;
+  out->monotone = 1;
+  // the process aggregates (side stream) land in their own staging slot before the one wait
+  if (c->proc_pending && c->proc_pending_n > 0) CK(cudaStreamWaitEvent(s, c->ev_proc, 0));
+  char* st = (char*)c->h_stage + 1024;
+  static_assert(1024 + sizeof(ChainOut) <= 3072, "the packed block must stay clear of the process slot");
+  CK(cudaMemcpyAsync(st, c->d_chain_out, sizeof(ChainOut), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  ChainOut r;
+  memcpy(&r, st, sizeof(r));
+  memcpy(band_out->sum, r.band_sum, sizeof(band_out->sum));
+  memcpy(band_out->cnt, r.band_cnt, sizeof(band_out->cnt));
+  for (int k = 0; k < 16; ++k) { band_out->tail_first[k] = r.tail[2 * k]; band_out->tail_last[k] = r.tail[2 * k + 1]; }
+  return fused_result(c, c->chain_n, c->chain_window, r.acc, r.fin, out, aligned, ok);
 }
 
 int tml_win_set_defer(tml_ctx* c, int on) {

@@ -13,6 +13,16 @@ int tml_set_error_(int code, const char* fmt, ...);
 void** tml_run_ws_slot_(tml_ctx* ctx);
 void tml_run_ws_free_(void* ws);
 
+// The dense single-rank build as one device submission (tml_reduce_run's world == 1 branch).
+// launch: k_window_fused, which finalises itself, then k_bands over `series` with `bands` (the
+// host knows n_window, so the band layout, before the pass).  finish: joins the process
+// aggregates launched in between (their event), one device-to-host copy, one stream wait; then
+// reports what tml_win_fused and tml_win_bands would.  *ok = 0: not dense, drop the bands.
+int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
+                                void* stream);
+int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
+                                tml_band_out* band_out, uint32_t* ok);
+
 #ifdef __cplusplus
 }
 #endif

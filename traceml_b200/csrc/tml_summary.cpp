@@ -365,6 +365,14 @@ bool trend_layout(u64 n, u64 min_points, double warmup_frac, u64 lo[3], u64 hi[3
 
 // ------------------------------------------------------------------ the run
 constexpr u64 TML_FUSED_MIN_ROWS = 1u << 17;  // == TML_EXACT_SUM_MAX: below it the staged path gives reference-order sums
+
+// TML_FUSED_CHAIN=0: the single-rank bulk build as three host waits (pass + k_finalize, process
+// aggregates, bands) instead of one chained submission.  An A/B switch, never needed for
+// correctness; read once per process.
+bool fused_chain_enabled() {
+  static const bool on = [] { const char* e = getenv("TML_FUSED_CHAIN"); return !e || e[0] != '0'; }();
+  return on;
+}
 constexpr u64 P2P_MIN_ROWS = 1000000;  // reduce.py: the one-shot IPC mapping pays above this
 
 struct KindState {
@@ -523,21 +531,35 @@ int reduce_pass(Run& r, u32 kind, u32 mask, u32 mode, KindState* ks, int series_
 // `extra` (n_extra doubles per rank, may be 0) rides in the band exchange: the deferred
 // reference-order sums of K3e, so that they cost no exchange of their own.  *extra_done tells the
 // caller whether the exchange happened (no aligned window -> no band exchange).
+// what k_bands is asked for over a series of n columns, of which [shard_lo, shard_hi) are here
+void band_args(u64 n, u64 shard_lo, u64 shard_hi, tml_band_args* a) {
+  memset(a, 0, sizeof(*a));
+  a->n_common = n; a->shard_lo = shard_lo; a->shard_hi = shard_hi;
+  u64 lo[3], hi[3];
+  if (trend_layout(n, 200, 0.10, lo, hi)) for (int b = 0; b < 3; ++b) { a->band_lo[0][b] = lo[b]; a->band_hi[0][b] = hi[b]; }
+  if (trend_layout(n, 50, 0.0, lo, hi)) for (int b = 0; b < 3; ++b) { a->band_lo[1][b] = lo[b]; a->band_hi[1][b] = hi[b]; }
+  a->tail_first[0] = 0;
+  a->tail_first[1] = n - (n < 1000 ? n : 1000);
+}
+
+int bands_collect(Run& r, tml_kind_result* res, const tml_band_out& bo, const double* extra, int n_extra,
+                  double* extra_all, bool* extra_done);
+
 int bands(Run& r, tml_kind_result* res, const double* extra = nullptr, int n_extra = 0,
           double* extra_all = nullptr, bool* extra_done = nullptr) {
   const u64 n = res->n_common;
   if (extra_done) *extra_done = false;
   if (n == 0 || !res->series) return TML_OK;
   tml_band_args a;
-  memset(&a, 0, sizeof(a));
-  a.n_common = n; a.shard_lo = res->shard_lo; a.shard_hi = res->shard_hi;
-  u64 lo[3], hi[3];
-  if (trend_layout(n, 200, 0.10, lo, hi)) for (int b = 0; b < 3; ++b) { a.band_lo[0][b] = lo[b]; a.band_hi[0][b] = hi[b]; }
-  if (trend_layout(n, 50, 0.0, lo, hi)) for (int b = 0; b < 3; ++b) { a.band_lo[1][b] = lo[b]; a.band_hi[1][b] = hi[b]; }
-  a.tail_first[0] = 0;
-  a.tail_first[1] = n - (n < 1000 ? n : 1000);
+  band_args(n, res->shard_lo, res->shard_hi, &a);
   tml_band_out bo;
   CKT(tml_win_bands(r.c, res->series, &a, r.s, &bo));
+  return bands_collect(r, res, bo, extra, n_extra, extra_all, extra_done);
+}
+
+// the band exchange and its rank-order sums, from this rank's k_bands results
+int bands_collect(Run& r, tml_kind_result* res, const tml_band_out& bo, const double* extra, int n_extra,
+                  double* extra_all, bool* extra_done) {
   double vec[128 + 16];
   for (int s = 0; s < 16; ++s)
     for (int b = 0; b < 3; ++b) { vec[s * 3 + b] = bo.sum[s][b]; vec[48 + s * 3 + b] = (double)bo.cnt[s][b]; }
@@ -599,57 +621,72 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
 
   // ---- stage 1: local window + bounds; process aggregates and the speculative alignment ride along
   // K6 on the side stream: three tiny kernels that would otherwise sit in front of K3a;
-  // tml_proc_reduce_collect waits on their own event
+  // tml_proc_reduce_collect waits on their own event.  The side stream waits for what r.s held at
+  // entry (ring loads), not for the window pass, which the chained build enqueues first.
+  u64 n_win = 0;
+  CKT(tml_win_peek(c, window, nullptr, &n_win));
+  const bool bulk = world == 1 && n_win > (u64)TML_FUSED_MIN_ROWS;
+  const bool chain = bulk && fused_chain_enabled();
+  if (args->proc_rows) CKC(cudaEventRecord(r.w->side_gate, r.s));
+  if (chain) {
+    // the dense series has n_win columns, so the band layout is known before the pass
+    CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
+    tml_band_args ba;
+    band_args(n_win, 0, n_win, &ba);
+    CKT(tml_win_fused_chain_launch_(c, window, r.w->d_series[0], &ba, r.s));
+  }
   if (args->proc_rows) {
-    CKC(cudaEventRecord(r.w->side_gate, r.s));
     CKC(cudaStreamWaitEvent(r.w->side, r.w->side_gate, 0));
     CKT(tml_proc_reduce_launch(c, args->proc_rows, r.w->side));
   }
   // ---- single rank, bulk window: ring -> series in ONE pass (k_window_fused); the WindowRows
   // that K3a would write for K4 to re-read never exist.  Falls through to the staged path when the
-  // window is not dense (re-flushed step ids, rows without memory, ...).
-  if (world == 1) {
-    u64 n_ret = 0, n_win = 0;
-    CKT(tml_win_peek(c, window, &n_ret, &n_win));
-    if (n_win > (u64)TML_FUSED_MIN_ROWS) {
+  // window is not dense (re-flushed step ids, rows without memory, ...).  Chained (the default):
+  // pass, bands and process aggregates are one device submission with one copy and one wait.
+  if (bulk) {
+    tml_win_info finfo;
+    tml_align_info fal;
+    tml_band_out cbo;
+    uint32_t ok = 0;
+    if (chain) {
+      CKT(tml_win_fused_chain_finish_(c, r.s, &finfo, &fal, &cbo, &ok));
+    } else {
       CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
-      tml_win_info finfo;
-      tml_align_info fal;
-      uint32_t ok = 0;
       CKT(tml_win_fused(c, window, r.w->d_series[0], r.s, &finfo, &fal, &ok));
-      if (ok) {
-        tml_proc_agg pagg0;
-        memset(&pagg0, 0, sizeof(pagg0));
-        if (args->proc_rows) CKT(tml_proc_reduce_collect(c, &pagg0));
-        out->n_ranks = 1;
-        out->infos[0] = finfo;
-        out->procs[0] = pagg0;
-        for (tml_kind_result* res : {&out->time, &out->mem}) {
-          res->observed = 1; res->n_used = 1; res->used[0] = 0;
-          res->n_common = fal.n_common; res->start_step = fal.start_step; res->end_step = fal.end_step;
-          res->n_rows[0] = fal.n_rows;
-          memcpy(res->t_sums[0], fal.t_sums, sizeof(fal.t_sums));
-          memcpy(res->m_sums[0], fal.m_sums, sizeof(fal.m_sums));
-          res->series = r.w->d_series[0];
-          res->shard_lo = 0; res->shard_hi = fal.n_common;
-        }
-        out->exchange_used = TML_XCHG_LOCAL;
-        out->fused_pass = 2;  // 2: K3a and K4 fused as well (no WindowRows)
-        const double tf = now_ms();
-        CKT(bands(r, &out->time));
-        memcpy(out->mem.band_sum, out->time.band_sum, sizeof(out->time.band_sum));
-        memcpy(out->mem.band_cnt, out->time.band_cnt, sizeof(out->time.band_cnt));
-        memcpy(out->mem.tail_first, out->time.tail_first, sizeof(out->time.tail_first));
-        memcpy(out->mem.tail_last, out->time.tail_last, sizeof(out->time.tail_last));
-        out->mem.has_bands = out->time.has_bands;
-        const double te = now_ms();
-        out->n_exchanges = r.n_exchanges;
-        out->k3a_ms = finfo.kernel_ms;
-        out->k4_ms = 0.0;
-        out->stage_ms[0] = tf - t0; out->stage_ms[1] = 0.0; out->stage_ms[2] = 0.0;
-        out->stage_ms[3] = te - tf; out->stage_ms[4] = te - t0;
-        return TML_OK;
+    }
+    if (ok) {
+      tml_proc_agg pagg0;
+      memset(&pagg0, 0, sizeof(pagg0));
+      if (args->proc_rows) CKT(tml_proc_reduce_collect(c, &pagg0));
+      out->n_ranks = 1;
+      out->infos[0] = finfo;
+      out->procs[0] = pagg0;
+      for (tml_kind_result* res : {&out->time, &out->mem}) {
+        res->observed = 1; res->n_used = 1; res->used[0] = 0;
+        res->n_common = fal.n_common; res->start_step = fal.start_step; res->end_step = fal.end_step;
+        res->n_rows[0] = fal.n_rows;
+        memcpy(res->t_sums[0], fal.t_sums, sizeof(fal.t_sums));
+        memcpy(res->m_sums[0], fal.m_sums, sizeof(fal.m_sums));
+        res->series = r.w->d_series[0];
+        res->shard_lo = 0; res->shard_hi = fal.n_common;
       }
+      out->exchange_used = TML_XCHG_LOCAL;
+      out->fused_pass = 2;  // 2: K3a and K4 fused as well (no WindowRows)
+      const double tf = now_ms();
+      if (chain) CKT(bands_collect(r, &out->time, cbo, nullptr, 0, nullptr, nullptr));
+      else CKT(bands(r, &out->time));
+      memcpy(out->mem.band_sum, out->time.band_sum, sizeof(out->time.band_sum));
+      memcpy(out->mem.band_cnt, out->time.band_cnt, sizeof(out->time.band_cnt));
+      memcpy(out->mem.tail_first, out->time.tail_first, sizeof(out->time.tail_first));
+      memcpy(out->mem.tail_last, out->time.tail_last, sizeof(out->time.tail_last));
+      out->mem.has_bands = out->time.has_bands;
+      const double te = now_ms();
+      out->n_exchanges = r.n_exchanges;
+      out->k3a_ms = finfo.kernel_ms;
+      out->k4_ms = 0.0;
+      out->stage_ms[0] = tf - t0; out->stage_ms[1] = 0.0; out->stage_ms[2] = 0.0;
+      out->stage_ms[3] = te - tf; out->stage_ms[4] = te - t0;
+      return TML_OK;
     }
   }
   tml_win_info info;

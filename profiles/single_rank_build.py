@@ -9,6 +9,11 @@ line:
   * ``stage_ms``: the native driver's own stage times and ``k3a`` (the fused pass), medians;
   * ``sections_json_ms``: the host time of ``tml_sections_json`` alone, and ``python_rest_ms``,
     what is left of the wall time after the native driver and the JSON emitter;
+  * ``segments_ms``: host time of each segment of a build (medians): Python entry -> native call,
+    native call -> pass submitted, -> return from the wait, native collect, sections JSON, the
+    Python after it;
+  * ``kernel_ms``: device time per build of each kernel (torch.profiler, a run of its own), and
+    ``device_idle_ms``: ``build_ms`` minus the pass and the band kernel;
   * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved, the fused pass's
     bytes at W = 4e6), CUDA events, median of 25 after warm-up; the fused pass against it;
   * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
@@ -58,6 +63,71 @@ def copy_ceiling(torch, nbytes: int = 512_000_000, reps: int = 25) -> dict:
     del src, dst
     torch.cuda.empty_cache()
     return {"bytes_moved": 2 * nbytes, "ms": ms, "GBps": 2 * nbytes / (ms * 1e-3) / 1e9}
+
+
+def segments(summ, W: int, steps: int) -> dict:
+    """Host time of each segment of one build, medians over ``steps`` builds.  The native entry points
+    are wrapped to stamp their calls; the driver's own stage times split the reduce inside them:
+    ``reduce`` is its host time up to the submission of the pass (0 where a driver does not report
+    it), ``prepare`` up to the return from the wait, ``bands`` the collect after it."""
+    from traceml_b200 import _abi
+
+    lib = _abi.lib()
+    stamps: list = []
+    wrapped = {}
+    for name in ("tml_summary_run_", "tml_reduce_run", "tml_sections_json"):
+        fn = getattr(lib, name, None)
+        if fn is None:
+            continue
+
+        def stamp(*a, _fn=fn):
+            t0 = time.perf_counter()
+            rc = _fn(*a)
+            stamps.append((t0, time.perf_counter()))
+            return rc
+
+        wrapped[name] = fn
+        setattr(lib, name, stamp)
+    keys = ("python_to_native", "native_launch", "launch_to_wait_return", "native_collect", "sections_json",
+            "python_rest", "wall")
+    rows: dict = {k: [] for k in keys}
+    try:
+        for _ in range(steps):
+            stamps.clear()
+            t0 = time.perf_counter()
+            res = summ.build(W, PROC_ROWS)
+            t1 = time.perf_counter()
+            st = res["reduce"].timings_ms
+            before = (stamps[0][0] - t0) * 1e3
+            native = sum(b - a for a, b in stamps) * 1e3
+            rows["python_to_native"].append(before)
+            rows["native_launch"].append(st["reduce"])
+            rows["launch_to_wait_return"].append(st["prepare"] - st["reduce"])
+            rows["native_collect"].append(st["bands"])
+            rows["sections_json"].append(native - st["total"])
+            rows["python_rest"].append((t1 - t0) * 1e3 - before - native)
+            rows["wall"].append((t1 - t0) * 1e3)
+    finally:
+        for name, fn in wrapped.items():
+            setattr(lib, name, fn)
+    return {k: statistics.median(v) for k, v in rows.items()}
+
+
+def kernel_times(torch, summ, W: int, n: int = 30) -> dict:
+    """Device time per build of each of the library's kernels (``k_*``), from torch.profiler over
+    ``n`` builds: a run of its own, since tracing slows the host."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(n):
+            summ.build(W, PROC_ROWS)
+        torch.cuda.synchronize()
+    out: dict = {}
+    for e in prof.key_averages():
+        name = e.key.split("(")[0]
+        if name.startswith("k_"):
+            out[name] = out.get(name, 0.0) + e.device_time_total / 1e3 / n
+    return out
 
 
 def measure(steps: int, window: int, warmup: int) -> dict:
@@ -114,6 +184,8 @@ def measure(steps: int, window: int, warmup: int) -> dict:
         t0 = time.perf_counter()
         eng.sections_json(o, replay.PROC_RAM_TOTAL_BYTES, 1, W, PROC_ROWS)
         sj.append((time.perf_counter() - t0) * 1e3)
+    seg = segments(summ, W, steps)
+    kern = kernel_times(torch, summ, W)
     eng.close()
     del host, recs
     med = {k: statistics.median(v) for k, v in stage.items() if not k.startswith("host_")}
@@ -128,6 +200,9 @@ def measure(steps: int, window: int, warmup: int) -> dict:
         "stage_ms": med, "sections_json_ms": sj_ms,
         "python_rest_ms": wall_ms - med.get("total", 0.0) - sj_ms,
         "native_minus_fused_ms": med.get("total", 0.0) - k3a,
+        "segments_ms": seg, "kernel_ms": kern,
+        # what the device does not spend in the pass or the band sums (both timed on the device)
+        "device_idle_ms": build_ms - k3a - (kern.get("k_bands") or 0.0),
         "copy_ceiling": ceil,
         "fused_pass": {"bytes": fused_bytes, "ms": k3a, "GBps": fused_gbps,
                        "of_copy_ceiling": (fused_gbps / ceil["GBps"]) if fused_gbps else None,
@@ -158,13 +233,15 @@ def alternate(args) -> None:
                 "all": xs}
 
     summary = {"compare": {}, "gpu": runs["chain"][0]["gpu"]}
-    for key in ("build_ms", "build_wall_ms"):
+    for key in ("build_ms", "build_wall_ms", "device_idle_ms"):
         per = {a: stats([r[key] for r in runs[a]]) for a in ARMS}
         d = per["three_wait"]["median"] - per["chain"]["median"]
         summary["compare"][key] = dict(per, saving_ms=d, saving_frac=d / per["three_wait"]["median"],
                                        beyond_spread=d > max(per["chain"]["spread"], per["three_wait"]["spread"]))
     summary["stage_ms"] = {a: {k: statistics.median(r["stage_ms"][k] for r in runs[a]) for k in runs[a][0]["stage_ms"]}
                            for a in ARMS}
+    summary["segments_ms"] = {a: {k: statistics.median(r["segments_ms"][k] for r in runs[a])
+                                  for k in runs[a][0]["segments_ms"]} for a in ARMS}
     summary["launches_per_build"] = {a: runs[a][0]["launches_per_build"] for a in ARMS}
     summary["copy_ceiling_GBps"] = statistics.median(r["copy_ceiling"]["GBps"] for a in ARMS for r in runs[a])
     summary["fused_of_copy_ceiling"] = {a: statistics.median(r["fused_pass"]["of_copy_ceiling"] for r in runs[a])

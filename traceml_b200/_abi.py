@@ -221,6 +221,10 @@ SIGNATURES = {
     "tml_diag_step_time": (C.c_int, [C.POINTER(StDiagIn), C.c_char_p, C.c_size_t]),
     "tml_diag_step_memory": (C.c_int, [C.POINTER(MemDiagIn), C.c_char_p, C.c_size_t]),
     "tml_diag_process": (C.c_int, [C.POINTER(ProcDiagIn), C.c_char_p, C.c_size_t]),
+    # private (csrc/tml_internal.h): tml_reduce_run that emits an earlier reduce's sections meanwhile
+    "tml_summary_run_": (C.c_int, [vp, C.POINTER(Comm), C.POINTER(ReduceRunArgs), vp, C.POINTER(ReduceRunOut),
+                                   C.POINTER(ReduceRunOut), C.POINTER(SectionsArgs), vp, C.c_size_t,
+                                   C.POINTER(C.c_int)]),
 }
 
 _LIB: Optional[C.CDLL] = None
@@ -282,19 +286,42 @@ def diag_json(fn_name: str, arg: C.Structure, cap: int = 1 << 16) -> Any:
 _SEC_BUF = None
 
 
-def sections_json(run_out, ram_total: float, gpu_count: int, window: int, proc_rows: int) -> Any:
-    """tml_sections_json -> dict; rank-keyed step-time tables get their int keys back."""
+def _sections_text(run_out, args) -> bytes:
     global _SEC_BUF
     if _SEC_BUF is None:
         _SEC_BUF = C.create_string_buffer(1 << 18)
-    args = SectionsArgs(float(ram_total), int(gpu_count), int(window), int(proc_rows or 0), 0)
     rc = lib().tml_sections_json(C.byref(run_out), C.byref(args), _SEC_BUF, len(_SEC_BUF))
     if rc == -8:  # TML_ERR_SMALL
         _SEC_BUF = C.create_string_buffer(len(_SEC_BUF) * 8)
-        return sections_json(run_out, ram_total, gpu_count, window, proc_rows)
+        return _sections_text(run_out, args)
     check(rc, "tml_sections_json")
     # string_at: strlen + one copy; .value walks the 256 KB buffer byte by byte in Python's C loop
-    return Sections(C.string_at(_SEC_BUF))
+    return C.string_at(_SEC_BUF)
+
+
+def sections_json(run_out, ram_total: float, gpu_count: int, window: int, proc_rows: int) -> Any:
+    """tml_sections_json -> dict; rank-keyed step-time tables get their int keys back."""
+    args = SectionsArgs(float(ram_total), int(gpu_count), int(window), int(proc_rows or 0), 0)
+    return Sections(_sections_text(run_out, args))
+
+
+_PREV_BUF = None
+
+
+def summary_run(handle, comm, run_args, run_out, stream: int, prev: "Sections") -> None:
+    """tml_reduce_run into ``run_out``; while its pass runs, the native driver emits the text of
+    ``prev`` (the sections of an earlier reduce, from their own copy of its result), which it
+    would otherwise emit on first access."""
+    global _PREV_BUF
+    if _PREV_BUF is None:
+        _PREV_BUF = C.create_string_buffer(1 << 18)
+    prc = C.c_int(0)
+    check(lib().tml_summary_run_(handle, C.byref(comm), C.byref(run_args), stream, C.byref(run_out),
+                                 C.byref(prev._src), C.byref(prev._args), _PREV_BUF, len(_PREV_BUF), C.byref(prc)),
+          "tml_summary_run_")
+    if prc.value == 0 and prev._raw is None:
+        prev._raw = C.string_at(_PREV_BUF)
+    # else (TML_ERR_SMALL, ...): prev emits its text itself on first access, and reports errors there
 
 
 class Sections:
@@ -304,12 +331,21 @@ class Sections:
     only asked for its diagnosis label, never pays for the rest.  ``reduce`` (the raw reduce
     output) and anything else the caller attaches live beside the parsed sections."""
 
-    __slots__ = ("raw", "_parsed", "_extra")
+    __slots__ = ("_raw", "_src", "_args", "_parsed", "_extra")
 
-    def __init__(self, raw: bytes):
-        self.raw = raw
+    def __init__(self, raw: Optional[bytes] = None, src=None, args=None):
+        """``raw``: the text; or ``src`` (a ReduceRunOut the object owns) and ``args`` (SectionsArgs)
+        to emit it from, on first access unless ``summary_run`` has emitted it before."""
+        self._raw = raw
+        self._src, self._args = src, args
         self._parsed = None
         self._extra = {}
+
+    @property
+    def raw(self) -> bytes:
+        if self._raw is None:
+            self._raw = _sections_text(self._src, self._args)
+        return self._raw
 
     def _get(self):
         if self._parsed is None:

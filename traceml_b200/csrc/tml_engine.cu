@@ -121,12 +121,6 @@ struct ChainOut {
   u64 band_cnt[48];
   double tail[32];      // k_bands: [series][first, last]
 };
-// The chained pass's own accumulator and completion ticket, armed at context creation and
-// re-armed by the pass's last CTA, so no host copy sits in front of the kernel.
-struct ChainState {
-  WinAcc acc;
-  unsigned int ticket;
-};
 
 // ------------------------------------------------------------------ device helpers
 
@@ -418,14 +412,13 @@ __device__ __forceinline__ void block_sum(double (&v)[NV], double* out) {
 // out[c] = reduce over b of partials[b * ncols + c]; op per column: 0 sum, 1 max.
 // One warp per column: lane l folds blocks l, l+32, ... in order, then a fixed
 // shuffle tree -- deterministic for a given grid, and ~nblk/32 dependent loads deep.
-// Shared by k_finalize and the last CTA of k_window_fused, so both give the same bits.  The
-// partials come from other CTAs of a running grid in the latter: L2 loads, never the nc path.
+// Shared by k_finalize and the chained build's extra k_bands CTAs, so both give the same bits.
 __device__ __forceinline__ void finalize_column(const double* partials, int nblk, int ncols, u32 max_mask,
                                                 int c, int lane, double* out) {
   const bool is_max = (max_mask >> c) & 1u;
   double x = is_max ? -INFINITY : 0.0;
   // eight loads in flight before they are folded, still in block order: one L2 round trip per
-  // eight blocks instead of one per block (it is the tail of the chained pass)
+  // eight blocks instead of one per block
   for (int b0 = lane; b0 < nblk; b0 += 32 * 8) {
     double p[8];
 #pragma unroll
@@ -761,18 +754,14 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // consecutive doubles per tile: 256-B fully coalesced stores, no staging buffer.  Bounds, counters,
 // tree sums and maxima are produced exactly as in k_window_rows; the host accepts the series only
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
-// otherwise it falls back to the staged path.
-// CHAINED (the chained build): the CTAs count themselves out on the ticket and the last
-// one folds the partials with finalize_column and hands the accumulator over to chain_out, then
-// re-arms both -- no k_finalize launch behind the pass and no accumulator copy in front of it.
+// otherwise it falls back to the staged path.  In the chained build the extra CTAs of the
+// k_bands launch behind it fold the partials and hand the accumulator over (k_bands).
 #define WF_WARP_U4 (2 * 32 * 8)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
 
-template <bool CHAINED>
 __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
     const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
-    double* __restrict__ series, u64 n_ser, WinAcc* acc, double* partials, unsigned int* ticket,
-    ChainOut* chain_out) {
+    double* __restrict__ series, u64 n_ser, WinAcc* acc, double* partials) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint4* w_in0 = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
@@ -927,24 +916,6 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
       double x = -INFINITY;
       for (int w = 0; w < WR_THREADS / 32; ++w) x = fmax(x, s_mx[w][tid]);
       partials[(size_t)blockIdx.x * 11 + 9 + tid] = x;
-    }
-  }
-  if (CHAINED) {  // chained build: the last CTA to finish does k_finalize's work, in its order
-    __threadfence();  // this CTA's partials and accumulator atomics, before its ticket
-    int last = 0;
-    if (tid == 0) last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    // the vote rides the barrier: a 16-B __shared__ flag made the whole pass ~30 us slower on an
-    // H100 80GB HBM3 (400 W), measured; static shared memory stays at 704 B, as unchained
-    if (__syncthreads_or(last)) {
-      __threadfence();
-      for (int col = warp; col < 11; col += WR_WARPS)
-        finalize_column(partials, (int)gridDim.x, 11, (1u << 9) | (1u << 10), col, lane, chain_out->fin);
-      if (tid < WINACC_WORDS) {  // hand the accumulator over and re-arm it for the next pass
-        u64* a = reinterpret_cast<u64*>(acc);
-        reinterpret_cast<u64*>(&chain_out->acc)[tid] = __ldcg(a + tid);
-        a[tid] = tid < 2 ? ~0ull : 0ull;  // lo[0], lo[1] start at ~0, every other word at 0
-        if (tid == 0) *ticket = 0u;
-      }
     }
   }
 }
@@ -1370,12 +1341,31 @@ struct BandParams {
   u64 n_common, shard_lo, shard_hi;
   u64 lo[2][3], hi[2][3];
   u64 tail_first[2];
+  // the chained build's k_window_fused (fin_nblk CTAs): its partials, accumulator and result block
+  const double* fin_partials;
+  int fin_nblk;
+  WinAcc* fin_acc;
+  ChainOut* fin_out;
 };
 
-// grid (16 series, 4): y = 0..2 band sums over band ^ shard, y = 3 tail endpoints
+// grid (16 series, 4): y = 0..2 band sums over band ^ shard, y = 3 tail endpoints.
+// Chained build, grid (16, 5): row y = 4 finishes the window pass in front instead of a k_finalize
+// launch -- CTA x < 11 folds column x with finalize_column (k_finalize's code and block order, so
+// the same bits), CTA 11 hands the accumulator over to fin_out and re-arms it for the next pass.
 __global__ void __launch_bounds__(256) k_bands(const __grid_constant__ BandParams p, double* out_sum,
                                                u64* out_cnt, double* out_tail) {
   const int s = blockIdx.x, b = blockIdx.y;
+  if (b == 4) {
+    if (s < 11) {
+      if (threadIdx.x < 32)
+        finalize_column(p.fin_partials, p.fin_nblk, 11, (1u << 9) | (1u << 10), s, threadIdx.x, p.fin_out->fin);
+    } else if (s == 11 && threadIdx.x < WINACC_WORDS) {
+      u64* a = reinterpret_cast<u64*>(p.fin_acc);
+      reinterpret_cast<u64*>(&p.fin_out->acc)[threadIdx.x] = a[threadIdx.x];
+      a[threadIdx.x] = threadIdx.x < 2 ? ~0ull : 0ull;  // lo[0], lo[1] start at ~0, every other word at 0
+    }
+    return;
+  }
   const int kind = (s >= 12) ? 1 : 0;
   const double* v = p.series + (u64)s * p.n_common;
   if (b == 3) {
@@ -1605,10 +1595,12 @@ struct tml_ctx {
   cudaEvent_t xs_gate = nullptr, xs_done = nullptr;
   bool xs_defer = false, xs_pending = false;
   double* d_partials = nullptr;  // max(grid) * 16 doubles
-  double* d_final = nullptr;     // 64 doubles, then d_winacc, d_chain_out, d_chain_state
+  double* d_final = nullptr;     // 64 doubles, then d_winacc, d_chain_out, d_chain_acc
   u64* d_bandcnt = nullptr;
-  ChainOut* d_chain_out = nullptr;      // the chained single-rank build's results (one copy), in d_final's allocation
-  ChainState* d_chain_state = nullptr;  // ... and its pass's own accumulator + ticket (always armed)
+  ChainOut* d_chain_out = nullptr;  // the chained single-rank build's results (one copy), in d_final's allocation
+  // ... and its pass's own accumulator: armed at context creation and re-armed by the k_bands launch
+  // that reads it, so no host copy sits in front of the pass
+  WinAcc* d_chain_acc = nullptr;
   u64 chain_n = 0, chain_window = 0;    // the chained pass in flight: retained rows, window
   bool chain_pending = false;
   void* h_stage = nullptr;       // pinned 4 KB result staging
@@ -1768,21 +1760,21 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   CK(cudaMalloc(&c->d_xs_out, 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_xs_stats, 8 * sizeof(u64)));
   CK(cudaMalloc(&c->d_partials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
-  // d_final | K3a's WinAcc (one D2H copy fetches both) | the chained build's ChainOut, ChainState
+  // d_final | K3a's WinAcc (one D2H copy fetches both) | the chained build's ChainOut, accumulator
   const size_t fin_bytes = 64 * sizeof(double) + sizeof(WinAcc);
   static_assert((64 * sizeof(double) + sizeof(WinAcc)) % 8 == 0 && sizeof(ChainOut) % 8 == 0, "8-B aligned");
-  CK(cudaMalloc(&c->d_final, fin_bytes + sizeof(ChainOut) + sizeof(ChainState)));
+  CK(cudaMalloc(&c->d_final, fin_bytes + sizeof(ChainOut) + sizeof(WinAcc)));
   c->d_winacc = reinterpret_cast<WinAcc*>(c->d_final + 64);
   c->d_chain_out = reinterpret_cast<ChainOut*>((char*)c->d_final + fin_bytes);
-  c->d_chain_state = reinterpret_cast<ChainState*>((char*)c->d_final + fin_bytes + sizeof(ChainOut));
+  c->d_chain_acc = reinterpret_cast<WinAcc*>((char*)c->d_final + fin_bytes + sizeof(ChainOut));
   CK(cudaMalloc(&c->d_ppartials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_pfinal, 32 * sizeof(double)));
   CK(cudaMalloc(&c->d_bandcnt, 64 * sizeof(u64)));
-  {  // armed once here; every chained pass re-arms it on its way out
-    ChainState armed;
+  {  // armed once here; the k_bands launch behind every chained pass re-arms it
+    WinAcc armed;
     memset(&armed, 0, sizeof(armed));
-    armed.acc.lo[0] = armed.acc.lo[1] = ~0ull;
-    CK(cudaMemcpy(c->d_chain_state, &armed, sizeof(armed), cudaMemcpyHostToDevice));
+    armed.lo[0] = armed.lo[1] = ~0ull;
+    CK(cudaMemcpy(c->d_chain_acc, &armed, sizeof(armed), cudaMemcpyHostToDevice));
   }
   CK(cudaHostAlloc(&c->h_stage, 4096, cudaHostAllocDefault));
   *out = c;
@@ -2302,9 +2294,9 @@ int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_
 }
 
 // k_window_fused on stream s over the retained ring's last `window` rows (n > 0), between ev0 and
-// ev1.  chained: the pass finalises itself into d_chain_out from its own, always armed,
-// accumulator; otherwise d_winacc is armed by a copy in front and k_finalize runs behind.
-static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, bool chained) {
+// ev1; *grid_out: its CTAs.  chained: into d_chain_acc, always armed, and the caller finalises it
+// (k_bands); otherwise d_winacc is armed by a copy in front and k_finalize runs behind.
+static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, bool chained, int* grid_out) {
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
   const u64 t_start = n > window ? n - window : 0;
@@ -2318,21 +2310,16 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t 
   }
   static bool wf_attr = false;
   if (!wf_attr) {
-    CK(cudaFuncSetAttribute(k_window_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
-    CK(cudaFuncSetAttribute(k_window_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
     wf_attr = true;
   }
   int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
   if (grid > c->n_sms * 2) grid = c->n_sms * 2;
+  *grid_out = grid;
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   CK(cudaEventRecord(c->ev0, s));
-  if (chained)
-    k_window_fused<true><<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
-                                                            &c->d_chain_state->acc, c->d_partials,
-                                                            &c->d_chain_state->ticket, c->d_chain_out);
-  else
-    k_window_fused<false><<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
-                                                            c->d_winacc, c->d_partials, nullptr, nullptr);
+  k_window_fused<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
+                                                         chained ? c->d_chain_acc : c->d_winacc, c->d_partials);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
   c->launches += 1;
@@ -2401,7 +2388,8 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
   out->n_retained = n;
   out->monotone = 1;
   if (n == 0) return TML_OK;
-  int rc = fused_pass(c, window, series, s, false);
+  int grid = 0;
+  int rc = fused_pass(c, window, series, s, false, &grid);
   if (rc != TML_OK) return rc;
   // d_final[32..43) tree sums + maxima | d_final[64..] WinAcc: one copy
   char* st = (char*)c->h_stage;
@@ -2426,16 +2414,19 @@ int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, con
   c->chain_n = n;
   c->chain_window = window;
   c->chain_pending = false;
-  int rc = fused_pass(c, window, series, s, true);
+  int grid = 0;
+  int rc = fused_pass(c, window, series, s, true, &grid);
   if (rc != TML_OK) return rc;
-  // k_bands exactly as tml_win_bands launches it, into the packed block's own slots
+  // k_bands as tml_win_bands launches it, into the packed block's own slots, plus the row of CTAs
+  // that finishes the pass
   BandParams p;
   p.series = series; p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
   memcpy(p.lo, bands->band_lo, sizeof(p.lo));
   memcpy(p.hi, bands->band_hi, sizeof(p.hi));
   memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
+  p.fin_partials = c->d_partials; p.fin_nblk = grid; p.fin_acc = c->d_chain_acc; p.fin_out = c->d_chain_out;
   char* co = (char*)c->d_chain_out;
-  k_bands<<<dim3(16, 4), 256, 0, s>>>(p, (double*)(co + offsetof(ChainOut, band_sum)),
+  k_bands<<<dim3(16, 5), 256, 0, s>>>(p, (double*)(co + offsetof(ChainOut, band_sum)),
                                       (u64*)(co + offsetof(ChainOut, band_cnt)), (double*)(co + offsetof(ChainOut, tail)));
   CK(cudaPeekAtLastError());
   c->launches += 1;
@@ -2812,6 +2803,7 @@ int tml_win_bands(tml_ctx* c, const double* series, const tml_band_args* a, void
   memcpy(p.lo, a->band_lo, sizeof(p.lo));
   memcpy(p.hi, a->band_hi, sizeof(p.hi));
   memcpy(p.tail_first, a->tail_first, sizeof(p.tail_first));
+  p.fin_partials = nullptr; p.fin_nblk = 0; p.fin_acc = nullptr; p.fin_out = nullptr;
   double* d_sum = c->d_final;            // 48 doubles
   double* d_tail = c->d_partials;        // 32 doubles (scratch)
   k_bands<<<dim3(16, 4), 256, 0, s>>>(p, d_sum, c->d_bandcnt, d_tail);

@@ -14,14 +14,22 @@ void** tml_run_ws_slot_(tml_ctx* ctx);
 void tml_run_ws_free_(void* ws);
 
 // The dense single-rank build as one device submission (tml_reduce_run's world == 1 branch).
-// launch: k_window_fused, which finalises itself, then k_bands over `series` with `bands` (the
-// host knows n_window, so the band layout, before the pass).  finish: joins the process
-// aggregates launched in between (their event), one device-to-host copy, one stream wait; then
-// reports what tml_win_fused and tml_win_bands would.  *ok = 0: not dense, drop the bands.
+// launch: k_window_fused, then k_bands over `series` with `bands` (the host knows n_window, so the
+// band layout, before the pass) and one more row of CTAs that finalises the pass.  finish: one
+// device-to-host copy, one stream wait; then reports what tml_win_fused and tml_win_bands would.
+// *ok = 0: not dense, drop the bands.
 int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
                                 void* stream);
 int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
                                 tml_band_out* band_out, uint32_t* ok);
+
+// tml_reduce_run that also emits tml_sections_json(prev, prev_sections) into prev_json (status in
+// *prev_rc): an earlier reduce's sections, from the caller's own copy of its result.  The chained
+// single-rank build emits them while its window pass runs, every other path after the reduce.
+// Back-to-back builds (SummaryEngine.build) so keep the JSON emitter off the GPU's critical path.
+int tml_summary_run_(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args, void* stream,
+                     tml_reduce_run_out* out, const tml_reduce_run_out* prev, const tml_sections_args* prev_sections,
+                     char* prev_json, size_t prev_cap, int* prev_rc);
 
 #ifdef __cplusplus
 }

@@ -598,10 +598,24 @@ double now_ms() {
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
 }
 
-}  // namespace
+// Host work tml_summary_run_ hands in to be done while the chained pass runs: an earlier reduce's
+// sections JSON (it needs nothing of this reduce).
+struct PreWait {
+  const tml_reduce_run_out* prev;
+  const tml_sections_args* prev_sections;
+  char* json;
+  size_t cap;
+  int rc = TML_OK;
+  bool done = false;
+  void run() {
+    if (done) return;
+    rc = tml_sections_json(prev, prev_sections, json, cap);
+    done = true;
+  }
+};
 
-extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args, void* stream,
-                              tml_reduce_run_out* out) {
+int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args, void* stream,
+               tml_reduce_run_out* out, PreWait* pre) {
   if (!c || !args || !out || args->window == 0) return TML_ERR_ARG;
   const int world = comm ? comm->world : 1, rank = comm ? comm->rank : 0;
   if (world < 1 || world > (int)TML_MAX_RANKS || rank < 0 || rank >= world) return TML_ERR_ARG;
@@ -639,6 +653,7 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
     CKC(cudaStreamWaitEvent(r.w->side, r.w->side_gate, 0));
     CKT(tml_proc_reduce_launch(c, args->proc_rows, r.w->side));
   }
+  const double tl = now_ms();
   // ---- single rank, bulk window: ring -> series in ONE pass (k_window_fused); the WindowRows
   // that K3a would write for K4 to re-read never exist.  Falls through to the staged path when the
   // window is not dense (re-flushed step ids, rows without memory, ...).  Chained (the default):
@@ -649,6 +664,7 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
     tml_band_out cbo;
     uint32_t ok = 0;
     if (chain) {
+      if (pre) pre->run();  // the GPU is busy with the pass
       CKT(tml_win_fused_chain_finish_(c, r.s, &finfo, &fal, &cbo, &ok));
     } else {
       CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
@@ -684,7 +700,8 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
       out->n_exchanges = r.n_exchanges;
       out->k3a_ms = finfo.kernel_ms;
       out->k4_ms = 0.0;
-      out->stage_ms[0] = tf - t0; out->stage_ms[1] = 0.0; out->stage_ms[2] = 0.0;
+      // prepare: up to the end of the wait; reduce (launch): up to the submission of the pass
+      out->stage_ms[0] = tf - t0; out->stage_ms[1] = 0.0; out->stage_ms[2] = tl - t0;
       out->stage_ms[3] = te - tf; out->stage_ms[4] = te - t0;
       return TML_OK;
     }
@@ -834,6 +851,26 @@ extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce
   out->stage_ms[0] = t1 - t0; out->stage_ms[1] = t2 - t1; out->stage_ms[2] = t3 - t2;
   out->stage_ms[3] = t4 - t3; out->stage_ms[4] = t4 - t0;
   return TML_OK;
+}
+
+}  // namespace
+
+extern "C" int tml_reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args, void* stream,
+                              tml_reduce_run_out* out) {
+  return reduce_run(c, comm, args, stream, out, nullptr);
+}
+
+extern "C" int tml_summary_run_(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args, void* stream,
+                                tml_reduce_run_out* out, const tml_reduce_run_out* prev,
+                                const tml_sections_args* prev_sections, char* prev_json, size_t prev_cap,
+                                int* prev_rc) {
+  if (!prev || !prev_sections || !prev_json || !prev_rc || prev == out) return TML_ERR_ARG;
+  PreWait pre;
+  pre.prev = prev; pre.prev_sections = prev_sections; pre.json = prev_json; pre.cap = prev_cap;
+  const int rc = reduce_run(c, comm, args, stream, out, &pre);
+  pre.run();  // every path but the chained build: after the reduce
+  *prev_rc = pre.rc;
+  return rc;
 }
 
 extern "C" void tml_run_ws_free_(void* p) {

@@ -212,11 +212,16 @@ class Engine:
         return int(p.value) + int.from_bytes(handle[64:72], "little")
 
     def reduce_run(self, window: int, proc_rows: int, exchange: str, speculate: bool, comm_ptr: int,
-                   rank: int, world: int, stream: int = 0) -> _abi.ReduceRunOut:
-        """The whole staged reduce, sequenced natively (csrc/tml_summary.cpp)."""
+                   rank: int, world: int, stream: int = 0, prev=None) -> _abi.ReduceRunOut:
+        """The whole staged reduce, sequenced natively (csrc/tml_summary.cpp).  ``prev``: sections
+        (``_abi.Sections``) of an earlier reduce whose text is still to be emitted; the driver emits
+        it while this reduce's window pass runs."""
         comm = _abi.Comm(comm_ptr or None, int(rank), int(world))
         args = _abi.ReduceRunArgs(int(window), int(proc_rows or 0), _abi.XCHG[exchange], 1 if speculate else 0)
         out = self._run_out  # ~45 KB: reused, not reallocated per call
+        if prev is not None:
+            _abi.summary_run(self._h, comm, args, out, stream, prev)
+            return out
         _abi.check(self._lib.tml_reduce_run(self._h, C.byref(comm), C.byref(args), stream, C.byref(out)),
                    "tml_reduce_run")
         return out

@@ -478,8 +478,9 @@ class WindowReducer:
             return True
         return bool(getattr(self.comm, "nccl_comm_ptr", lambda d: None)(self.device))
 
-    def run_native(self, window: int, proc_rows: Optional[int], stream: Optional[int] = None):
-        """tml_reduce_run on this process's engine; the raw result struct (valid until the next run)."""
+    def run_native(self, window: int, proc_rows: Optional[int], stream: Optional[int] = None, prev=None):
+        """tml_reduce_run on this process's engine; the raw result struct (valid until the next run).
+        ``prev``: see ``Engine.reduce_run``."""
         eng = self.engines[0]
         world = self.comm.world
         ptr = self.comm.nccl_comm_ptr(self.device) if world > 1 else 0
@@ -488,7 +489,7 @@ class WindowReducer:
             xchg = "a2a"  # the native driver's own "auto" assumes one host (p2p from 10^6 rows)
         return eng.reduce_run(window, int(proc_rows or 0), xchg,
                               self.speculate, ptr or 0, self.comm.index, world,
-                              _stream_of(self.device) if stream is None else stream)
+                              _stream_of(self.device) if stream is None else stream, prev=prev)
 
     def _reduce_native(self, window: int, proc_rows: Optional[int], stream: int) -> ReduceOutput:
         return self.convert_native(self.run_native(window, proc_rows, stream), window, proc_rows)

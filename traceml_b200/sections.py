@@ -282,6 +282,7 @@ class SummaryEngine:
                 ram_total = float(os.sysconf("SC_PAGE_SIZE") * os.sysconf("SC_PHYS_PAGES"))
         self.ram_total = ram_total
         self.gpu_count = gpu_count
+        self._unemitted: Optional[_abi.Sections] = None  # the last native build's sections
 
     def build(self, window: int = 10_000, proc_rows: int = 10_000, *, timings: bool = False) -> Dict[str, Any]:
         import torch
@@ -292,10 +293,17 @@ class SummaryEngine:
             # all native (csrc/tml_summary.cpp, tml_sections.cpp); the host parses one JSON
             from .reduce import NativeReduceOutput
 
+            # The text is emitted from the result's own copy: on first access, or by the next build
+            # while its window pass runs, whichever comes first -- so back-to-back builds keep the
+            # JSON emitter out of the time the GPU waits for the host.
             rows = max(1, int(proc_rows))
-            o = self.reducer.run_native(max(1, int(window)), rows)
-            res = self.engines[0].sections_json(o, self.ram_total, gpu_count, max(1, int(window)), rows)
-            res["reduce"] = NativeReduceOutput(self.reducer, o, max(1, int(window)), rows)
+            w = max(1, int(window))
+            prev = self._unemitted
+            o = self.reducer.run_native(w, rows, prev=prev if prev is not None and prev._raw is None else None)
+            red = NativeReduceOutput(self.reducer, o, w, rows)
+            res = _abi.Sections(src=red._snap, args=_abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0))
+            res["reduce"] = red
+            self._unemitted = res
             return res
         box: Dict[str, Any] = {}
 

@@ -51,7 +51,7 @@ static_assert(sizeof(tml_proc_record) == 64, "ProcRecord must be 64 B");
 #define RF_USABLE 1u       // some summarised phase > 0  (model.py:188-196)
 #define RF_HAS_MEM 2u
 #define RF_IN_TIME 4u      // inside the last-W time window
-#define RF_CAND_T 8u       // time-alignment candidate: usable, in window, first row of its step id
+#define RF_CAND_T 8u       // time-alignment candidate: usable, in window, oldest usable row of its step id
 #define RF_CAND_M 16u      // memory candidate: has_mem and last row of its step id
 
 // ------------------------------------------------------------------ device state
@@ -548,6 +548,7 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     if (slot_next >= ring_slots) slot_next -= ring_slots;
     if (next < nwt) wr_issue_warp(nxt, ring4, ring_slots, slot_next, n, next * 32, lane);
     cp_async_commit();
+    const u64 slot_tile = slot_cur;  // ring slot of this tile's first record
     // tile-edge neighbours (first/last-of-step tests) straight from the ring
     u64 halo_step = 0;
     u32 halo_flags = 0;
@@ -577,6 +578,34 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     if (lane == 31) { next_step = halo_step; next_flags = halo_flags; }
     double t_dl = 0.0, t_fwd = 0.0, t_bwd = 0.0, t_opt = 0.0, t_wall = 0.0, t_tr = 0.0;  // K3e chunk sums
 
+    // Time candidate: the OLDEST USABLE row of its step id inside the window.  The reference reads the
+    // rows newest first, skips unusable ones and lets an older row overwrite a newer one of the same
+    // step (model.py:226-248), so a step whose oldest row is unusable is kept through a newer row.
+    // A run of one step id is contiguous in a monotone ring; runs are cut at t_start.
+    const bool uit_row = live && i >= t_start &&
+                         ((((u64)c0.z | ((u64)c0.w << 32)) | ((u64)c1.z | ((u64)c1.w << 32)) |
+                           ((u64)c2.x | ((u64)c2.y << 32)) | ((u64)c2.z | ((u64)c2.w << 32)) |
+                           ((u64)c3.x | ((u64)c3.y << 32))) != 0ull);  // usable: a summarised phase > 0 ns
+    const u32 heads = __ballot_sync(0xffffffffu, lane == 0 || i == t_start || prev_step != step);
+    const u32 uits = __ballot_sync(0xffffffffu, uit_row);
+    const int head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));  // lane where this row's run starts
+    bool older_usable = (uits & ((1u << lane) - 1u) & ~((1u << head) - 1u)) != 0u;
+    {
+      bool carry = false;  // the run of lane 0 began in an earlier tile: a usable window row before it?
+      if (lane == 0 && live && base > t_start && prev_step == step) {
+        u64 j = base, sl = slot_tile;
+        while (j > t_start) {
+          --j;
+          sl = sl == 0 ? ring_slots - 1 : sl - 1;
+          const tml_step_record* p = &ring[sl];
+          if (p->step != step) break;
+          if ((p->dur_ns[0] | p->dur_ns[2] | p->dur_ns[3] | p->dur_ns[4] | p->dur_ns[5]) != 0ull) { carry = true; break; }
+        }
+      }
+      carry = __shfl_sync(0xffffffffu, carry, 0);
+      older_usable = older_usable || (head == 0 && carry);
+    }
+
     if (live) {
       const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
       const u64 d1 = (u64)c1.x | ((u64)c1.y << 32);
@@ -593,13 +622,12 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
       const bool in_time = i >= t_start;
       const bool uit = usable && in_time;
       const bool has_prev = i > 0, has_next = (i + 1) < n;
-      const bool first_in_win = (i == t_start) || !has_prev || (prev_step != step);
       const bool last_m = !has_next || (next_step != step) || ((next_flags & TML_REC_HAS_MEM) == 0u);
       u8 f = 0;
       if (usable) f |= RF_USABLE;
       if (has_mem) f |= RF_HAS_MEM;
       if (in_time) f |= RF_IN_TIME;
-      const bool cand_t = usable && in_time && first_in_win;
+      const bool cand_t = usable && in_time && !older_usable;
       const bool cand_m = has_mem && last_m;
       if (cand_t) f |= RF_CAND_T;
       if (cand_m) f |= RF_CAND_M;
@@ -752,7 +780,9 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // W = 4e6) -- never exist.  Same warp-private
 // cp.async pipeline as k_window_rows; lane = record, so each of the 16 series receives 32
 // consecutive doubles per tile: 256-B fully coalesced stores, no staging buffer.  Bounds, counters,
-// tree sums and maxima are produced exactly as in k_window_rows; the host accepts the series only
+// tree sums and maxima are produced as in k_window_rows, except that a time candidate is simply the
+// oldest row of its step id in the window: the two rules differ only where a step id repeats, and
+// such a window is never dense under either.  The host accepts the series only
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
 // otherwise it falls back to the staged path.  In the chained build the extra CTAs of the
 // k_bands launch behind it fold the partials and hand the accumulator over (k_bands).

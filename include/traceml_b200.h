@@ -377,6 +377,83 @@ int tml_proc_reduce(tml_ctx* ctx, uint32_t max_rows, void* stream,
 int tml_proc_reduce_launch(tml_ctx* ctx, uint32_t max_rows, void* stream);
 int tml_proc_reduce_collect(tml_ctx* ctx, tml_proc_agg* out);
 
+/* ---------------------------------------------------------------- SYSTEM
+ * The host / all-GPU snapshot of local rank 0 (samplers/system_sampler.py:42-221): one fixed-size
+ * record per sample in its own HBM ring, reduced on the device into the System section's window
+ * aggregates (reporting/sections/system/loader.py:97-156) and the per-sample derived columns of the
+ * reference's writer (aggregator/sqlite_writers/system.py:381-474).  The ring (proc_slots slots)
+ * is allocated by the first commit or load.                                                     */
+#define TML_SYS_MAX_GPUS 16u
+#define TML_SYS_GPU_AVAILABLE 1u
+
+/* 32 B: the raw NVML integers of one GPU.  A GPU whose query failed is all zeros (the reference's
+ * placeholder), so that entry index == GPU id.  Watts are power_mw / 1000.0. */
+typedef struct tml_sys_gpu {
+  uint32_t util;            /* nvmlDeviceGetUtilizationRates().gpu, %  */
+  uint32_t temp_c;          /* nvmlDeviceGetTemperature, deg C         */
+  uint64_t mem_used;        /* nvmlDeviceGetMemoryInfo().used, bytes   */
+  uint64_t mem_total;
+  uint32_t power_mw;        /* nvmlDeviceGetPowerUsage                 */
+  uint32_t power_limit_mw;  /* nvmlDeviceGetPowerManagementLimit       */
+} tml_sys_gpu;
+
+/* 576 B: 64-B header + TML_SYS_MAX_GPUS GPU entries (the first n_gpus are valid). */
+typedef struct tml_sys_record {
+  uint64_t seq;
+  double ts;                /* unix seconds                            */
+  double cpu_pct;           /* psutil.cpu_percent()                    */
+  uint64_t ram_used;        /* psutil.virtual_memory().used            */
+  uint64_t ram_total;
+  uint32_t flags;           /* TML_SYS_*                               */
+  uint32_t gpu_count;       /* nvmlDeviceGetCount() (0 without NVML)   */
+  uint32_t n_gpus;          /* GPU entries in this sample (<= 16)      */
+  uint32_t _pad0;
+  uint64_t _pad1;
+  tml_sys_gpu gpu[TML_SYS_MAX_GPUS];
+} tml_sys_record;
+
+/* Per-GPU-index window aggregates (loader.py:128-156), W for power. */
+typedef struct tml_sys_gpu_agg {
+  uint64_t n;               /* samples that carried this GPU index     */
+  double util_avg, util_peak;
+  double mem_avg, mem_peak, mem_total;
+  double temp_avg, temp_peak;
+  double power_avg, power_peak, power_limit;
+} tml_sys_gpu_agg;
+
+/* Window aggregates over the latest min(retained, max_rows) samples (loader.py:97-125).  The gpu_*
+ * columns average the per-sample derived values over the n_gpu samples that have them. */
+typedef struct tml_sys_agg {
+  uint64_t n;               /* samples in the window                   */
+  uint64_t n_gpu;           /* samples with at least one GPU entry     */
+  double first_ts, last_ts;
+  double cpu_avg, cpu_peak;
+  double ram_avg, ram_peak, ram_total;
+  double gpu_util_avg, gpu_util_peak;
+  double gpu_mem_avg, gpu_mem_peak;
+  double gpu_temp_avg, gpu_temp_peak;
+  double gpu_power_avg, gpu_power_peak;
+  uint32_t gpu_available;   /* any sample had TML_SYS_GPU_AVAILABLE    */
+  uint32_t gpu_count;       /* max gpu_count                           */
+  uint32_t n_gpus;          /* GPU indices present: gpu[0 .. n_gpus)   */
+  uint32_t _pad;
+  tml_sys_gpu_agg gpu[TML_SYS_MAX_GPUS];
+} tml_sys_agg;
+
+/* One sample -> the system ring, by a 1-warp kernel on `stream` (the sampler's side stream); the
+ * record travels as a kernel argument.  No host synchronisation; never the training stream. */
+int tml_sys_commit(tml_ctx* ctx, const tml_sys_record* sample, void* stream);
+/* Bulk append from host memory (replay, tests): async H2D copies on `stream`. */
+int tml_sys_load(tml_ctx* ctx, const tml_sys_record* host_records, uint64_t n, void* stream);
+uint64_t tml_sys_count(tml_ctx* ctx); /* samples committed or loaded so far */
+/* The latest min(retained, max_records) samples, oldest first, into host memory (synchronises
+ * `stream`). */
+int tml_sys_read(tml_ctx* ctx, tml_sys_record* out, uint32_t max_records, uint32_t* n_out, void* stream);
+/* K6s k_sys_reduce over the latest min(retained, max_rows) samples: launch without synchronising
+ * (an empty ring launches nothing); collect waits on the result copy's own event. */
+int tml_sys_reduce_launch(tml_ctx* ctx, uint32_t max_rows, void* stream);
+int tml_sys_reduce_collect(tml_ctx* ctx, tml_sys_agg* out);
+
 /* ---------------------------------------------------------------- WHOLE REDUCE
  * The staged reduce above, sequenced natively for the production layout (one rank
  * per process / GPU): prepare -> bounds exchange (+ process aggregates + the
@@ -574,6 +651,18 @@ typedef struct tml_proc_diag_in {
  * diagnostics/process/context.py:242-340, rules.py:71-345, api.py:84-118. */
 int tml_diag_process(const tml_proc_diag_in* in, char* json_out, size_t cap);
 
+typedef struct tml_sys_diag_in {
+  int32_t node_rank;        /* -1: unknown (the label is then the global rank)               */
+  int32_t _pad;
+  char node_label[32];      /* SystemNodeIdentity.label of the one node (NUL-terminated)      */
+  tml_sys_agg agg;          /* n == 0: no samples (NO_DATA)                                   */
+} tml_sys_diag_in;
+
+/* Replaces diagnose_system over one node: diagnostics/system/context.py:285-373,
+ * rules.py:55-310, api.py:68-209, policy.py:22-36.  Writes {"primary", "issues", "aggregate",
+ * "per_gpu"}: the diagnosis, SystemSummaryAgg and the PerGPUSummary rows (model.py:50-117). */
+int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t cap);
+
 /* ---------------------------------------------------------------- SECTIONS
  * All three sections of one tml_reduce_run as one JSON object
  * {"step_time": {data, diagnosis, global, overview}, "step_memory": {...},
@@ -630,6 +719,12 @@ int tml_layer_drain(tml_ctx* ctx, tml_layer_record* out, uint32_t max_steps, uin
  * plan (every tile composed under the true exponent); ``slow_rows`` = rows that needed a real
  * dependent add.  Never called by the product.                                           */
 int tml_xs_host_sum(const double* x, uint64_t n, int planned, double* out_sum, uint64_t* slow_rows);
+
+/* Host emulation of k_sys_reduce's float sums (csrc/tml_sys_sum.h), so the CPU suite can fuzz them
+ * against CPython's sum().  mode 0: the per-sample restatement of CPython 3.12's compensated loop;
+ * mode 1: the window sum -- a TwoSum double-double carried through the kernel's exact reduction
+ * tree for a grid of `nblk` CTAs, rounded once.  Never called by the product. */
+int tml_sys_host_sum(const double* x, uint64_t n, uint32_t mode, uint32_t nblk, double* out_sum);
 
 #ifdef __cplusplus
 }

@@ -95,6 +95,40 @@ class ProcAgg(C.Structure):
                 ("any_gpu_available", u32), ("sum_cpu_lo", f64)]
 
 
+TML_SYS_MAX_GPUS = 16
+SYS_GPU_AVAILABLE = 1
+
+
+class SysGpu(C.Structure):
+    _fields_ = [("util", u32), ("temp_c", u32), ("mem_used", u64), ("mem_total", u64),
+                ("power_mw", u32), ("power_limit_mw", u32)]
+
+
+class SysRecord(C.Structure):
+    _fields_ = [("seq", u64), ("ts", f64), ("cpu_pct", f64), ("ram_used", u64), ("ram_total", u64),
+                ("flags", u32), ("gpu_count", u32), ("n_gpus", u32), ("_pad0", u32), ("_pad1", u64),
+                ("gpu", SysGpu * TML_SYS_MAX_GPUS)]
+
+
+class SysGpuAgg(C.Structure):
+    _fields_ = [("n", u64), ("util_avg", f64), ("util_peak", f64), ("mem_avg", f64), ("mem_peak", f64),
+                ("mem_total", f64), ("temp_avg", f64), ("temp_peak", f64), ("power_avg", f64),
+                ("power_peak", f64), ("power_limit", f64)]
+
+
+class SysAgg(C.Structure):
+    _fields_ = [("n", u64), ("n_gpu", u64), ("first_ts", f64), ("last_ts", f64),
+                ("cpu_avg", f64), ("cpu_peak", f64), ("ram_avg", f64), ("ram_peak", f64), ("ram_total", f64),
+                ("gpu_util_avg", f64), ("gpu_util_peak", f64), ("gpu_mem_avg", f64), ("gpu_mem_peak", f64),
+                ("gpu_temp_avg", f64), ("gpu_temp_peak", f64), ("gpu_power_avg", f64), ("gpu_power_peak", f64),
+                ("gpu_available", u32), ("gpu_count", u32), ("n_gpus", u32), ("_pad", u32),
+                ("gpu", SysGpuAgg * TML_SYS_MAX_GPUS)]
+
+
+class SysDiagIn(C.Structure):
+    _fields_ = [("node_rank", i32), ("_pad", i32), ("node_label", C.c_char * 32), ("agg", SysAgg)]
+
+
 class Comm(C.Structure):
     _fields_ = [("nccl_comm", vp), ("rank", i32), ("world", i32)]
 
@@ -160,7 +194,7 @@ class ProcDiagIn(C.Structure):
                 ("ram_total", f64 * TML_MAX_RANKS), ("gpu_count", i32 * TML_MAX_RANKS)]
 
 
-assert C.sizeof(StepRecord) == 128 and C.sizeof(ProcRecord) == 64
+assert C.sizeof(StepRecord) == 128 and C.sizeof(ProcRecord) == 64 and C.sizeof(SysRecord) == 576
 
 # name -> (restype, argtypes); every symbol include/traceml_b200.h declares
 SIGNATURES = {
@@ -221,10 +255,20 @@ SIGNATURES = {
     "tml_diag_step_time": (C.c_int, [C.POINTER(StDiagIn), C.c_char_p, C.c_size_t]),
     "tml_diag_step_memory": (C.c_int, [C.POINTER(MemDiagIn), C.c_char_p, C.c_size_t]),
     "tml_diag_process": (C.c_int, [C.POINTER(ProcDiagIn), C.c_char_p, C.c_size_t]),
+    "tml_sys_commit": (C.c_int, [vp, C.POINTER(SysRecord), vp]),
+    "tml_sys_load": (C.c_int, [vp, vp, u64, vp]),
+    "tml_sys_count": (u64, [vp]),
+    "tml_sys_read": (C.c_int, [vp, vp, u32, C.POINTER(u32), vp]),
+    "tml_sys_reduce_launch": (C.c_int, [vp, u32, vp]),
+    "tml_sys_reduce_collect": (C.c_int, [vp, C.POINTER(SysAgg)]),
+    "tml_diag_system": (C.c_int, [C.POINTER(SysDiagIn), C.c_char_p, C.c_size_t]),
+    "tml_sys_host_sum": (C.c_int, [vp, u64, u32, u32, C.POINTER(f64)]),
     # private (csrc/tml_internal.h): tml_reduce_run that emits an earlier reduce's sections meanwhile
     "tml_summary_run_": (C.c_int, [vp, C.POINTER(Comm), C.POINTER(ReduceRunArgs), vp, C.POINTER(ReduceRunOut),
                                    C.POINTER(ReduceRunOut), C.POINTER(SectionsArgs), vp, C.c_size_t,
                                    C.POINTER(C.c_int)]),
+    # private: K6s on the native driver's side stream, behind the caller's stream
+    "tml_sys_reduce_beside_": (C.c_int, [vp, u32, vp]),
 }
 
 _LIB: Optional[C.CDLL] = None

@@ -1049,3 +1049,192 @@ extern "C" int tml_diag_process(const tml_proc_diag_in* in, char* json_out, size
                   .kv("per_global_rank", per_rank.done()).done(),
               json_out, cap);
 }
+
+// ================================================================== system
+// diagnose_system over the engine's one node (diagnostics/system/api.py:189-209): the node's
+// rules (context.py:285-373, rules.py:55-310, policy.py:22-36), scoped to the node
+// (api.py:106-170); without an issue the cluster-level default primary (api.py:68-103).  Also
+// emits SystemSummaryAgg and the PerGPUSummary rows (reporting/sections/system/model.py:50-117).
+extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t cap) {
+  tml_json::Scope json_scope;
+  if (!in) return TML_ERR_ARG;
+  const tml_sys_agg& a = in->agg;
+  const bool have = a.n > 0, hg = a.n_gpu > 0;
+  const int n_gpus = have ? (int)std::min<uint32_t>(a.n_gpus, TML_SYS_MAX_GPUS) : 0;
+  char label_buf[33];
+  memcpy(label_buf, in->node_label, 32);
+  label_buf[32] = 0;
+  const S label(label_buf);
+  const bool has_node_rank = in->node_rank >= 0;
+
+  // ---- node signals (context.py:285-373); every GPU index < n_gpus has all its values
+  auto frac = [](double num, double den, double* out) {  // context.py:154-164
+    if (den <= 0.0) return false;
+    *out = std::max(0.0, num / den);
+    return true;
+  };
+  double ram_pct = 0.0;
+  const bool h_ram = have && frac(a.ram_peak, a.ram_total, &ram_pct);
+  if (h_ram) ram_pct = ram_pct * 100.0;
+  double mem_frac = 0.0, pow_frac = 0.0;
+  int hi_mem_idx = -1, hi_pow_idx = -1, hi_temp_idx = -1, lo_util_idx = -1;
+  double best_mem = 0.0, best_pow = 0.0, best_temp = 0.0, best_util = 0.0;
+  bool h_mem = false, h_pow = false;
+  for (int g = 0; g < n_gpus; ++g) {
+    const tml_sys_gpu_agg& q = a.gpu[g];
+    double f;
+    if (frac(q.mem_peak, q.mem_total, &f)) {
+      if (!h_mem || f > mem_frac) mem_frac = f;
+      if (hi_mem_idx < 0 || f > best_mem) { hi_mem_idx = g; best_mem = f; }
+      h_mem = true;
+    }
+    if (frac(q.power_avg, q.power_limit, &f)) {
+      if (!h_pow || f > pow_frac) pow_frac = f;
+      if (hi_pow_idx < 0 || f > best_pow) { hi_pow_idx = g; best_pow = f; }
+      h_pow = true;
+    }
+    if (hi_temp_idx < 0 || q.temp_peak > best_temp) { hi_temp_idx = g; best_temp = q.temp_peak; }
+    if (lo_util_idx < 0 || q.util_avg < best_util) { lo_util_idx = g; best_util = q.util_avg; }
+  }
+  const double mem_pct = mem_frac * 100.0, pow_pct = pow_frac * 100.0;
+
+  // ---- rules, in DEFAULT_SYSTEM_RULES order; SYSTEM_ISSUE_PRIORITY is that same order
+  std::vector<Issue> issues;
+  auto pct_s = [](double v) { return fmt("%.1f%%", v); };  // rules.py:13-14
+  auto mk = [&](const char* kind, const char* status, const char* sev, S summary, const char* action,
+                const char* metric, const char* phase, double score, int gpu, const S& ev_head) {
+    Issue i;
+    i.kind = kind; i.status = status; i.severity = sev; i.action = action;
+    i.metric = metric; i.phase = phase; i.has_metric = i.has_phase = true;
+    i.has_score = true; i.score = score;
+    if (gpu >= 0) i.ranks.push_back(gpu);
+    // _scoped_issue / _scope_text (api.py:106-150)
+    Obj scope;
+    scope.kv("level", jstr(gpu >= 0 ? "gpu" : "node")).kv("node", jstr(label))
+        .kv("node_rank", jopt_int(in->node_rank, has_node_rank));
+    if (gpu >= 0) {
+      scope.kv("gpu_idx", jint(gpu));
+      const S existing = fmt(" on gpu%d", gpu), suffix = S(" on ") + label + fmt(" gpu%d", gpu);
+      const size_t at = summary.find(existing);
+      if (at != S::npos) {
+        S o;
+        size_t from = 0, p = at;
+        while (p != S::npos) { o += summary.substr(from, p - from); o += suffix; from = p + existing.size(); p = summary.find(existing, from); }
+        o += summary.substr(from);
+        summary = o;
+      } else {
+        while (!summary.empty() && summary.back() == '.') summary.pop_back();
+        summary += suffix + ".";
+      }
+    } else if (!label.empty()) {
+      while (!summary.empty() && summary.back() == '.') summary.pop_back();
+      summary += S(" on ") + label + ".";
+    }
+    i.summary = summary;
+    S ev = ev_head;  // the rule's evidence, then scope and samples_used
+    ev.pop_back();
+    if (ev.size() > 1) ev += ",";
+    ev += "\"scope\":"; ev += scope.done();
+    ev += ",\"samples_used\":"; ev += jint((long long)a.n);
+    ev += "}";
+    i.evidence = ev;
+    issues.push_back(i);
+  };
+  auto gpu_suffix = [](int g) { return g >= 0 ? fmt(" on gpu%d", g) : S(); };
+  if (have) {
+    const S mem_band = band_of(h_mem, mem_pct, 30.0, true, 80.0, true, 90.0, true);
+    const S mem_ev = Obj().kv("gpu_mem_peak_percent", jopt_num(mem_pct, h_mem))
+                         .kv("gpu_idx", jopt_int(hi_mem_idx, hi_mem_idx >= 0)).done();
+    if (mem_band == "very_high")
+      mk("VERY_HIGH_GPU_MEMORY", "VERY HIGH GPU MEMORY", "crit",
+         S("GPU memory was very high, peaking at ") + pct_s(mem_pct) + gpu_suffix(hi_mem_idx) + ".",
+         "Reduce GPU memory pressure before scaling this run.", "gpu_mem_peak_percent", "gpu_memory", mem_pct,
+         hi_mem_idx, mem_ev);
+    if (S(band_of(hg, a.gpu_temp_peak, 0, false, 85.0, true, 0, false)) == "high")
+      mk("HIGH_GPU_TEMPERATURE", "HIGH GPU TEMPERATURE", "crit",
+         fmt("GPU temperature was high, peaking at %.1f C", a.gpu_temp_peak) + gpu_suffix(hi_temp_idx) + ".",
+         "Check cooling and thermal throttling risk.", "gpu_temp_peak_c", "gpu_temperature", a.gpu_temp_peak,
+         hi_temp_idx,
+         Obj().kv("gpu_temp_peak_c", jnum(a.gpu_temp_peak)).kv("gpu_idx", jopt_int(hi_temp_idx, hi_temp_idx >= 0)).done());
+    if (mem_band == "high")
+      mk("HIGH_GPU_MEMORY", "HIGH GPU MEMORY", "warn",
+         S("GPU memory was high, peaking at ") + pct_s(mem_pct) + gpu_suffix(hi_mem_idx) + ".",
+         "Watch GPU memory headroom for larger batches or models.", "gpu_mem_peak_percent", "gpu_memory", mem_pct,
+         hi_mem_idx, mem_ev);
+    if (S(band_of(h_pow, pow_pct, 30.0, true, 80.0, true, 0, false)) == "high")
+      mk("HIGH_GPU_POWER", "HIGH GPU POWER", "warn",
+         S("GPU power was high, averaging ") + pct_s(pow_pct) + " of limit" + gpu_suffix(hi_pow_idx) + ".",
+         "Review power headroom if this run is unstable.", "gpu_power_avg_limit_percent", "gpu_power", pow_pct,
+         hi_pow_idx,
+         Obj().kv("gpu_power_avg_limit_percent", jnum(pow_pct)).kv("gpu_idx", jopt_int(hi_pow_idx, hi_pow_idx >= 0)).done());
+    if (S(band_of(h_ram, ram_pct, 30.0, true, 80.0, true, 0, false)) == "high")
+      mk("HIGH_HOST_MEMORY", "HIGH HOST MEMORY", "warn",
+         S("Host RAM usage was high, peaking at ") + pct_s(ram_pct) + " of total.",
+         "Reduce host memory pressure or inspect data workers.", "ram_peak_percent", "ram", ram_pct, -1,
+         Obj().kv("ram_peak_percent", jnum(ram_pct)).done());
+    if (S(band_of(true, a.cpu_avg, 30.0, true, 80.0, true, 0, false)) == "high")
+      mk("HIGH_CPU", "HIGH CPU", "warn", S("CPU usage was high, averaging ") + pct_s(a.cpu_avg) + ".",
+         "Inspect CPU-side preprocessing or host contention.", "cpu_avg_percent", "cpu", a.cpu_avg, -1,
+         Obj().kv("cpu_avg_percent", jnum(a.cpu_avg)).done());
+    if (S(band_of(hg, a.gpu_util_avg, 30.0, true, 80.0, true, 0, false)) == "low")
+      mk("LOW_GPU_UTILIZATION", "LOW GPU UTILIZATION", "info",
+         S("GPU utilization was low, averaging ") + pct_s(a.gpu_util_avg) + ".",
+         "Use step-time diagnostics to check host or input stalls.", "gpu_util_avg_percent", "gpu_utilization",
+         100.0 - a.gpu_util_avg, lo_util_idx,
+         Obj().kv("gpu_util_avg_percent", jnum(a.gpu_util_avg))
+             .kv("lowest_util_gpu_idx", jopt_int(lo_util_idx, lo_util_idx >= 0)).done());
+  }
+
+  // ---- primary (api.py:68-103, 173-186)
+  auto pd = [&](const S& kind, const S& sev, const S& status, const S& reason, const S& action, long long used,
+                const S& scope) {
+    return Obj().kv("severity", jstr(sev)).kv("status", jstr(status)).kv("reason", jstr(reason))
+        .kv("action", jstr(action)).kv("kind", jstr(kind)).kv("samples_used", jint(used)).kv("scope", scope).done();
+  };
+  S primary;
+  if (!issues.empty()) {
+    const Issue& t = issues[0];
+    const size_t at = t.evidence.find("\"scope\":");
+    const size_t end = t.evidence.find('}', at);
+    primary = pd(t.kind, t.severity, t.status, t.summary, t.action, (long long)a.n,
+                 t.evidence.substr(at + 8, end + 1 - (at + 8)));
+  } else if (!have) {
+    primary = pd("NO_DATA", "info", "NO DATA", "No system telemetry was recorded.",
+                 "Collect system telemetry for host-level context.", 0, Obj().kv("level", jstr("cluster")).done());
+  } else {
+    // cluster signals carry no per-GPU rows: only the utilisation / temperature columns count
+    primary = pd("NORMAL", "info", "NORMAL",
+                 hg ? "CPU, RAM, and GPU showed no system pressure." : "CPU and RAM showed no system pressure.",
+                 "Use training diagnostics for model-level bottlenecks.", (long long)a.n,
+                 Obj().kv("level", jstr("cluster")).done());
+  }
+
+  // ---- SystemSummaryAgg and PerGPUSummary (model.py:50-117, loader.py:97-156)
+  S agg = Obj().kv("first_ts", jopt_num(a.first_ts, have)).kv("last_ts", jopt_num(a.last_ts, have))
+      .kv("system_samples", jint((long long)a.n))
+      .kv("cpu_avg_percent", jopt_num(a.cpu_avg, have)).kv("cpu_peak_percent", jopt_num(a.cpu_peak, have))
+      .kv("ram_avg_bytes", jopt_num(a.ram_avg, have)).kv("ram_peak_bytes", jopt_num(a.ram_peak, have))
+      .kv("ram_total_bytes", jopt_num(a.ram_total, have))
+      .kv("gpu_available", have ? jbool(a.gpu_available != 0) : JNULL)
+      .kv("gpu_count", jopt_int(a.gpu_count, have))
+      .kv("gpu_util_avg_percent", jopt_num(a.gpu_util_avg, hg)).kv("gpu_util_peak_percent", jopt_num(a.gpu_util_peak, hg))
+      .kv("gpu_mem_avg_bytes", jopt_num(a.gpu_mem_avg, hg)).kv("gpu_mem_peak_bytes", jopt_num(a.gpu_mem_peak, hg))
+      .kv("gpu_temp_avg_c", jopt_num(a.gpu_temp_avg, hg)).kv("gpu_temp_peak_c", jopt_num(a.gpu_temp_peak, hg))
+      .kv("gpu_power_avg_w", jopt_num(a.gpu_power_avg, hg)).kv("gpu_power_peak_w", jopt_num(a.gpu_power_peak, hg))
+      .done();
+  Obj per_gpu;
+  for (int g = 0; g < n_gpus; ++g) {
+    const tml_sys_gpu_agg& q = a.gpu[g];
+    per_gpu.kv(fmt("%d", g).c_str(),
+        Obj().kv("gpu_idx", jint(g)).kv("util_avg_percent", jnum(q.util_avg)).kv("util_peak_percent", jnum(q.util_peak))
+            .kv("mem_avg_bytes", jnum(q.mem_avg)).kv("mem_peak_bytes", jnum(q.mem_peak))
+            .kv("mem_total_bytes", jnum(q.mem_total)).kv("temp_avg_c", jnum(q.temp_avg))
+            .kv("temp_peak_c", jnum(q.temp_peak)).kv("power_avg_w", jnum(q.power_avg))
+            .kv("power_peak_w", jnum(q.power_peak)).kv("power_limit_w", jnum(q.power_limit)).done());
+  }
+  std::vector<S> is;
+  for (const Issue& i : issues) is.push_back(i.json());
+  return emit(Obj().kv("primary", primary).kv("issues", jarr(is)).kv("aggregate", agg)
+                  .kv("per_gpu", per_gpu.done()).done(),
+              json_out, cap);
+}

@@ -12,6 +12,8 @@
 //   K4  k_window_reduce<R>            per-step cross-rank median/max, 16 series
 //   K4b k_bands                       trend band sums
 //   K6  k_proc_reduce                 per-rank process aggregates
+//   K5s k_sys_commit                  576-B host / all-GPU sample into the system ring
+//   K6s k_sys_reduce                  System section window aggregates (one launch)
 //
 // Nothing here is a dense contraction: no tensor-core path.  Every bulk kernel
 // is HBM-bound; accesses are 16-byte vectorised and warp-coalesced, tiles are
@@ -34,6 +36,7 @@
 
 #include "../../include/traceml_b200.h"
 #include "tml_internal.h"
+#include "tml_sys_sum.h"
 
 typedef unsigned long long u64;
 typedef unsigned int u32;
@@ -42,6 +45,7 @@ typedef unsigned char u8;
 static_assert(sizeof(tml_step_record) == 128, "StepRecord must be 128 B");
 static_assert(sizeof(tml_window_row) == 64, "WindowRow must be 64 B");
 static_assert(sizeof(tml_proc_record) == 64, "ProcRecord must be 64 B");
+static_assert(sizeof(tml_sys_gpu) == 32 && sizeof(tml_sys_record) == 576, "SysRecord must be 64 + 16 x 32 B");
 
 #define TML_N_SLOTS 64u      // begin-timestamp slots (regions in flight)
 #define TML_N_EPOCHS 8u      // in-flight accumulator sets (steps in flight)
@@ -383,6 +387,15 @@ __global__ void k_proc_commit(DevState* st, tml_proc_record* ring, u32 slots,
     st->proc_head = seq + 1;
     page->pmirror_head = seq + 1;
   }
+}
+
+// ------------------------------------------------------------------ K5s: system commit
+// The 576-B record is the kernel's argument (grid-constant: read in place, never copied to local
+// memory); one warp stores it into the slot the host counted.  Nothing is written to host memory.
+__global__ void k_sys_commit(tml_sys_record* ring, u32 slots, u64 pos, const __grid_constant__ tml_sys_record r) {
+  const u64* src = reinterpret_cast<const u64*>(&r);
+  u64* dst = reinterpret_cast<u64*>(&ring[pos % slots]);
+  for (int k = threadIdx.x; k < (int)(sizeof(tml_sys_record) / 8); k += 32) dst[k] = src[k];
 }
 
 // ------------------------------------------------------------------ reductions
@@ -1524,6 +1537,210 @@ __global__ void k_finalize_dd(const double* __restrict__ partials, int nblk, int
   if (lane == 0) { out[hi_col] = h; out[lo_col] = l; }
 }
 
+// ------------------------------------------------------------------ K6s: system reduce
+// One launch over the latest n system records (tml_sys_sum.h has the arithmetic contract):
+//   pass A  one thread per record: the writer's per-sample derived GPU columns (sys_derive) and
+//           the sample-level window columns;
+//   pass B  one thread per (record, GPU index), GPU = tid % 16: the per-GPU columns.
+// Each CTA folds its threads in a fixed tree (warp butterfly, then warps in order) into one
+// partial; the last CTA to finish folds the partials in CTA order and writes the finished
+// tml_sys_agg.  Every float sum is a TwoSum double-double until that last fold; integer columns
+// are exact u64 sums.  The result does not depend on which CTA finishes last.
+
+struct SysPartA {
+  double cpu_hi, cpu_lo, cpu_max, ts_min, ts_max;
+  double d_hi[4], d_lo[4], d_max[4];  // derived util / mem / temp / power: avg sums, peaks
+  u64 ram_sum, ram_max, ram_total_max, n, n_gpu;
+  u32 avail, gpu_count, n_gpus, _pad;
+};
+struct SysPartG {
+  double p_hi, p_lo;  // watts
+  u64 n, util_sum, mem_sum, temp_sum, mem_max, mem_total_max;
+  u32 util_max, temp_max, power_max, plimit_max;  // power in mW: mW / 1000.0 is monotone
+};
+
+__device__ __forceinline__ void sysa_init(SysPartA& a) {
+  a.cpu_hi = a.cpu_lo = 0.0; a.cpu_max = -INFINITY; a.ts_min = INFINITY; a.ts_max = -INFINITY;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { a.d_hi[k] = 0.0; a.d_lo[k] = 0.0; a.d_max[k] = -INFINITY; }
+  a.ram_sum = a.ram_max = a.ram_total_max = a.n = a.n_gpu = 0;
+  a.avail = a.gpu_count = a.n_gpus = a._pad = 0;
+}
+__device__ __forceinline__ void sysa_merge(SysPartA& a, const SysPartA& b) {
+  sys_dd_add(a.cpu_hi, a.cpu_lo, b.cpu_hi, b.cpu_lo);
+  a.cpu_max = fmax(a.cpu_max, b.cpu_max); a.ts_min = fmin(a.ts_min, b.ts_min); a.ts_max = fmax(a.ts_max, b.ts_max);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) { sys_dd_add(a.d_hi[k], a.d_lo[k], b.d_hi[k], b.d_lo[k]); a.d_max[k] = fmax(a.d_max[k], b.d_max[k]); }
+  a.ram_sum += b.ram_sum; a.ram_max = max(a.ram_max, b.ram_max); a.ram_total_max = max(a.ram_total_max, b.ram_total_max);
+  a.n += b.n; a.n_gpu += b.n_gpu;
+  a.avail |= b.avail; a.gpu_count = max(a.gpu_count, b.gpu_count); a.n_gpus = max(a.n_gpus, b.n_gpus);
+}
+__device__ __forceinline__ SysPartA sysa_shfl(const SysPartA& a, int m) {
+  SysPartA o;
+  o.cpu_hi = shfl_xor_f64(a.cpu_hi, m); o.cpu_lo = shfl_xor_f64(a.cpu_lo, m); o.cpu_max = shfl_xor_f64(a.cpu_max, m);
+  o.ts_min = shfl_xor_f64(a.ts_min, m); o.ts_max = shfl_xor_f64(a.ts_max, m);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    o.d_hi[k] = shfl_xor_f64(a.d_hi[k], m); o.d_lo[k] = shfl_xor_f64(a.d_lo[k], m); o.d_max[k] = shfl_xor_f64(a.d_max[k], m);
+  }
+  o.ram_sum = __shfl_xor_sync(0xffffffffu, a.ram_sum, m); o.ram_max = __shfl_xor_sync(0xffffffffu, a.ram_max, m);
+  o.ram_total_max = __shfl_xor_sync(0xffffffffu, a.ram_total_max, m);
+  o.n = __shfl_xor_sync(0xffffffffu, a.n, m); o.n_gpu = __shfl_xor_sync(0xffffffffu, a.n_gpu, m);
+  o.avail = __shfl_xor_sync(0xffffffffu, a.avail, m); o.gpu_count = __shfl_xor_sync(0xffffffffu, a.gpu_count, m);
+  o.n_gpus = __shfl_xor_sync(0xffffffffu, a.n_gpus, m); o._pad = 0;
+  return o;
+}
+__device__ __forceinline__ void sysg_init(SysPartG& g) {
+  g.p_hi = g.p_lo = 0.0;
+  g.n = g.util_sum = g.mem_sum = g.temp_sum = g.mem_max = g.mem_total_max = 0;
+  g.util_max = g.temp_max = g.power_max = g.plimit_max = 0;
+}
+__device__ __forceinline__ void sysg_merge(SysPartG& a, const SysPartG& b) {
+  sys_dd_add(a.p_hi, a.p_lo, b.p_hi, b.p_lo);
+  a.n += b.n; a.util_sum += b.util_sum; a.mem_sum += b.mem_sum; a.temp_sum += b.temp_sum;
+  a.mem_max = max(a.mem_max, b.mem_max); a.mem_total_max = max(a.mem_total_max, b.mem_total_max);
+  a.util_max = max(a.util_max, b.util_max); a.temp_max = max(a.temp_max, b.temp_max);
+  a.power_max = max(a.power_max, b.power_max); a.plimit_max = max(a.plimit_max, b.plimit_max);
+}
+
+// partials written by other CTAs of the same launch: L2 loads (never the read-only / L1 path)
+template <class T>
+__device__ __forceinline__ T sys_ld_cg(const T* p) {
+  static_assert(sizeof(T) % 8 == 0, "8-B words");
+  T v;
+  const u64* s = reinterpret_cast<const u64*>(p);
+  u64* d = reinterpret_cast<u64*>(&v);
+#pragma unroll
+  for (int i = 0; i < (int)(sizeof(T) / 8); ++i) d[i] = __ldcg(s + i);
+  return v;
+}
+
+__global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record* __restrict__ ring, u32 slots,
+                                                            u64 first_k, u64 n, SysPartA* pa,
+                                                            SysPartG* pg, unsigned int* ticket,
+                                                            tml_sys_agg* __restrict__ out) {
+  __shared__ SysPartA s_a[SYS_THREADS / 32];
+  __shared__ SysPartG s_g[SYS_THREADS / 32][TML_SYS_MAX_GPUS];
+  __shared__ bool s_last;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // ---- pass A: samples
+  SysPartA a;
+  sysa_init(a);
+  for (u64 i = (u64)blockIdx.x * SYS_THREADS + tid; i < n; i += (u64)gridDim.x * SYS_THREADS) {
+    const tml_sys_record* r = &ring[(first_k + i) % slots];
+    const double ts = __ldg(&r->ts), cpu = __ldg(&r->cpu_pct);
+    const u64 ram = __ldg((const u64*)&r->ram_used), ram_total = __ldg((const u64*)&r->ram_total);
+    const u32 fl = __ldg(&r->flags), gc = __ldg(&r->gpu_count);
+    u32 ng = __ldg(&r->n_gpus);
+    if (ng > TML_SYS_MAX_GPUS) ng = TML_SYS_MAX_GPUS;
+    sys_dd_add(a.cpu_hi, a.cpu_lo, cpu, 0.0);
+    a.cpu_max = fmax(a.cpu_max, cpu); a.ts_min = fmin(a.ts_min, ts); a.ts_max = fmax(a.ts_max, ts);
+    a.ram_sum += ram; a.ram_max = max(a.ram_max, ram); a.ram_total_max = max(a.ram_total_max, ram_total);
+    a.n += 1; a.avail |= (fl & TML_SYS_GPU_AVAILABLE) ? 1u : 0u;
+    a.gpu_count = max(a.gpu_count, gc); a.n_gpus = max(a.n_gpus, ng);
+    if (ng > 0) {
+      double d[8];
+      sys_derive(r->gpu, (int)ng, d);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        sys_dd_add(a.d_hi[k], a.d_lo[k], d[2 * k], 0.0);
+        a.d_max[k] = fmax(a.d_max[k], d[2 * k + 1]);
+      }
+      a.n_gpu += 1;
+    }
+  }
+#pragma unroll
+  for (int m = 16; m >= 1; m >>= 1) {
+    const SysPartA o = sysa_shfl(a, m);
+    sysa_merge(a, o);
+  }
+  if (lane == 0) s_a[warp] = a;
+  // ---- pass B: (sample, GPU index) pairs
+  const u32 gi = tid & (TML_SYS_MAX_GPUS - 1);
+  SysPartG g;
+  sysg_init(g);
+  for (u64 i = (u64)blockIdx.x * (SYS_THREADS / TML_SYS_MAX_GPUS) + (tid >> 4); i < n;
+       i += (u64)gridDim.x * (SYS_THREADS / TML_SYS_MAX_GPUS)) {
+    const tml_sys_record* r = &ring[(first_k + i) % slots];
+    if (gi >= __ldg(&r->n_gpus)) continue;
+    const tml_sys_gpu* e = &r->gpu[gi];
+    const u32 util = __ldg(&e->util), temp = __ldg(&e->temp_c), pw = __ldg(&e->power_mw), pl = __ldg(&e->power_limit_mw);
+    const u64 mu = __ldg((const u64*)&e->mem_used), mt = __ldg((const u64*)&e->mem_total);
+    g.n += 1; g.util_sum += util; g.temp_sum += temp; g.mem_sum += mu;
+    g.util_max = max(g.util_max, util); g.temp_max = max(g.temp_max, temp);
+    g.mem_max = max(g.mem_max, mu); g.mem_total_max = max(g.mem_total_max, mt);
+    g.power_max = max(g.power_max, pw); g.plimit_max = max(g.plimit_max, pl);
+    sys_dd_add(g.p_hi, g.p_lo, (double)pw / 1000.0, 0.0);
+  }
+  {  // lanes l and l ^ 16 hold the same GPU index
+    SysPartG o;
+    o.p_hi = shfl_xor_f64(g.p_hi, 16); o.p_lo = shfl_xor_f64(g.p_lo, 16);
+    o.n = __shfl_xor_sync(0xffffffffu, g.n, 16); o.util_sum = __shfl_xor_sync(0xffffffffu, g.util_sum, 16);
+    o.mem_sum = __shfl_xor_sync(0xffffffffu, g.mem_sum, 16); o.temp_sum = __shfl_xor_sync(0xffffffffu, g.temp_sum, 16);
+    o.mem_max = __shfl_xor_sync(0xffffffffu, g.mem_max, 16);
+    o.mem_total_max = __shfl_xor_sync(0xffffffffu, g.mem_total_max, 16);
+    o.util_max = __shfl_xor_sync(0xffffffffu, g.util_max, 16); o.temp_max = __shfl_xor_sync(0xffffffffu, g.temp_max, 16);
+    o.power_max = __shfl_xor_sync(0xffffffffu, g.power_max, 16);
+    o.plimit_max = __shfl_xor_sync(0xffffffffu, g.plimit_max, 16);
+    sysg_merge(g, o);
+  }
+  if (lane < TML_SYS_MAX_GPUS) s_g[warp][lane] = g;
+  __syncthreads();
+  if (tid == 0) {
+    SysPartA b;
+    sysa_init(b);
+    for (int w = 0; w < SYS_THREADS / 32; ++w) sysa_merge(b, s_a[w]);
+    pa[blockIdx.x] = b;
+  } else if (tid >= 32 && tid < 32 + (int)TML_SYS_MAX_GPUS) {
+    SysPartG b;
+    sysg_init(b);
+    for (int w = 0; w < SYS_THREADS / 32; ++w) sysg_merge(b, s_g[w][tid - 32]);
+    pg[(size_t)blockIdx.x * TML_SYS_MAX_GPUS + (tid - 32)] = b;
+  }
+  // ---- the last CTA folds the partials in CTA order
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  const int nb = (int)gridDim.x;
+  if (tid == 0) {
+    SysPartA b;
+    sysa_init(b);
+    for (int k = 0; k < nb; ++k) sysa_merge(b, sys_ld_cg(pa + k));
+    const double cnt = (double)b.n;
+    out->n = b.n; out->n_gpu = b.n_gpu;
+    out->first_ts = b.ts_min; out->last_ts = b.ts_max;
+    out->cpu_avg = (b.cpu_hi + b.cpu_lo) / cnt; out->cpu_peak = b.cpu_max;
+    out->ram_avg = (double)b.ram_sum / cnt; out->ram_peak = (double)b.ram_max;
+    out->ram_total = (double)b.ram_total_max;
+    const double cg = (double)b.n_gpu;
+    const bool hg = b.n_gpu > 0;
+    out->gpu_util_avg = hg ? (b.d_hi[0] + b.d_lo[0]) / cg : 0.0; out->gpu_util_peak = hg ? b.d_max[0] : 0.0;
+    out->gpu_mem_avg = hg ? (b.d_hi[1] + b.d_lo[1]) / cg : 0.0; out->gpu_mem_peak = hg ? b.d_max[1] : 0.0;
+    out->gpu_temp_avg = hg ? (b.d_hi[2] + b.d_lo[2]) / cg : 0.0; out->gpu_temp_peak = hg ? b.d_max[2] : 0.0;
+    out->gpu_power_avg = hg ? (b.d_hi[3] + b.d_lo[3]) / cg : 0.0; out->gpu_power_peak = hg ? b.d_max[3] : 0.0;
+    out->gpu_available = b.avail; out->gpu_count = b.gpu_count; out->n_gpus = b.n_gpus; out->_pad = 0;
+    *ticket = 0u;  // re-armed for the next launch (every other CTA has taken its ticket)
+  } else if (tid >= 32 && tid < 32 + (int)TML_SYS_MAX_GPUS) {
+    const int gx = tid - 32;
+    SysPartG b;
+    sysg_init(b);
+    for (int k = 0; k < nb; ++k) sysg_merge(b, sys_ld_cg(pg + (size_t)k * TML_SYS_MAX_GPUS + gx));
+    tml_sys_gpu_agg& o = out->gpu[gx];
+    const double cnt = (double)b.n;
+    const bool h = b.n > 0;
+    o.n = b.n;
+    o.util_avg = h ? (double)b.util_sum / cnt : 0.0; o.util_peak = (double)b.util_max;
+    o.mem_avg = h ? (double)b.mem_sum / cnt : 0.0; o.mem_peak = (double)b.mem_max;
+    o.mem_total = (double)b.mem_total_max;
+    o.temp_avg = h ? (double)b.temp_sum / cnt : 0.0; o.temp_peak = (double)b.temp_max;
+    o.power_avg = h ? (b.p_hi + b.p_lo) / cnt : 0.0; o.power_peak = (double)b.power_max / 1000.0;
+    o.power_limit = (double)b.plimit_max / 1000.0;
+  }
+}
+
 // =================================================================== host side
 
 static thread_local char g_err[512] = "";
@@ -1637,6 +1854,19 @@ struct tml_ctx {
   std::unordered_map<std::string, void*> peers;
   void* comb[2] = {nullptr, nullptr};  // live step-combined workspaces, per kind (tml_combined.cuh)
   void* run_ws = nullptr;        // tml_reduce_run's workspace (tml_summary.cpp)
+  // system ring and its reduce (tml_sys_*): allocated by the first commit / load
+  tml_sys_record* d_sring = nullptr;
+  u64 sys_commits = 0;
+  std::mutex sys_mu;
+  void* d_sys_ws = nullptr;         // SysPartA[grid cap] | SysPartG[grid cap][16] | ticket | tml_sys_agg
+  SysPartA* d_sys_pa = nullptr;
+  SysPartG* d_sys_pg = nullptr;
+  unsigned int* d_sys_ticket = nullptr;
+  tml_sys_agg* d_sys_out = nullptr;
+  tml_sys_agg* h_sys_out = nullptr; // pinned: the result's copy lands here
+  cudaEvent_t ev_sys = nullptr;
+  bool sys_pending = false;
+  u64 sys_pending_n = 0;
 };
 
 static void comb_free(tml_ctx* c);
@@ -1832,6 +2062,9 @@ int tml_shutdown(tml_ctx* c) {
   if (c->d_ticket) cudaFree(c->d_ticket);
   cudaFree(c->d_partials); cudaFree(c->d_final); cudaFree(c->d_bandcnt);
   cudaFree(c->d_ppartials); cudaFree(c->d_pfinal);
+  cudaFree(c->d_sring); cudaFree(c->d_sys_ws);
+  if (c->h_sys_out) cudaFreeHost(c->h_sys_out);
+  if (c->ev_sys) cudaEventDestroy(c->ev_sys);
   cudaFreeHost(c->h_stage);
   comb_free(c);
   tml_run_ws_free_(c->run_ws);
@@ -2015,6 +2248,11 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
 uint64_t tml_step_count(tml_ctx* c) { return c ? c->commits : 0; }
 uint64_t tml_launch_count(tml_ctx* c) { return c ? c->launches : 0; }
 uint64_t tml_proc_count(tml_ctx* c) { return c ? c->proc_commits.load() : 0; }
+uint64_t tml_sys_count(tml_ctx* c) {
+  if (!c) return 0;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  return c->sys_commits;
+}
 
 // ---------------------------------------------------------------- sampler side
 
@@ -2142,6 +2380,75 @@ int tml_proc_load(tml_ctx* c, const tml_proc_record* host, uint64_t n, void* str
   return TML_OK;
 }
 
+}  // extern "C"
+
+// the system ring (proc_slots slots, the process ring's retention) and the reduce's workspace
+static int sys_ensure(tml_ctx* c) {
+  if (c->d_sring) return TML_OK;
+  const u64 cap = (u64)c->n_sms * 4ull;  // grid_for's cap
+  const size_t o_pg = cap * sizeof(SysPartA), o_t = o_pg + cap * TML_SYS_MAX_GPUS * sizeof(SysPartG);
+  const size_t o_out = (o_t + sizeof(unsigned int) + 255) & ~(size_t)255;
+  CK(cudaMalloc(&c->d_sys_ws, o_out + sizeof(tml_sys_agg)));
+  char* base = (char*)c->d_sys_ws;
+  c->d_sys_pa = (SysPartA*)base; c->d_sys_pg = (SysPartG*)(base + o_pg);
+  c->d_sys_ticket = (unsigned int*)(base + o_t); c->d_sys_out = (tml_sys_agg*)(base + o_out);
+  CK(cudaMemset(c->d_sys_ticket, 0, sizeof(unsigned int)));
+  CK(cudaHostAlloc(&c->h_sys_out, sizeof(tml_sys_agg), cudaHostAllocDefault));
+  CK(cudaEventCreateWithFlags(&c->ev_sys, cudaEventDisableTiming));
+  CK(cudaMalloc(&c->d_sring, (size_t)c->proc_slots * sizeof(tml_sys_record)));
+  return TML_OK;
+}
+
+extern "C" {
+
+int tml_sys_commit(tml_ctx* c, const tml_sys_record* sample, void* stream) {
+  if (!c || !sample) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  DeviceGuard dg(c);  // the sampler thread is not the training thread
+  {
+    int rc = sys_ensure(c);
+    if (rc != TML_OK) return rc;
+  }
+  k_sys_commit<<<1, 32, 0, (cudaStream_t)stream>>>(c->d_sring, c->proc_slots, c->sys_commits, *sample);
+  c->launches += 1;
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "sys_commit launch: %s", cudaGetErrorString(cudaGetLastError()));
+  c->sys_commits += 1;
+  return TML_OK;
+}
+
+int tml_sys_load(tml_ctx* c, const tml_sys_record* host, uint64_t n, void* stream) {
+  if (!c || (!host && n)) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  DeviceGuard dg(c);
+  {
+    int rc = sys_ensure(c);
+    if (rc != TML_OK) return rc;
+  }
+  int rc = load_span(c->d_sring, c->proc_slots, sizeof(tml_sys_record), c->sys_commits, host, n, (cudaStream_t)stream);
+  if (rc != TML_OK) return rc;
+  c->sys_commits += n;
+  return TML_OK;
+}
+
+int tml_sys_read(tml_ctx* c, tml_sys_record* out, uint32_t max_records, uint32_t* n_out, void* stream) {
+  if (!c || !n_out || (!out && max_records)) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  DeviceGuard dg(c);
+  const u64 total = c->sys_commits;
+  u64 n = total < c->proc_slots ? total : c->proc_slots;
+  if (n > max_records) n = max_records;
+  *n_out = (uint32_t)n;
+  if (n == 0) return TML_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  const u64 first = total - n, pos = first % c->proc_slots;
+  const u64 a = (pos + n <= c->proc_slots) ? n : c->proc_slots - pos;
+  CK(cudaMemcpyAsync(out, c->d_sring + pos, (size_t)a * sizeof(tml_sys_record), cudaMemcpyDeviceToHost, s));
+  if (a < n) CK(cudaMemcpyAsync(out + a, c->d_sring, (size_t)(n - a) * sizeof(tml_sys_record), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return TML_OK;
+}
+
 int tml_ring_reset(tml_ctx* c) {
   if (!c) return TML_ERR_ARG;
   CK(cudaSetDevice(c->device));
@@ -2149,6 +2456,7 @@ int tml_ring_reset(tml_ctx* c) {
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   memset(c->h_page, 0, sizeof(HostPage));
   c->commits = 0; c->proc_commits.store(0); c->next_slot = 0;
+  c->sys_commits = 0;
   c->drain_tail = 0; c->pdrain_tail = 0; c->mirror_copied = 0;
   memset(c->host_dur, 0, sizeof(c->host_dur));
   memset(c->host_calls, 0, sizeof(c->host_calls));
@@ -2905,6 +3213,41 @@ int tml_proc_reduce_collect(tml_ctx* c, tml_proc_agg* out) {
   out->ts_max = f[10]; out->ts_min = -f[11];
   out->max_cores = (u32)f[12];
   out->any_gpu_available = f[13] > 0.5 ? 1u : 0u;
+  return TML_OK;
+}
+
+// K6s: one launch, then the async copy of the finished tml_sys_agg into pinned memory and an event.
+// An empty ring launches nothing (collect then reports n = 0).
+int tml_sys_reduce_launch(tml_ctx* c, uint32_t max_rows, void* stream) {
+  if (!c || max_rows == 0) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  cudaStream_t s = (cudaStream_t)stream;
+  const u64 total = c->sys_commits;
+  u64 n = total < c->proc_slots ? total : c->proc_slots;
+  if (n > max_rows) n = max_rows;
+  c->sys_pending_n = n;
+  c->sys_pending = true;
+  if (n == 0) return TML_OK;
+  CK(cudaSetDevice(c->device));
+  const int grid = grid_for(c, n, SYS_THREADS);
+  k_sys_reduce<<<grid, SYS_THREADS, 0, s>>>(c->d_sring, c->proc_slots, total - n, n, c->d_sys_pa, c->d_sys_pg,
+                                            c->d_sys_ticket, c->d_sys_out);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  CK(cudaMemcpyAsync(c->h_sys_out, c->d_sys_out, sizeof(tml_sys_agg), cudaMemcpyDeviceToHost, s));
+  CK(cudaEventRecord(c->ev_sys, s));
+  return TML_OK;
+}
+
+int tml_sys_reduce_collect(tml_ctx* c, tml_sys_agg* out) {
+  if (!c || !out) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  if (!c->sys_pending) return set_err(TML_ERR_STATE, "tml_sys_reduce_collect without a launch");
+  c->sys_pending = false;
+  memset(out, 0, sizeof(*out));
+  if (c->sys_pending_n == 0) return TML_OK;
+  CK(cudaEventSynchronize(c->ev_sys));  // normally landed already: the build's own wait covered it
+  memcpy(out, c->h_sys_out, sizeof(*out));
   return TML_OK;
 }
 

@@ -93,3 +93,39 @@ extern "C" int tml_xs_host_sum(const double* x, uint64_t n, int planned, double*
   if (slow_rows) *slow_rows = slow;
   return TML_OK;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Host emulation of k_sys_reduce's float sums (tml_sys_sum.h): mode 0 the per-sample CPython
+// restatement, mode 1 the window's double-double through the kernel's tree -- grid-stride
+// threads of nblk CTAs, warp butterfly (lane l merges lane l ^ m, m = 16 .. 1), the eight warps
+// in order, then the CTA partials in order -- rounded once.
+#include "tml_sys_sum.h"
+
+extern "C" int tml_sys_host_sum(const double* x, uint64_t n, uint32_t mode, uint32_t nblk, double* out_sum) {
+  if ((!x && n) || !out_sum || mode > 1) return TML_ERR_ARG;
+  if (mode == 0) { *out_sum = sys_cpython_sum(x, n); return TML_OK; }
+  if (nblk == 0) return TML_ERR_ARG;
+  double gh = 0.0, gl = 0.0;
+  for (uint32_t b = 0; b < nblk; ++b) {
+    double th[SYS_THREADS], tl[SYS_THREADS];
+    for (int t = 0; t < SYS_THREADS; ++t) {
+      th[t] = 0.0; tl[t] = 0.0;
+      for (uint64_t i = (uint64_t)b * SYS_THREADS + t; i < n; i += (uint64_t)nblk * SYS_THREADS)
+        sys_dd_add(th[t], tl[t], x[i], 0.0);
+    }
+    double bh = 0.0, bl = 0.0;
+    for (int w = 0; w < SYS_THREADS / 32; ++w) {
+      double h[32], l[32];
+      for (int k = 0; k < 32; ++k) { h[k] = th[w * 32 + k]; l[k] = tl[w * 32 + k]; }
+      for (int m = 16; m >= 1; m >>= 1) {
+        double nh[32], nl[32];
+        for (int k = 0; k < 32; ++k) { nh[k] = h[k]; nl[k] = l[k]; sys_dd_add(nh[k], nl[k], h[k ^ m], l[k ^ m]); }
+        for (int k = 0; k < 32; ++k) { h[k] = nh[k]; l[k] = nl[k]; }
+      }
+      sys_dd_add(bh, bl, h[0], l[0]);
+    }
+    sys_dd_add(gh, gl, bh, bl);
+  }
+  *out_sum = gh + gl;
+  return TML_OK;
+}

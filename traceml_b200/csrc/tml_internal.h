@@ -31,6 +31,10 @@ int tml_summary_run_(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args
                      tml_reduce_run_out* out, const tml_reduce_run_out* prev, const tml_sections_args* prev_sections,
                      char* prev_json, size_t prev_cap, int* prev_rc);
 
+// tml_sys_reduce_launch on the native driver's side stream (the one the process aggregates use),
+// ordered behind what `stream` holds at the call: SummaryEngine.build runs K6s beside the window pass.
+int tml_sys_reduce_beside_(tml_ctx* c, uint32_t max_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

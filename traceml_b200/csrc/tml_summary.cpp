@@ -885,6 +885,19 @@ extern "C" void tml_run_ws_free_(void* p) {
   delete w;
 }
 
+// K6s beside the window pass: on the driver's side stream, behind what `stream` holds at the call
+// (ring loads, the sampler's commits ordered before the build), so it overlaps the pass instead of
+// sitting in front of it.  An empty system ring launches nothing.  Collected after the build's wait.
+extern "C" int tml_sys_reduce_beside_(tml_ctx* c, uint32_t max_rows, void* stream) {
+  if (!c || max_rows == 0) return TML_ERR_ARG;
+  if (tml_sys_count(c) == 0) return tml_sys_reduce_launch(c, max_rows, stream);
+  RunWs* w = nullptr;
+  CKT(ensure_ws(c, &w));
+  CKC(cudaEventRecord(w->side_gate, (cudaStream_t)stream));
+  CKC(cudaStreamWaitEvent(w->side, w->side_gate, 0));
+  return tml_sys_reduce_launch(c, max_rows, w->side);
+}
+
 extern "C" uint64_t tml_struct_size(const char* name) {
   if (!name) return 0;
 #define TML_SZ(T) if (!strcmp(name, #T)) return sizeof(T)
@@ -894,6 +907,7 @@ extern "C" uint64_t tml_struct_size(const char* name) {
   TML_SZ(tml_kind_result); TML_SZ(tml_reduce_run_out); TML_SZ(tml_combined_info); TML_SZ(tml_combined_align);
   TML_SZ(tml_st_diag_in); TML_SZ(tml_mem_diag_in); TML_SZ(tml_proc_diag_in);
   TML_SZ(tml_layer_record);
+  TML_SZ(tml_sys_gpu); TML_SZ(tml_sys_record); TML_SZ(tml_sys_gpu_agg); TML_SZ(tml_sys_agg); TML_SZ(tml_sys_diag_in);
   TML_SZ(tml_sections_args); TML_SZ(tml_live_phase); TML_SZ(tml_rank_means); TML_SZ(tml_trend_in); TML_SZ(tml_mem_metric_in);
 #undef TML_SZ
   return 0;

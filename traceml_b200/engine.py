@@ -299,6 +299,40 @@ class Engine:
         _abi.check(self._lib.tml_proc_reduce_collect(self._h, C.byref(out)), "tml_proc_reduce_collect")
         return out
 
+    # ---- system ring (host / all-GPU samples of local rank 0): header "SYSTEM"
+    @property
+    def sys_count(self) -> int:
+        return int(self._lib.tml_sys_count(self._h))
+
+    def sys_commit(self, rec: _abi.SysRecord, stream: int = 0) -> None:
+        """One sample into the system ring by a 1-warp kernel on ``stream`` (no host sync)."""
+        _abi.check(self._lib.tml_sys_commit(self._h, C.byref(rec), stream), "tml_sys_commit")
+
+    def load_sys(self, records, stream: int = 0) -> None:
+        """Bulk-append ``_abi.SysRecord`` samples (a ctypes array) from host memory."""
+        self._keep_s = records  # keep alive until the stream is synchronised
+        _abi.check(self._lib.tml_sys_load(self._h, C.addressof(records) if len(records) else None,
+                                          len(records), stream), "tml_sys_load")
+
+    def sys_read(self, max_records: int, stream: int = 0):
+        """The latest min(retained, max_records) samples, oldest first (synchronises ``stream``)."""
+        buf = (_abi.SysRecord * max(1, int(max_records)))()
+        n = C.c_uint32(0)
+        _abi.check(self._lib.tml_sys_read(self._h, buf, int(max_records), C.byref(n), stream), "tml_sys_read")
+        return buf[: n.value]
+
+    def sys_reduce_launch(self, max_rows: int, stream: int = 0) -> None:
+        _abi.check(self._lib.tml_sys_reduce_launch(self._h, int(max_rows), stream), "tml_sys_reduce_launch")
+
+    def sys_reduce_beside(self, max_rows: int, stream: int = 0) -> None:
+        """K6s on the native driver's side stream, behind ``stream``: it overlaps the window pass."""
+        _abi.check(self._lib.tml_sys_reduce_beside_(self._h, int(max_rows), stream), "tml_sys_reduce_beside_")
+
+    def sys_reduce_collect(self) -> _abi.SysAgg:
+        out = _abi.SysAgg()
+        _abi.check(self._lib.tml_sys_reduce_collect(self._h, C.byref(out)), "tml_sys_reduce_collect")
+        return out
+
     def proc_reduce(self, max_rows: int, stream: int = 0) -> _abi.ProcAgg:
         out = _abi.ProcAgg()
         _abi.check(self._lib.tml_proc_reduce(self._h, int(max_rows), stream, C.byref(out)),

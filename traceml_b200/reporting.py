@@ -173,6 +173,38 @@ def to_reference_process(sec: Dict[str, Any], identities: Dict[int, Dict[str, An
     return ProcessSectionData(aggregate=agg, per_global_rank=per), diag
 
 
+def to_reference_system(sec: Dict[str, Any]):
+    """-> (SystemSectionData, DiagnosticResult[SystemDiagnosis]) of the section
+    ``sections.build_system`` made (reporting/sections/system/loader.py:32-36, model.py:50-158,
+    diagnostics/system/api.py:36-44)."""
+    from traceml.diagnostics.common import DiagnosticResult
+    from traceml.diagnostics.system import SystemDiagnosis
+    from traceml.reporting.sections.system.loader import SystemSectionData
+    from traceml.reporting.sections.system.model import (PerGPUSummary, SystemClusterSummary, SystemNodeIdentity,
+                                                         SystemNodeSummary, SystemSummaryAgg)
+
+    nodes = {label: SystemNodeSummary(identity=SystemNodeIdentity(**n["identity"]),
+                                      aggregate=SystemSummaryAgg(**n["aggregate"]),
+                                      per_gpu={int(i): PerGPUSummary(**g) for i, g in sorted(n["per_gpu"].items(),
+                                                                                           key=lambda kv: int(kv[0]))})
+             for label, n in sorted(sec["nodes"].items())}
+    data = SystemSectionData(cluster=SystemClusterSummary(aggregate=SystemSummaryAgg(**sec["aggregate"]), nodes=nodes,
+                                                          expected_nodes=int(sec["expected_nodes"])))
+    p = sec["diagnosis"]["primary"]
+    diag = DiagnosticResult(
+        primary=SystemDiagnosis(severity=p["severity"], status=p["status"], reason=p["reason"], action=p["action"],
+                                kind=p["kind"], samples_used=p["samples_used"], scope=dict(p["scope"])),
+        issues=_issues(sec["diagnosis"]["issues"]))
+    return data, diag
+
+
+def _no_system() -> Dict[str, Any]:
+    """The System section of an engine without a system ring: zero samples (NO_DATA)."""
+    from .sections import build_system
+
+    return build_system(None, {"global_rank": 0, "node_rank": 0})
+
+
 def reference_payloads(res: Dict[str, Any], identities: Dict[int, Dict[str, Any]]) -> Dict[str, Any]:
     """Run the KEPT builders: {section: {"payload": ..., "text": ...}}."""
     from traceml.reporting.sections.process.builder import build_process_payload
@@ -192,6 +224,12 @@ def reference_payloads(res: Dict[str, Any], identities: Dict[int, Dict[str, Any]
     d, g = to_reference_process(res["process"], identities)
     p = build_process_payload(d, g)
     out["process"] = {"payload": p, "text": format_process_section_text(p)}
+    from traceml.reporting.sections.system.builder import build_system_payload
+    from traceml.reporting.sections.system.formatter import format_system_section_text
+
+    d, g = to_reference_system(res["system"] if "system" in res else _no_system())
+    p = build_system_payload(d, g)
+    out["system"] = {"payload": p, "text": format_system_section_text(p)}
     return out
 
 
@@ -200,8 +238,8 @@ def build_final_summary(res: Dict[str, Any], identities: Optional[Dict[int, Dict
     """The final_summary envelope: key set and formats of reporting/final.py:254-267
     (``schema_version 1.2, generated_at`` ISO-8601 UTC, ``duration_s, system, process,
     step_time, step_memory, text``).  With the reference importable the kept builders produce
-    the section payloads and the kept ``final.py`` the combined text; the System section (NVML
-    sampler: out of this path's scope) stays empty."""
+    the section payloads -- System included (``res["system"]``; a result without one counts as
+    zero system samples) -- and the kept ``final.py`` the combined text."""
     from datetime import datetime, timezone
 
     ranks = res["reduce"].ranks if "reduce" in res else []
@@ -213,7 +251,7 @@ def build_final_summary(res: Dict[str, Any], identities: Optional[Dict[int, Dict
         from traceml.reporting import final as ref_final
 
         sec = reference_payloads(res, identities)
-        for k in ("process", "step_time", "step_memory"):
+        for k in ("system", "process", "step_time", "step_memory"):
             env[k] = dict(sec[k]["payload"])
         env["duration_s"] = ref_final._summary_duration_s(env["step_time"], env["process"], env["system"])
         env["text"] = ref_final._build_final_summary_text_from_sections(
@@ -230,6 +268,9 @@ def build_final_summary(res: Dict[str, Any], identities: Optional[Dict[int, Dict
             f"Step Memory: {sm['primary']['status']} -- {sm['primary']['reason']}",
             f"Process: {res['process']['primary']['status']} -- {res['process']['primary']['reason']}",
         ])
+        env["system"] = res["system"] if "system" in res else _no_system()
+        sp = env["system"]["diagnosis"]["primary"]
+        env["text"] += f"\nSystem: {sp['status']} -- {sp['reason']}"
     return env
 
 
@@ -290,4 +331,4 @@ class ReferenceComputerAdapter:
 
 __all__ = ["to_reference_step_combined", "to_reference_step_memory_combined", "ReferenceComputerAdapter",
            "build_final_summary", "reference_payloads", "reference_available", "default_identity",
-           "to_reference_step_time", "to_reference_step_memory", "to_reference_process"]
+           "to_reference_step_time", "to_reference_step_memory", "to_reference_process", "to_reference_system"]

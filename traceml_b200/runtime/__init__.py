@@ -151,6 +151,7 @@ class TraceMLRuntime:
         self.sample_system = (int(os.environ.get("LOCAL_RANK", "0") or 0) == 0) if sample_system is None \
             else bool(sample_system)
         self._sys = None
+        self._sys_stream = None
         self._native = None
         self._stop = threading.Event()
         self._thread: Optional[threading.Thread] = None
@@ -165,6 +166,15 @@ class TraceMLRuntime:
         from ..samplers import ProcessProbe
 
         self._proc = None
+        if self.sample_system and self._sys is None:
+            # NVML / psutil set-up here, not inside a tick: initialising NVML holds the driver for
+            # long enough to stall the native sampler's launches and the training thread's
+            try:
+                from ..samplers import SystemProbe
+
+                self._sys = SystemProbe()
+            except Exception as exc:  # noqa: BLE001 -- samplers never interfere with training
+                print(f"[TraceML] system probe unavailable: {exc}", file=sys.stderr)
         if self.sample_process and self.native_process_hz > 0:
             from ..utils import timing
 
@@ -195,13 +205,21 @@ class TraceMLRuntime:
                 self._proc.sample(eng)
         out = drain_to_wire(eng, ram_total=getattr(self._proc, "ram_total", None))
         out["system"] = []
-        if self.sample_system and self.sinks:
+        if self.sample_system:
+            # with or without sinks (the reference's registry samples regardless): the snapshot goes
+            # into the engine's system ring for the final summary, and its wire row to the sinks
             try:
                 if self._sys is None:
                     from ..samplers import SystemProbe
 
-                    self._sys = SystemProbe()
-                out["system"] = [self._sys.sample()]
+                    self._sys = SystemProbe()  # start() could not make one: try again
+                row, rec = self._sys.snapshot()
+                out["system"] = [row]
+                import torch
+
+                if self._sys_stream is None:
+                    self._sys_stream = torch.cuda.Stream(device=eng.device)  # never the training stream
+                eng.sys_commit(rec, int(self._sys_stream.cuda_stream))
             except Exception as exc:  # noqa: BLE001
                 print(f"[TraceML] system sample failed: {exc}", file=sys.stderr)
         self.steps_seen += len(out["step_time"])

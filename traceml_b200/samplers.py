@@ -261,10 +261,11 @@ class ProcessSampler(_TapSampler):
 
 class SystemProbe:
     """One host / all-GPU snapshot per call: the wire row of ``SystemSample.to_wire``
-    (samplers/system_sampler.py:42-221, samplers/schema/system.py:133-157).  Host-side by nature
-    (psutil + NVML); there is no device-side counterpart, so nothing goes through the ring: the row
-    is handed to the sinks as it is.  NVML failures degrade to CPU/RAM only, a failing GPU yields
-    the reference's zeroed placeholder so that index == GPU id."""
+    (samplers/system_sampler.py:42-221, samplers/schema/system.py:133-157) and the same snapshot
+    as the engine's fixed-size system record (the raw NVML integers; watts are derived from them
+    as ``mW / 1000.0`` exactly where the wire row does it).  Host-side by nature (psutil + NVML).
+    NVML failures degrade to CPU/RAM only, a failing GPU yields the reference's zeroed placeholder
+    so that index == GPU id.  The record keeps the first 16 GPUs of a host."""
 
     def __init__(self):
         import psutil
@@ -276,6 +277,7 @@ class SystemProbe:
         self.gpu_available = False
         self.gpu_count = 0
         self._nvml = None
+        self._handles: Dict[int, Any] = {}
         try:
             psutil.cpu_percent(interval=None)  # warm-up: the first real call must not block
             self.cores = psutil.cpu_count(logical=True) or 0
@@ -292,36 +294,74 @@ class SystemProbe:
         except Exception:
             self._nvml = None
 
-    def _gpus(self) -> List[List[float]]:
+    def _raw_gpus(self) -> List[tuple]:
+        """(util %, mem used, mem total, temp C, power mW, power limit mW) per GPU, as NVML
+        returns them; zeros for a GPU whose query failed."""
         if not self.gpu_available or self._nvml is None:
             return []
         n, out = self._nvml, []
         for i in range(self.gpu_count):
             try:
-                h = n.nvmlDeviceGetHandleByIndex(i)
+                h = self._handles.get(i)
+                if h is None:  # a handle is fixed for the process: looked up once (again after a failure)
+                    h = self._handles[i] = n.nvmlDeviceGetHandleByIndex(i)
                 util = n.nvmlDeviceGetUtilizationRates(h)
                 mem = n.nvmlDeviceGetMemoryInfo(h)
                 temp = n.nvmlDeviceGetTemperature(h, n.NVML_TEMPERATURE_GPU)
-                out.append([float(util.gpu), float(mem.used), float(mem.total), float(temp),
-                            float(n.nvmlDeviceGetPowerUsage(h) / 1000.0),
-                            float(n.nvmlDeviceGetPowerManagementLimit(h) / 1000.0)])
+                out.append((int(util.gpu), int(mem.used), int(mem.total), int(temp),
+                            int(n.nvmlDeviceGetPowerUsage(h)), int(n.nvmlDeviceGetPowerManagementLimit(h))))
             except Exception:
-                out.append([0.0, 0.0, 0.0, 0.0, 0.0, 0.0])
+                out.append((0, 0, 0, 0, 0, 0))
         return out
 
-    def sample(self) -> Dict[str, Any]:
+    def _gpus(self) -> List[List[float]]:
+        return [self._wire_gpu(g) for g in self._raw_gpus()]
+
+    @staticmethod
+    def _wire_gpu(g: tuple) -> List[float]:
+        util, used, total, temp, mw, limit_mw = g
+        return [float(util), float(used), float(total), float(temp), float(mw / 1000.0), float(limit_mw / 1000.0)]
+
+    def snapshot(self):
+        """(wire row, ``_abi.SysRecord``) of one sample: the same numbers twice."""
         self.seq += 1
         try:
             cpu = float(self._psutil.cpu_percent(interval=None))
         except Exception:
             cpu = 0.0
         try:
-            ram_used = float(self._psutil.virtual_memory().used)
+            ram_used = int(self._psutil.virtual_memory().used)
         except Exception:
-            ram_used = 0.0
-        return {"seq": self.seq, "ts": time.time(), "cpu": cpu, "ram_used": ram_used,
-                "ram_total": self.ram_total, "gpu_available": self.gpu_available,
-                "gpu_count": self.gpu_count, "gpus": self._gpus()}
+            ram_used = 0
+        ts = time.time()
+        raw = self._raw_gpus()
+        row = {"seq": self.seq, "ts": ts, "cpu": cpu, "ram_used": float(ram_used),
+               "ram_total": self.ram_total, "gpu_available": self.gpu_available,
+               "gpu_count": self.gpu_count, "gpus": [self._wire_gpu(g) for g in raw]}
+        return row, sys_record(self.seq, ts, cpu, ram_used, int(self.ram_total), self.gpu_available,
+                               self.gpu_count, raw)
+
+    def sample(self) -> Dict[str, Any]:
+        return self.snapshot()[0]
+
+
+def sys_record(seq: int, ts: float, cpu: float, ram_used: int, ram_total: int, gpu_available: bool,
+               gpu_count: int, gpus) -> Any:
+    """The engine's 576-B system record of one snapshot; ``gpus`` = raw NVML integer tuples
+    (util %, mem used, mem total, temp C, power mW, power limit mW), the first 16 kept."""
+    from . import _abi
+
+    r = _abi.SysRecord()
+    r.seq, r.ts, r.cpu_pct, r.ram_used, r.ram_total = int(seq), float(ts), float(cpu), int(ram_used), int(ram_total)
+    r.flags = _abi.SYS_GPU_AVAILABLE if gpu_available else 0
+    r.gpu_count = int(gpu_count)
+    gpus = list(gpus)[: _abi.TML_SYS_MAX_GPUS]
+    r.n_gpus = len(gpus)
+    for i, (util, used, total, temp, mw, limit_mw) in enumerate(gpus):
+        e = r.gpu[i]
+        e.util, e.mem_used, e.mem_total, e.temp_c = int(util), int(used), int(total), int(temp)
+        e.power_mw, e.power_limit_mw = int(mw), int(limit_mw)
+    return r
 
 
 class SystemSampler:
@@ -363,5 +403,5 @@ def build_samplers(engine, rank_zero: Optional[bool] = None) -> List[Any]:
     return out + [ProcessSampler(tap), StepTimeSampler(tap), StepMemorySampler(tap)]
 
 
-__all__ = ["drain_to_wire", "ProcessProbe", "SystemProbe", "TableStore", "RecordTap", "StepTimeSampler",
+__all__ = ["drain_to_wire", "ProcessProbe", "SystemProbe", "sys_record", "TableStore", "RecordTap", "StepTimeSampler",
            "StepMemorySampler", "ProcessSampler", "SystemSampler", "build_samplers", "host_constants"]

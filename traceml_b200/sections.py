@@ -264,12 +264,49 @@ def proc_agg_dict(agg: _abi.ProcAgg, *, ram_total: float, gpu_count: int) -> Dic
     return d
 
 
+# ----------------------------------------------------------------------------- system
+def system_node_label(identity: Dict[str, Any]) -> str:
+    """SystemNodeIdentity.label (reporting/sections/system/loader.py:78-81)."""
+    if identity.get("node_rank") is not None:
+        return str(int(identity["node_rank"]))
+    return str(int(identity.get("global_rank") or 0))
+
+
+def build_system(agg: Optional[_abi.SysAgg], identity: Dict[str, Any]) -> Dict[str, Any]:
+    """The System section of the engine's one node from the K6s aggregates: the cluster aggregate,
+    ``nodes``, ``expected_nodes`` (loader.py:159-167, 300-359) and the diagnosis of the C++ rule
+    engine (``tml_diag_system``).  ``agg`` None or empty: no samples, the reference's NO_DATA."""
+    if agg is None:
+        agg = _abi.SysAgg()
+    label = system_node_label(identity)
+    din = _abi.SysDiagIn()
+    din.node_rank = int(identity["node_rank"]) if identity.get("node_rank") is not None else -1
+    din.node_label = label.encode()[:31]
+    din.agg = agg
+    d = _abi.diag_json("tml_diag_system", din)
+    n = int(agg.n)
+    nodes: Dict[str, Any] = {}
+    expected = 1
+    if n:
+        ident = {"label": label}
+        ident.update({k: identity.get(k) for k in ("node_rank", "hostname", "global_rank", "local_rank",
+                                                   "local_world_size", "world_size")})
+        nodes[label] = {"identity": ident, "aggregate": dict(d["aggregate"]),
+                        "per_gpu": {int(k): v for k, v in d["per_gpu"].items()}}
+        world, lws = identity.get("world_size"), identity.get("local_world_size")
+        if world and lws:
+            expected = max(1, int(math.ceil(float(world) / float(lws))))
+    return {"aggregate": d["aggregate"], "nodes": nodes, "expected_nodes": expected,
+            "diagnosis": {"primary": d["primary"], "issues": d["issues"]}}
+
+
 # ----------------------------------------------------------------------------- driver
 class SummaryEngine:
     """All three sections for the local engines of this process."""
 
     def __init__(self, engines, comm=None, *, exchange: str = "auto",
-                 ram_total: Optional[float] = None, gpu_count: Optional[int] = None, native: bool = True):
+                 ram_total: Optional[float] = None, gpu_count: Optional[int] = None, native: bool = True,
+                 system_identity: Optional[Dict[str, Any]] = None):
         self.reducer = WindowReducer(engines, comm, exchange=exchange, native=native)
         self.engines = list(engines)
         self.comm = self.reducer.comm
@@ -283,6 +320,32 @@ class SummaryEngine:
         self.ram_total = ram_total
         self.gpu_count = gpu_count
         self._unemitted: Optional[_abi.Sections] = None  # the last native build's sections
+        # the System section has one source: the engine of local rank 0 (comm index 0), whose
+        # system ring the sampler fills; its node identity comes from the launcher's environment
+        self.system_identity = system_identity
+        self._ident: Optional[Dict[str, Any]] = None
+        self._no_system: Optional[Dict[str, Any]] = None
+
+    def _system_launch(self, rows: int):
+        """K6s beside the window pass on the engine holding the system ring; None (and nothing
+        launched) when this process has no ring or the ring is empty."""
+        eng = self.engines[0] if self.engines else None
+        if self.comm.index != 0 or not hasattr(eng, "sys_reduce_beside") or eng.sys_count == 0:
+            return None
+        eng.sys_reduce_beside(rows, _stream_of(self.reducer.device))
+        return eng
+
+    def _system_section(self, eng) -> Dict[str, Any]:
+        if self._ident is None:
+            from .reporting import default_identity
+
+            self._ident = self.system_identity or default_identity(
+                0, max(1, int(self.comm.world)) * max(1, len(self.engines)))
+        if eng is None:  # zero samples (NO_DATA): the same section every build
+            if self._no_system is None:
+                self._no_system = build_system(None, self._ident)
+            return self._no_system
+        return build_system(eng.sys_reduce_collect(), self._ident)
 
     def build(self, window: int = 10_000, proc_rows: int = 10_000, *, timings: bool = False) -> Dict[str, Any]:
         import torch
@@ -299,10 +362,12 @@ class SummaryEngine:
             rows = max(1, int(proc_rows))
             w = max(1, int(window))
             prev = self._unemitted
+            seng = self._system_launch(rows)  # K6s beside the window pass; nothing without samples
             o = self.reducer.run_native(w, rows, prev=prev if prev is not None and prev._raw is None else None)
             red = NativeReduceOutput(self.reducer, o, w, rows)
             res = _abi.Sections(src=red._snap, args=_abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0))
             res["reduce"] = red
+            res["system"] = self._system_section(seng)
             self._unemitted = res
             return res
         box: Dict[str, Any] = {}
@@ -319,6 +384,7 @@ class SummaryEngine:
             box["aggs"] = aggs
             box["process"] = build_process(aggs)
 
+        seng = self._system_launch(max(1, int(proc_rows)))
         # the process rules need only the first exchange: they run under the K4 launch
         out = self.reducer.reduce(window, proc_rows=max(1, int(proc_rows)), overlap=_process,
                                   stage_timings=timings)
@@ -333,10 +399,12 @@ class SummaryEngine:
             "step_time": build_step_time(out),
             "step_memory": build_step_memory(out, gpu_total, no_gpu),
             "process": box["process"],
+            "system": self._system_section(seng),
             "reduce": out,
         }
 
 
-__all__ = ["SummaryEngine", "build_step_time", "build_step_memory", "build_process",
+__all__ = ["SummaryEngine", "build_step_time", "build_step_memory", "build_process", "build_system",
+           "system_node_label",
            "proc_agg_dict", "closest_rank_to_median", "step_time_global", "step_time_overview",
            "step_memory_global", "wait_avg_ms"]

@@ -130,6 +130,11 @@ def final_summary(*, timeout_sec: float = 30.0, poll_interval_sec: float = 0.1,
                                            window_rows or summary_window_rows())
     if rank0_only and comm.index != 0:
         return None
+    if distributed and not rank0_only:
+        # one System source (local rank 0 = comm index 0): every rank reports its section
+        box = [res["system"] if comm.index == 0 else None]
+        dist.broadcast_object_list(box, src=0)
+        res["system"] = box[0]
     out = build_final_summary(res)
     root = session_root or os.environ.get("TRACEML_SESSION_ROOT")
     if root and comm.index == 0:

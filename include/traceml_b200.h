@@ -355,9 +355,11 @@ typedef struct tml_proc_agg {
   uint64_t n_gpu;      /* rows carrying GPU metrics                          */
   double ts_min, ts_max;
   double sum_cpu, max_cpu;
-  double sum_rss, max_rss;
-  double sum_used, max_used;
-  double sum_resv, max_resv;
+  /* Byte sums are exact integers, as the reference's AVG sums them (sum_used and
+   * sum_resv over the n_gpu rows); exact while n * (largest value) < 2^64.      */
+  uint64_t sum_rss; double max_rss;
+  uint64_t sum_used; double max_used;
+  uint64_t sum_resv; double max_resv;
   double max_total;
   double max_ratio;    /* MAX(resv / used) over rows with used > 0, else -1  */
   uint32_t max_cores;

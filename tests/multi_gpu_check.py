@@ -112,6 +112,37 @@ def main():
             except AssertionError as exc:
                 failures += 1
                 print(f"[multi_gpu_check] {scenario}: FAILED {exc}")
+    # ---- process aggregates whose byte totals pass 2^53 on every rank (10^4 samples of ~1.8 TiB):
+    # the exact u64 sums must cross every exchange intact, native (pack_proc) and Python drivers
+    import process_cases as pc
+
+    P = 10_000
+    steps = replay.make_step_replay("straggler", world, 300, seed=5)[rank]
+    pres = {}
+    for label, mode, native in (("nccl", "nccl", False), ("a2a", "a2a", True), ("a2a_py", "a2a", False),
+                                ("auto", "auto", True)):
+        eng = Engine(device=local, rank=rank, world=world, ring_slots=512, proc_slots=P + 8)
+        eng.load_steps(steps)
+        eng.load_procs(pc.make("bytes_1t8", P, seed=12, rank=rank))
+        torch.cuda.synchronize()
+        se = sections.SummaryEngine([eng], TorchDistComm(), exchange=mode, native=native,
+                                    ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=world)
+        pres[label] = plain(se.build(256, P)["process"])
+        dist.barrier()
+        eng.close()
+    if rank == 0:
+        try:
+            procs_all = {r: pc.make("bytes_1t8", P, seed=12, rank=r) for r in range(world)}
+            pref = process_oracle.process_section(oracle_proc_rows(procs_all, world), max_rows=P)
+            for label, got in pres.items():
+                assert got["aggregate"] == plain(pref["data"]["aggregate"]), f"proc > 2^53 {label}: aggregate"
+                assert got["per_global_rank"] == plain(pref["data"]["per_global_rank"]), f"proc > 2^53 {label}"
+                assert got["primary"] == plain(pref["diagnosis"]["primary"]), f"proc > 2^53 {label}: primary"
+            print(f"[multi_gpu_check] process bytes > 2^53 R={world}: OK ({', '.join(pres)})")
+        except AssertionError as exc:
+            failures += 1
+            print(f"[multi_gpu_check] process bytes > 2^53: FAILED {exc}")
+
     # ---- live tick across the real ranks
     from oracle import live_oracle
     from traceml_b200 import records as rec_mod

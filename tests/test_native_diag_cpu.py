@@ -112,13 +112,13 @@ def _agg_from_records(recs, max_rows):
 
     a.sum_cpu, a.max_cpu = math.fsum(r["cpu_pct"].tolist()), float(r["cpu_pct"].max())
     a.sum_cpu_lo = 0.0
-    rss = r["rss"].astype(np.float64)
-    a.sum_rss, a.max_rss = float(rss.sum()), float(rss.max())
+    # byte sums are exact integers, as K6 gives them (Python ints: no u64 wrap in numpy's sum)
+    a.sum_rss, a.max_rss = sum(int(x) for x in r["rss"]), float(r["rss"].max())
     if a.n_gpu:
         used = r["mem_alloc"][has].astype(np.float64)
         resv = r["mem_resv"][has].astype(np.float64)
-        a.sum_used, a.max_used = float(used.sum()), float(used.max())
-        a.sum_resv, a.max_resv = float(resv.sum()), float(resv.max())
+        a.sum_used, a.max_used = sum(int(x) for x in r["mem_alloc"][has]), float(used.max())
+        a.sum_resv, a.max_resv = sum(int(x) for x in r["mem_resv"][has]), float(resv.max())
         a.max_total = float(r["mem_total"][has].max())
         pos = used > 0
         a.max_ratio = float((resv[pos] / used[pos]).max()) if pos.any() else -1.0

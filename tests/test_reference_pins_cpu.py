@@ -547,10 +547,11 @@ def _native_proc(ranks, ram_total=1000.0, gpu_count=1):
         a.n_gpu = n if v.get("gpu", True) else 0
         a.ts_min, a.ts_max = 0.0, 10.0
         a.sum_cpu, a.max_cpu, a.sum_cpu_lo = v.get("cpu_avg", 120.0) * n, v.get("cpu_peak", 200.0), 0.0
-        a.sum_rss, a.max_rss = v.get("rss_avg", 100.0) * n, v.get("rss_peak", 200.0)
+        # byte sums are exact integers (u64), as K6 gives them
+        a.sum_rss, a.max_rss = int(v.get("rss_avg", 100) * n), v.get("rss_peak", 200.0)
         if a.n_gpu:
-            a.sum_used, a.max_used = v.get("used_avg", 100.0) * n, v.get("used_peak", 200.0)
-            a.sum_resv, a.max_resv = v.get("resv_avg", 120.0) * n, v.get("resv_peak", 240.0)
+            a.sum_used, a.max_used = int(v.get("used_avg", 100) * n), v.get("used_peak", 200.0)
+            a.sum_resv, a.max_resv = int(v.get("resv_avg", 120) * n), v.get("resv_peak", 240.0)
             a.max_total = v.get("total", 1000.0)
             a.max_ratio = v.get("overhang", a.max_resv / a.max_used)
         else:

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import operator
 import os
 from typing import Any, Optional
 
@@ -89,10 +90,21 @@ class BandOut(C.Structure):
 
 class ProcAgg(C.Structure):
     _fields_ = [("n", u64), ("n_gpu", u64), ("ts_min", f64), ("ts_max", f64),
-                ("sum_cpu", f64), ("max_cpu", f64), ("sum_rss", f64), ("max_rss", f64),
-                ("sum_used", f64), ("max_used", f64), ("sum_resv", f64), ("max_resv", f64),
+                ("sum_cpu", f64), ("max_cpu", f64), ("sum_rss", u64), ("max_rss", f64),
+                ("sum_used", u64), ("max_used", f64), ("sum_resv", u64), ("max_resv", f64),
                 ("max_total", f64), ("max_ratio", f64), ("max_cores", u32),
                 ("any_gpu_available", u32), ("sum_cpu_lo", f64)]
+    _BYTE_SUMS = frozenset(("sum_rss", "sum_used", "sum_resv"))
+
+    def __setattr__(self, name, value):
+        # The byte sums are exact u64 integers.  A caller may still hand one over as a float (they
+        # were doubles before): it is taken as the nearest integer, exact for any integral value.
+        if name in self._BYTE_SUMS and not isinstance(value, int):
+            try:
+                value = operator.index(value)  # numpy integers, without a detour through float
+            except TypeError:
+                value = int(round(float(value)))
+        super().__setattr__(name, value)
 
 
 TML_SYS_MAX_GPUS = 16

@@ -820,8 +820,12 @@ extern "C" int tml_diag_process(const tml_proc_diag_in* in, char* json_out, size
   for (int i = 0; i < in->n_ranks; ++i) order[i] = i;
   std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return in->ranks[a] < in->ranks[b]; });
   // pooled aggregates (loader.py:56-139): AVG = sum / count over all rows of all ranks
+  // The byte sums pool as exact integers (64 ranks of u64 sums fit in 128 bits) and round once
+  // per average, as the reference's exact integer AVG does; a double accumulator rounds as soon
+  // as the pooled total passes 2^53.
   uint64_t n_all = 0, n_gpu_all = 0;
-  double s_cpu = 0, s_cpu_lo = 0, s_rss = 0, s_used = 0, s_resv = 0;
+  double s_cpu = 0, s_cpu_lo = 0;
+  unsigned __int128 s_rss = 0, s_used = 0, s_resv = 0;
   auto dd_add = [](double& hi, double& lo, double xh, double xl) {  // TwoSum accumulate
     const double s = hi + xh, bp = s - hi;
     const double err = (hi - (s - bp)) + (xh - bp);
@@ -859,9 +863,10 @@ extern "C" int tml_diag_process(const tml_proc_diag_in* in, char* json_out, size
   }
   const bool have = n_all > 0, have_gpu = n_gpu_all > 0;
   const double cpu_avg = have ? (s_cpu + s_cpu_lo) / (double)n_all : 0;
-  const double ram_avg = have ? s_rss / (double)n_all : 0;
-  const double used_avg = have_gpu ? s_used / (double)n_gpu_all : 0;
-  const double resv_avg = have_gpu ? s_resv / (double)n_gpu_all : 0;
+  // (double) of an unsigned __int128 rounds to nearest, like Python's float(int)
+  const double ram_avg = have ? (double)s_rss / (double)n_all : 0;
+  const double used_avg = have_gpu ? (double)s_used / (double)n_gpu_all : 0;
+  const double resv_avg = have_gpu ? (double)s_resv / (double)n_gpu_all : 0;
 
   // ---- signals (context.py:242-340)
   auto frac = [](bool hn, double num, bool hd, double den, double* out) {

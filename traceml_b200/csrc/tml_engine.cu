@@ -1440,10 +1440,16 @@ __global__ void __launch_bounds__(256) k_bands(const __grid_constant__ BandParam
 // cpu sum is therefore carried as an unevaluated double-double (hi, lo) through every
 // level of the reduction (TwoSum), so it rounds to the same double and rank-level
 // tie-breaks on cpu_percent agree with the reference.
+// The byte columns 1-3 are integer sums, exact like the reference's (SQLite sums integers
+// exactly; CPython's compensated sum() of integer-valued floats is the exact sum, correctly
+// rounded).  They are carried as u64 through every level -- the partials hold the u64 bits --
+// and land in tml_proc_agg as u64: a double tree sum rounds once a total passes 2^53.
+// Exact while n * (largest byte value) < 2^64: 10^6 rows of 16 TiB.
 
 #define PR_THREADS 256
 #define PR_COLS 16
 #define PR_MAXMASK (((1u << 14) - 1u) & ~0xFu)
+#define PR_U64MASK 0xEu  // columns 1-3: u64 sums, bit patterns in the double partials
 
 __device__ __forceinline__ void dd_add(double& hi, double& lo, double xh, double xl) {
   const double s = hi + xh;
@@ -1458,6 +1464,7 @@ __global__ void __launch_bounds__(PR_THREADS) k_proc_reduce(const tml_proc_recor
                                                            double* partials) {
   __shared__ double s_part[PR_THREADS / 32][PR_COLS];
   double a[PR_COLS];
+  u64 bsum[3] = {0ull, 0ull, 0ull};  // rss, used, resv: columns 1-3
 #pragma unroll
   for (int k = 0; k < PR_COLS; ++k) a[k] = ((PR_MAXMASK >> k) & 1u) ? -INFINITY : 0.0;
   for (u64 i = (u64)blockIdx.x * PR_THREADS + threadIdx.x; i < n; i += (u64)gridDim.x * PR_THREADS) {
@@ -1465,19 +1472,20 @@ __global__ void __launch_bounds__(PR_THREADS) k_proc_reduce(const tml_proc_recor
     uint4 c0 = __ldg(p), c1 = __ldg(p + 1), c2 = __ldg(p + 2), c3 = __ldg(p + 3);
     const double ts = __longlong_as_double((long long)((u64)c0.z | ((u64)c0.w << 32)));
     const double cpu = __longlong_as_double((long long)((u64)c1.x | ((u64)c1.y << 32)));
-    const double rss = (double)((u64)c1.z | ((u64)c1.w << 32));
-    const double used = (double)((u64)c2.x | ((u64)c2.y << 32));
-    const double resv = (double)((u64)c2.z | ((u64)c2.w << 32));
+    const u64 rss_b = (u64)c1.z | ((u64)c1.w << 32);
+    const u64 used_b = (u64)c2.x | ((u64)c2.y << 32);
+    const u64 resv_b = (u64)c2.z | ((u64)c2.w << 32);
+    const double rss = (double)rss_b, used = (double)used_b, resv = (double)resv_b;
     const double total = (double)((u64)c3.x | ((u64)c3.y << 32));
     const u32 fl = c3.z, cores = c3.w;
     dd_add(a[0], a[15], cpu, 0.0); a[4] = fmax(a[4], cpu);
-    a[1] += rss; a[5] = fmax(a[5], rss);
+    bsum[0] += rss_b; a[5] = fmax(a[5], rss);
     a[10] = fmax(a[10], ts); a[11] = fmax(a[11], -ts);
     a[12] = fmax(a[12], (double)cores);
     a[13] = fmax(a[13], (fl & TML_PROC_GPU_AVAILABLE) ? 1.0 : 0.0);
     if (fl & TML_PROC_HAS_GPU_METRICS) {
-      a[2] += used; a[6] = fmax(a[6], used);
-      a[3] += resv; a[7] = fmax(a[7], resv);
+      bsum[1] += used_b; a[6] = fmax(a[6], used);
+      bsum[2] += resv_b; a[7] = fmax(a[7], resv);
       a[8] = fmax(a[8], total);
       if (used > 0.0) a[9] = fmax(a[9], resv / used);  // loader.py:174-182
       a[14] += 1.0;
@@ -1490,7 +1498,14 @@ __global__ void __launch_bounds__(PR_THREADS) k_proc_reduce(const tml_proc_recor
     dd_add(a[0], a[15], oh, ol);
   }
 #pragma unroll
-  for (int k = 1; k < PR_COLS - 1; ++k) {
+  for (int q = 0; q < 3; ++q) {  // the exact byte sums
+    u64 x = bsum[q];
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) x += __shfl_xor_sync(0xffffffffu, x, m);
+    a[1 + q] = __longlong_as_double((long long)x);
+  }
+#pragma unroll
+  for (int k = 4; k < PR_COLS - 1; ++k) {
     const bool mx = (PR_MAXMASK >> k) & 1u;
     double x = a[k];
 #pragma unroll
@@ -1510,6 +1525,10 @@ __global__ void __launch_bounds__(PR_THREADS) k_proc_reduce(const tml_proc_recor
     for (int w = 0; w < PR_THREADS / 32; ++w) dd_add(h, l, s_part[w][0], s_part[w][15]);
     partials[(size_t)blockIdx.x * PR_COLS + 0] = h;
     partials[(size_t)blockIdx.x * PR_COLS + 15] = l;
+  } else if ((PR_U64MASK >> threadIdx.x) & 1u) {
+    u64 x = 0;
+    for (int w = 0; w < PR_THREADS / 32; ++w) x += (u64)__double_as_longlong(s_part[w][threadIdx.x]);
+    partials[(size_t)blockIdx.x * PR_COLS + threadIdx.x] = __longlong_as_double((long long)x);
   } else if (threadIdx.x < PR_COLS - 1) {
     const bool mx = (PR_MAXMASK >> threadIdx.x) & 1u;
     double x = mx ? -INFINITY : 0.0;
@@ -1522,9 +1541,11 @@ __global__ void __launch_bounds__(PR_THREADS) k_proc_reduce(const tml_proc_recor
 }
 
 // fold the per-CTA (hi, lo) cpu sums with TwoSum -> out[hi_col], out[lo_col]: one warp,
-// lane l folds CTAs l, l+32, ... then a shuffle tree of double-double adds (fixed order)
+// lane l folds CTAs l, l+32, ... then a shuffle tree of double-double adds (fixed order).
+// The columns in u64_mask hold u64 bit patterns: the same warp folds them as exact integer sums.
+// Both kinds of column overwrite what k_finalize (launched before, on the same stream) left there.
 __global__ void k_finalize_dd(const double* __restrict__ partials, int nblk, int ncols, int hi_col,
-                              int lo_col, double* __restrict__ out) {
+                              int lo_col, u32 u64_mask, double* __restrict__ out) {
   const int lane = threadIdx.x & 31;
   double h = 0.0, l = 0.0;
   for (int b = lane; b < nblk; b += 32)
@@ -1535,6 +1556,14 @@ __global__ void k_finalize_dd(const double* __restrict__ partials, int nblk, int
     dd_add(h, l, oh, ol);
   }
   if (lane == 0) { out[hi_col] = h; out[lo_col] = l; }
+  for (int c = 0; c < ncols; ++c) {
+    if (!((u64_mask >> c) & 1u)) continue;
+    u64 x = 0;
+    for (int b = lane; b < nblk; b += 32) x += (u64)__double_as_longlong(partials[(size_t)b * ncols + c]);
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) x += __shfl_xor_sync(0xffffffffu, x, m);
+    if (lane == 0) out[c] = __longlong_as_double((long long)x);
+  }
 }
 
 // ------------------------------------------------------------------ K6s: system reduce
@@ -3179,7 +3208,7 @@ int tml_proc_reduce_launch(tml_ctx* c, uint32_t max_rows, void* stream) {
   CK(cudaPeekAtLastError());
   k_finalize<<<1, 32 * PR_COLS, 0, s>>>(c->d_ppartials, grid, PR_COLS, PR_MAXMASK, c->d_pfinal);
   CK(cudaPeekAtLastError());
-  k_finalize_dd<<<1, 32, 0, s>>>(c->d_ppartials, grid, PR_COLS, 0, 15, c->d_pfinal);
+  k_finalize_dd<<<1, 32, 0, s>>>(c->d_ppartials, grid, PR_COLS, 0, 15, PR_U64MASK, c->d_pfinal);
   CK(cudaPeekAtLastError());
   c->launches += 3;
   CK(cudaMemcpyAsync((char*)c->h_stage + 3072, c->d_pfinal, PR_COLS * sizeof(double),
@@ -3202,12 +3231,14 @@ int tml_proc_reduce_collect(tml_ctx* c, tml_proc_agg* out) {
   CK(cudaEventSynchronize(c->ev_proc));
   double f[PR_COLS];
   memcpy(f, (char*)c->h_stage + 3072, sizeof(f));
+  u64 bsum[3];  // columns 1-3 hold the u64 byte sums
+  memcpy(bsum, f + 1, sizeof(bsum));
   out->n = n;
   out->n_gpu = (u64)f[14];
   out->sum_cpu = f[0]; out->sum_cpu_lo = f[15]; out->max_cpu = f[4];
-  out->sum_rss = f[1]; out->max_rss = f[5];
-  out->sum_used = f[2]; out->max_used = out->n_gpu ? f[6] : 0.0;
-  out->sum_resv = f[3]; out->max_resv = out->n_gpu ? f[7] : 0.0;
+  out->sum_rss = bsum[0]; out->max_rss = f[5];
+  out->sum_used = bsum[1]; out->max_used = out->n_gpu ? f[6] : 0.0;
+  out->sum_resv = bsum[2]; out->max_resv = out->n_gpu ? f[7] : 0.0;
   out->max_total = out->n_gpu ? f[8] : 0.0;
   out->max_ratio = (f[9] > -INFINITY) ? f[9] : -1.0;
   out->ts_max = f[10]; out->ts_min = -f[11];

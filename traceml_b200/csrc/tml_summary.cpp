@@ -276,7 +276,7 @@ struct Run {
 };
 
 // ------------------------------------------------------------------ packing
-constexpr int INFO_LEN = 23, PROC_LEN = 17, ALIGN_LEN = 15, HANDLE_LEN = 9;  // 72-byte handle = 9 doubles
+constexpr int INFO_LEN = 23, PROC_LEN = 20, ALIGN_LEN = 15, HANDLE_LEN = 9;  // 72-byte handle = 9 doubles
 
 void pack_info(const tml_win_info& i, double* v) {
   int k = 0;
@@ -303,20 +303,24 @@ void unpack_info(const double* v, tml_win_info* i) {
   i->t_count = (u64)llround(v[k++]); i->n_both = (u64)llround(v[k++]);
   for (int q = 0; q < 2; ++q) i->dense[q] = (u32)llround(v[k++]);
 }
+// The u64 byte sums travel as two 32-bit halves, each exact in a double (reduce.py's
+// _proc_pack / _proc_unpack use the same layout).
 void pack_proc(const tml_proc_agg& a, double* v) {
   int k = 0;
+  auto u64_halves = [&](u64 x) { v[k++] = (double)(x & 0xffffffffull); v[k++] = (double)(x >> 32); };
   v[k++] = (double)a.n; v[k++] = (double)a.n_gpu; v[k++] = a.ts_min; v[k++] = a.ts_max;
-  v[k++] = a.sum_cpu; v[k++] = a.max_cpu; v[k++] = a.sum_rss; v[k++] = a.max_rss;
-  v[k++] = a.sum_used; v[k++] = a.max_used; v[k++] = a.sum_resv; v[k++] = a.max_resv;
+  v[k++] = a.sum_cpu; v[k++] = a.max_cpu; u64_halves(a.sum_rss); v[k++] = a.max_rss;
+  u64_halves(a.sum_used); v[k++] = a.max_used; u64_halves(a.sum_resv); v[k++] = a.max_resv;
   v[k++] = a.max_total; v[k++] = a.max_ratio; v[k++] = (double)a.max_cores;
   v[k++] = (double)a.any_gpu_available; v[k++] = a.sum_cpu_lo;
 }
 void unpack_proc(const double* v, tml_proc_agg* a) {
   memset(a, 0, sizeof(*a));
   int k = 0;
+  auto u64_halves = [&]() { const u64 lo = (u64)v[k++]; return lo | ((u64)v[k++] << 32); };
   a->n = (u64)llround(v[k++]); a->n_gpu = (u64)llround(v[k++]); a->ts_min = v[k++]; a->ts_max = v[k++];
-  a->sum_cpu = v[k++]; a->max_cpu = v[k++]; a->sum_rss = v[k++]; a->max_rss = v[k++];
-  a->sum_used = v[k++]; a->max_used = v[k++]; a->sum_resv = v[k++]; a->max_resv = v[k++];
+  a->sum_cpu = v[k++]; a->max_cpu = v[k++]; a->sum_rss = u64_halves(); a->max_rss = v[k++];
+  a->sum_used = u64_halves(); a->max_used = v[k++]; a->sum_resv = u64_halves(); a->max_resv = v[k++];
   a->max_total = v[k++]; a->max_ratio = v[k++]; a->max_cores = (u32)llround(v[k++]);
   a->any_gpu_available = (u32)llround(v[k++]); a->sum_cpu_lo = v[k++];
 }

@@ -37,7 +37,34 @@ _INFO_LEN = 23
 _ALIGN_LEN = 15 + 72  # sums + the 72-byte CUDA-IPC rows handle, one byte per double
 _PROC_FIELDS = tuple(f for f, _ in _abi.ProcAgg._fields_)
 _PROC_INT_FIELDS = ("n", "n_gpu", "max_cores", "any_gpu_available")
-_PROC_LEN = len(_PROC_FIELDS)
+_PROC_U64_FIELDS = ("sum_rss", "sum_used", "sum_resv")  # exact byte sums: two 32-bit halves each
+_PROC_LEN = len(_PROC_FIELDS) + len(_PROC_U64_FIELDS)
+
+
+def _proc_pack(a) -> List[float]:
+    """A ``ProcAgg`` as doubles for the exchange (csrc/tml_summary.cpp pack_proc: same layout).
+    The u64 byte sums go as low and high 32-bit halves, each exact in a double."""
+    v: List[float] = []
+    for f in _PROC_FIELDS:
+        x = getattr(a, f)
+        if f in _PROC_U64_FIELDS:
+            v.extend((float(x & 0xFFFFFFFF), float(x >> 32)))
+        else:
+            v.append(float(x))
+    return v
+
+
+def _proc_unpack(v) -> Dict[str, Any]:
+    pa: Dict[str, Any] = {}
+    k = 0
+    for f in _PROC_FIELDS:
+        if f in _PROC_U64_FIELDS:
+            pa[f] = int(v[k]) | (int(v[k + 1]) << 32)
+            k += 2
+        else:
+            pa[f] = int(round(v[k])) if f in _PROC_INT_FIELDS else v[k]
+            k += 1
+    return pa
 
 # analytics/trends/schema.py:27-62
 _BANDS = ((0.15, 0.25), (0.45, 0.55), (0.90, 1.00))
@@ -355,7 +382,7 @@ class WindowReducer:
             if proc_rows:  # process aggregates (K6) ride in the same exchange
                 a = (eng.proc_reduce_collect() if hasattr(eng, "proc_reduce_collect")
                      else eng.proc_reduce(max(1, int(proc_rows)), stream))
-                flat.extend(float(getattr(a, f)) for f in _PROC_FIELDS)
+                flat.extend(_proc_pack(a))
             if slen:
                 sp = [0.0] * slen
                 if d["dense"][KIND_TIME] and d["n_cand"][KIND_TIME] > 0:
@@ -371,10 +398,7 @@ class WindowReducer:
                 v = row[l * per:(l + 1) * per]
                 infos[p * self.L + l] = self._info_unpack(v[:_INFO_LEN])
                 if proc_rows:
-                    pa = dict(zip(_PROC_FIELDS, v[_INFO_LEN:_INFO_LEN + plen]))
-                    for f in _PROC_INT_FIELDS:
-                        pa[f] = int(round(pa[f]))
-                    proc_aggs[p * self.L + l] = pa
+                    proc_aggs[p * self.L + l] = _proc_unpack(v[_INFO_LEN:_INFO_LEN + plen])
                 srow.extend(v[_INFO_LEN + plen:])
             if spec is not None:
                 spec.append(srow)

@@ -17,10 +17,6 @@ line:
   * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved, the fused pass's
     bytes at W = 4e6), CUDA events, median of 25 after warm-up; the fused pass against it;
   * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
-
-``--alternate N`` runs N rounds of the chained sequence and the three-wait sequence
-(``TML_FUSED_CHAIN=0``), each arm in a child process of its own (the switch is read once per
-process), in ABBA order, and prints every child's line plus a comparison line.
 """
 from __future__ import annotations
 
@@ -34,7 +30,6 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PROC_ROWS = 60_000
-ARMS = {"chain": "1", "three_wait": "0"}
 
 
 def gpu_info(index: int = 0) -> dict:
@@ -195,7 +190,7 @@ def measure(steps: int, window: int, warmup: int) -> dict:
     k3a = med.get("k3a") or 0.0
     fused_gbps = fused_bytes / (k3a * 1e-3) / 1e9 if k3a else None
     return {
-        "chain_env": os.environ.get("TML_FUSED_CHAIN"), "window": W, "steps": steps, "fused_rows": fused,
+        "window": W, "steps": steps, "fused_rows": fused,
         "build_ms": build_ms, "build_wall_ms": wall_ms, "launches_per_build": launches,
         "stage_ms": med, "sections_json_ms": sj_ms,
         "python_rest_ms": wall_ms - med.get("total", 0.0) - sj_ms,
@@ -211,58 +206,15 @@ def measure(steps: int, window: int, warmup: int) -> dict:
     }
 
 
-def alternate(args) -> None:
-    runs = {a: [] for a in ARMS}
-    order = list(ARMS)
-    for rnd in range(args.alternate):
-        for arm in (order if rnd % 2 == 0 else order[::-1]):
-            env = dict(os.environ, TML_FUSED_CHAIN=ARMS[arm])
-            cmd = [sys.executable, os.path.abspath(__file__), "--steps", str(args.steps),
-                   "--window", str(args.window), "--warmup", str(args.warmup)]
-            p = subprocess.run(cmd, env=env, capture_output=True, text=True, timeout=1800)
-            if p.returncode != 0:
-                sys.stderr.write(p.stderr[-4000:])
-                raise SystemExit(f"{arm} arm failed in round {rnd} (exit {p.returncode})")
-            line = json.loads(p.stdout.strip().splitlines()[-1])
-            line["arm"], line["round"] = arm, rnd
-            runs[arm].append(line)
-            print(json.dumps(line), flush=True)
-
-    def stats(xs):
-        return {"median": statistics.median(xs), "min": min(xs), "max": max(xs), "spread": max(xs) - min(xs),
-                "all": xs}
-
-    summary = {"compare": {}, "gpu": runs["chain"][0]["gpu"]}
-    for key in ("build_ms", "build_wall_ms", "device_idle_ms"):
-        per = {a: stats([r[key] for r in runs[a]]) for a in ARMS}
-        d = per["three_wait"]["median"] - per["chain"]["median"]
-        summary["compare"][key] = dict(per, saving_ms=d, saving_frac=d / per["three_wait"]["median"],
-                                       beyond_spread=d > max(per["chain"]["spread"], per["three_wait"]["spread"]))
-    summary["stage_ms"] = {a: {k: statistics.median(r["stage_ms"][k] for r in runs[a]) for k in runs[a][0]["stage_ms"]}
-                           for a in ARMS}
-    summary["segments_ms"] = {a: {k: statistics.median(r["segments_ms"][k] for r in runs[a])
-                                  for k in runs[a][0]["segments_ms"]} for a in ARMS}
-    summary["launches_per_build"] = {a: runs[a][0]["launches_per_build"] for a in ARMS}
-    summary["copy_ceiling_GBps"] = statistics.median(r["copy_ceiling"]["GBps"] for a in ARMS for r in runs[a])
-    summary["fused_of_copy_ceiling"] = {a: statistics.median(r["fused_pass"]["of_copy_ceiling"] for r in runs[a])
-                                        for a in ARMS}
-    print(json.dumps(summary), flush=True)
-
-
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--steps", type=int, default=1000, help="K: builds per timed loop")
     ap.add_argument("--window", type=int, default=4_000_000, help="W: step records")
     ap.add_argument("--warmup", type=int, default=10)
-    ap.add_argument("--alternate", type=int, default=0, metavar="N",
-                    help="N rounds of both sequences, each arm in a child process")
     args = ap.parse_args()
     if args.steps < 1 or args.window < 1:
         ap.error("--steps and --window must be at least 1")
-    if args.alternate > 0:
-        alternate(args)
-    else:
-        print(json.dumps(measure(args.steps, args.window, args.warmup)), flush=True)
+    print(json.dumps(measure(args.steps, args.window, args.warmup)), flush=True)
 
 
 if __name__ == "__main__":

@@ -118,3 +118,25 @@ def strip_device(diag):
             if isinstance(v, dict):
                 v.pop("device", None)
     return diag
+
+
+def build_vs_row_oracles(eng, recs, W, proc_rows=None):
+    """One native single-rank build of ``eng`` (which retains ``recs``) with window ``W``; its
+    step-time and step-memory sections must equal the row-level oracles'.  Returns the build."""
+    from oracle import step_memory_oracle, step_time_oracle
+    from traceml_b200 import sections
+
+    got = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1).build(W, proc_rows or W)
+    o = step_time_oracle.step_time_section(oracle_time_rows({0: recs}, W), max_rows=W)
+    g = got["step_time"]
+    assert_struct(plain(g["data"]), plain({k: o["data"][k] for k in g["data"]}), "data")
+    assert_struct(plain(g["diagnosis"]), plain(o["diagnosis"]), "diagnosis")
+    for k in ("average", "median", "worst"):
+        assert_struct(plain(g["global"][k]), plain(o["global"][k]), f"global.{k}")
+    mo = step_memory_oracle.step_memory_section(oracle_mem_rows({0: recs}), window_size=W,
+                                                gpu_total_bytes=got["step_memory"]["gpu_total_bytes"])
+    gd, od = strip_device(plain(got["step_memory"]["diagnosis"])), strip_device(plain(mo["diagnosis"]))
+    assert_struct(gd["primary"], od["primary"], "mem.primary")
+    assert_struct(gd["issues"], od["issues"], "mem.issues")
+    assert_struct(plain(got["step_memory"]["per_global_rank"]), plain(mo["per_global_rank"]), "mem.rows")
+    return got

@@ -27,7 +27,7 @@ import pytest
 import torch
 
 import series_geometry as sg
-from helpers import assert_struct, oracle_mem_rows, oracle_time_rows, plain, strip_device
+from helpers import build_vs_row_oracles
 
 pytestmark = pytest.mark.gpu
 
@@ -175,27 +175,6 @@ def test_window_pass_geometry(cuda, name, mode):
 
 
 # ----------------------------------------------------------------------------- adversarial acceptance
-def _build_vs_row_oracles(eng, recs, W):
-    import replay
-    from oracle import step_memory_oracle, step_time_oracle
-    from traceml_b200 import sections
-
-    got = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1).build(W, W)
-    o = step_time_oracle.step_time_section(oracle_time_rows({0: recs}, W), max_rows=W)
-    g = got["step_time"]
-    assert_struct(plain(g["data"]), plain({k: o["data"][k] for k in g["data"]}), "data")
-    assert_struct(plain(g["diagnosis"]), plain(o["diagnosis"]), "diagnosis")
-    for k in ("average", "median", "worst"):
-        assert_struct(plain(g["global"][k]), plain(o["global"][k]), f"global.{k}")
-    mo = step_memory_oracle.step_memory_section(oracle_mem_rows({0: recs}), window_size=W,
-                                                gpu_total_bytes=got["step_memory"]["gpu_total_bytes"])
-    gd, od = strip_device(plain(got["step_memory"]["diagnosis"])), strip_device(plain(mo["diagnosis"]))
-    assert_struct(gd["primary"], od["primary"], "mem.primary")
-    assert_struct(gd["issues"], od["issues"], "mem.issues")
-    assert_struct(plain(got["step_memory"]["per_global_rank"]), plain(mo["per_global_rank"]), "mem.rows")
-    return got
-
-
 @pytest.mark.parametrize("no_mem", [False, True], ids=["both_mem", "newer_without_mem"])
 @pytest.mark.parametrize("where", ["tile_edge", "seam", "t_start", "window_head", "window_tail"])
 @pytest.mark.parametrize("name", list(sg.ADVERSARIAL_RINGS))
@@ -218,7 +197,7 @@ def test_duplicate_behind_a_hole_is_never_dense(cuda, name, where, no_mem):
         assert _counters(info) == _restated(c)
         assert guard and ser.tobytes() == _expected_series(recs, W).tobytes()
         assert _counters(eng.win_prepare(W)) == _restated(c)
-        _build_vs_row_oracles(eng, recs, W)
+        build_vs_row_oracles(eng, recs, W)
     finally:
         eng.close()
 
@@ -279,7 +258,7 @@ def test_repeated_step_after_unusable_row(cuda, name, label):
         assert _counters(info) == _restated(sg.window_counters(recs, W, rule="fused"))
         assert ser.tobytes() == _expected_series(recs, W).tobytes()
         assert _counters(eng.win_prepare(W)) == _restated(c)
-        got = _build_vs_row_oracles(eng, recs, W)
+        got = build_vs_row_oracles(eng, recs, W)
         assert got["step_time"]["data"]["aligned_window"]["steps_analyzed"] == c["n_cand"][0]
     finally:
         eng.close()

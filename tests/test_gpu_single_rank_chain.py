@@ -1,33 +1,30 @@
-"""GPU: the chained single-rank build gives what the three-wait sequence gives.
+"""GPU: the single-rank build against the oracles.
 
 With one rank and a bulk window, ``tml_reduce_run`` submits the fused window pass (which finalises
 itself), the band sums and the process aggregates as one device submission with one copy and one
-wait.  ``TML_FUSED_CHAIN=0`` keeps the older sequence (pass + k_finalize, wait; process aggregates,
-wait; bands, wait).  The switch is read once per process, so each arm runs in a child process of its
-own and the two are compared byte for byte: the sections' JSON text and the per-step series.
+wait; a window that is not dense, or not above 2^17 rows, takes the staged path.  Every case builds
+once with the native driver and checks the per-step series bit for bit against
+``oracle.fast_oracle.series16`` over the aligned window, the step-time and step-memory sections
+against the row-level oracles, and the kernels launched per build.
 
-In one process (chained arm): builds that alternate with the staged path, which shares nothing
-with the chained pass's accumulator, and a ring reset + reload must repeat their results exactly.
+In one process: builds that alternate with the staged path, which shares nothing with the chained
+pass's accumulator, and a ring reset + reload must repeat their results exactly.
 """
-import json
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from helpers import build_vs_row_oracles
 
-# name: (scenario, steps, window, ring slots or None, process samples or None, fused expected)
+# name: (scenario, steps, window, ring slots or None, process samples or None, fused expected,
+#        kernels launched per build)
 CASES = {
-    "dense": ("balanced", 300_000, 300_000, None, None, True),
-    "straggler": ("input_straggler", 450_000, 300_000, None, None, True),
-    "wrapped": ("balanced", 400_000, 400_000, 250_000, None, True),
-    "duplicates": ("duplicates", 200_000, 200_000, None, None, False),   # not dense: staged fallback
-    "below": ("balanced", 100_000, 100_000, None, None, False),          # below the bulk threshold
-    "with_procs": ("balanced", 300_000, 300_000, None, 60_000, True),    # the process join on the device
-    "nonmonotone": ("balanced", 200_000, 200_000, None, None, None),     # step ids decrease: an error
+    "dense": ("balanced", 300_000, 300_000, None, None, True, 2),
+    "straggler": ("input_straggler", 450_000, 300_000, None, None, True, 2),
+    "wrapped": ("balanced", 400_000, 400_000, 250_000, None, True, 2),
+    "duplicates": ("duplicates", 200_000, 200_000, None, None, False, 22),   # not dense: staged fallback
+    "below": ("balanced", 100_000, 100_000, None, None, False, 9),           # below the bulk threshold
+    "with_procs": ("balanced", 300_000, 300_000, None, 60_000, True, 5),     # the process join on the device
+    "nonmonotone": ("balanced", 200_000, 200_000, None, None, None, None),   # step ids decrease: an error
 }
 PROC_SLOTS = 65_536
 
@@ -47,7 +44,7 @@ def _engine(name):
     import torch
     from traceml_b200.engine import Engine
 
-    scenario, S, W, ring, procs, _ = CASES[name]
+    scenario, S, W, ring, procs, _, _ = CASES[name]
     eng = Engine(device=0, rank=0, world=1, ring_slots=ring or (S + 8), proc_slots=PROC_SLOTS)
     if procs:
         eng.load_procs(replay.make_proc_replay("normal", 1, procs, seed=5)[0])
@@ -67,43 +64,18 @@ def _build(eng, W, proc_rows):
             bool(red.fused_rows))
 
 
-def _child(name, out_dir):
-    """Runs in a child process: one case under whatever TML_FUSED_CHAIN says, written to out_dir."""
-    import torch
+def _aligned_rows(recs, W):
+    """One rank's aligned windows as WindowRows in step order: time (the oldest usable row of each step
+    id among the last W rows) and memory (the newest row with memory of each step id, newest W ids)."""
+    from oracle import fast_oracle as fo
 
-    torch.cuda.set_device(0)
-    _, S, W, _, procs, _ = CASES[name]
-    eng = _engine(name)
-    meta = {"error": None}
-    try:
-        l0 = eng.launch_count
-        raw, ser, mser, fused = _build(eng, W, procs or W)
-        meta.update(launches=eng.launch_count - l0, fused=fused)
-        with open(os.path.join(out_dir, "raw.json"), "wb") as fh:
-            fh.write(raw)
-        np.save(os.path.join(out_dir, "time.npy"), ser)
-        np.save(os.path.join(out_dir, "mem.npy"), mser)
-    except Exception as exc:  # noqa: BLE001 -- the error itself is the result
-        meta["error"] = f"{type(exc).__name__}: {exc}"
-    finally:
-        eng.close()
-    with open(os.path.join(out_dir, "meta.json"), "w") as fh:
-        json.dump(meta, fh)
-
-
-def _run_arm(name, chain, tmp_path):
-    out = tmp_path / f"{name}_{chain}"
-    out.mkdir()
-    env = dict(os.environ, TML_FUSED_CHAIN=chain)
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__), name, str(out)]
-    p = subprocess.run(cmd, env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, p.stderr[-3000:]
-    with open(out / "meta.json") as fh:
-        meta = json.load(fh)
-    if meta["error"] is not None:
-        return meta, None, None, None
-    raw = (out / "raw.json").read_bytes()
-    return meta, raw, np.load(out / "time.npy"), np.load(out / "mem.npy")
+    win = recs[-W:]
+    rows = fo.window_rows(win)
+    usable = np.nonzero((rows[:, [fo.C_DL, fo.C_FWD, fo.C_BWD, fo.C_OPT, fo.C_WALL]] > 0).any(axis=1))[0]
+    _, first = np.unique(win["step"][usable], return_index=True)
+    mem = recs[(recs["flags"] & fo.FLAG_HAS_MEM) != 0]
+    _, last = np.unique(mem["step"][::-1], return_index=True)
+    return rows[usable[first]][-W:], fo.window_rows(mem[len(mem) - 1 - last])[-W:]
 
 
 @pytest.fixture(scope="module")
@@ -118,23 +90,34 @@ def cuda():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
-def test_chain_matches_three_wait_sequence(cuda, tmp_path, name):
-    fused = CASES[name][5]
-    m1, raw1, t1, g1 = _run_arm(name, "1", tmp_path)
-    m0, raw0, t0, g0 = _run_arm(name, "0", tmp_path)
-    if fused is None:  # a ring whose step ids decrease: the same error from both sequences
-        assert m1["error"] is not None and "step ids decrease" in m1["error"], m1
-        assert m1["error"] == m0["error"]
-        return
-    assert m1["error"] is None and m0["error"] is None, (m1, m0)
-    assert m1["fused"] == m0["fused"] == fused
-    assert raw1 == raw0
-    assert t1.tobytes() == t0.tobytes() and t1.shape == t0.shape
-    assert g1.tobytes() == g0.tobytes() and g1.shape == g0.shape
-    if fused:  # the k_finalize launch behind the pass is gone, nothing else
-        assert m0["launches"] - m1["launches"] == 1, (m0, m1)
-    else:
-        assert m0["launches"] == m1["launches"], (m0, m1)
+def test_single_rank_build_vs_oracles(cuda, name):
+    from oracle import fast_oracle
+    from traceml_b200 import _abi
+
+    scenario, S, W, ring, procs, fused, launches = CASES[name]
+    eng = _engine(name)
+    try:
+        if fused is None:  # a ring whose step ids decrease (one place)
+            with pytest.raises(_abi.TraceMLNativeError, match=r"step ids decrease.*\(1 places\)"):
+                _build(eng, W, W)
+            return
+        retained = _records(scenario, S)[-(ring or S + 8):]
+        l0 = eng.launch_count
+        got = build_vs_row_oracles(eng, retained, W, procs or W)
+        assert eng.launch_count - l0 == launches
+        red = got["reduce"]
+        assert red.fused_rows == fused
+        t_rows, m_rows = _aligned_rows(retained, W)
+        # one K4 pass serves both sections when their aligned windows cover the same steps: the
+        # memory series then comes from the time window's rows
+        exp_t = fast_oracle.series16(t_rows[None])
+        exp_m = fast_oracle.series16((t_rows if red.fused_pass else m_rows)[None])
+        t = red.time.series.cpu().numpy()
+        m = red.mem.series.cpu().numpy()
+        assert t.shape == exp_t.shape and t[:12].tobytes() == exp_t[:12].tobytes()
+        assert m.shape == exp_m.shape and m[12:16].tobytes() == exp_m[12:16].tobytes()
+    finally:
+        eng.close()
 
 
 @pytest.mark.gpu
@@ -142,9 +125,7 @@ def test_chain_interleaved_with_staged_and_reset(cuda):
     import replay
     from traceml_b200 import sections
 
-    if os.environ.get("TML_FUSED_CHAIN", "1").startswith("0"):
-        pytest.skip("the chained sequence is switched off in this process")
-    _, S, W, _, procs, _ = CASES["with_procs"]
+    _, S, W, _, procs, _, _ = CASES["with_procs"]
     eng = _engine("with_procs")
     try:
         first = _build(eng, W, procs)
@@ -170,9 +151,3 @@ def test_chain_interleaved_with_staged_and_reset(cuda):
         assert reloaded[1].tobytes() == first[1].tobytes() and reloaded[2].tobytes() == first[2].tobytes()
     finally:
         eng.close()
-
-
-if __name__ == "__main__":
-    sys.path.insert(0, ROOT)
-    sys.path.insert(0, os.path.join(ROOT, "tests"))
-    _child(sys.argv[1], sys.argv[2])

@@ -5,17 +5,16 @@
 - K6s (k_sys_reduce) equals oracle/system_oracle.py with ``==`` on every aggregate field, for every
   golden stream and for n = 1, 31, 32, 33, 10^4 + 1 over a wrapped ring and 10^5; its labels equal
   the goldens';
-- the single-rank chained build with system samples: the section is the same with
-  ``TML_FUSED_CHAIN=0`` (child processes: the switch is read once per process) and from the Python
-  driver; back-to-back builds repeat it bit for bit; K6s is exactly one more launch when samples
-  exist and none when they do not;
+- the single-rank chained build with system samples: the section equals the oracle's and the Python
+  driver's; back-to-back builds repeat it bit for bit; the other three sections are the same as
+  before the samples were loaded; K6s is exactly one more launch when samples exist and none when
+  they do not;
 - a real training loop with ``TraceMLRuntime(sample_system=True)`` and the compatibility SQLite
   sink: final_summary()'s System payload equals the reference's ``SystemSummarySection`` over the
   database the same rows went to.
 """
 import json
 import os
-import subprocess
 import sys
 
 import pytest
@@ -168,66 +167,43 @@ def test_k_sys_reduce_equals_oracle_at_edges(cuda, n, G, slots, rows, adv):
 W_BULK, S_BULK = 300_000, 300_000
 
 
-def _child(chain_dir):
-    """Runs in a child process under whatever TML_FUSED_CHAIN says."""
+def test_chained_build_with_system_samples(cuda):
     import torch
 
     import replay
+    from oracle import system_oracle
     from traceml_b200 import sections
     from traceml_b200.engine import Engine
 
-    torch.cuda.set_device(0)
     eng = Engine(device=0, rank=0, world=1, ring_slots=S_BULK + 8, proc_slots=65_536)
-    eng.load_steps(replay.make_step_replay("balanced", 1, S_BULK, seed=77)[0])
-    eng.load_procs(replay.make_proc_replay("normal", 1, 20_000, seed=5)[0])
-    torch.cuda.synchronize()
-    out = {}
-    se = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1,
-                                system_identity=sc.IDENTITY)
-    l0 = eng.launch_count
-    res = se.build(W_BULK, 10_000)
-    out["launches_empty"] = eng.launch_count - l0
-    out["system_empty"] = res["system"]
-    raw = sc.random_raw(12_000, 8, seed=11, adversarial=True)
-    eng.load_sys(sc.sys_records(raw))
-    torch.cuda.synchronize()
-    l0 = eng.launch_count
-    res = se.build(W_BULK, 10_000)
-    out["launches_sys"] = eng.launch_count - l0
-    out["system"] = res["system"]
-    out["fused"] = bool(res["reduce"].fused_rows)
-    out["raw"] = res.raw.decode()
-    out["repeat"] = [se.build(W_BULK, 10_000)["system"] for _ in range(2)]
-    py = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1,
-                                system_identity=sc.IDENTITY, native=False).build(W_BULK, 10_000)
-    out["python_driver"] = py["system"]
-    eng.close()
-    with open(os.path.join(chain_dir, "out.json"), "w") as fh:
-        json.dump(out, fh)
-
-
-def _run_arm(chain, tmp_path):
-    out = tmp_path / f"chain_{chain}"
-    out.mkdir()
-    env = dict(os.environ, TML_FUSED_CHAIN=chain)
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__), str(out)]
-    p = subprocess.run(cmd, env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, p.stderr[-3000:]
-    return json.loads((out / "out.json").read_text())
-
-
-def test_chained_build_with_system_samples(cuda, tmp_path):
-    from oracle import system_oracle
-
-    a1, a0 = _run_arm("1", tmp_path), _run_arm("0", tmp_path)
-    assert a1["fused"] and a0["fused"]
-    assert a1["system_empty"]["diagnosis"]["primary"]["kind"] == "NO_DATA"
-    assert a1["launches_sys"] - a1["launches_empty"] == 1 and a0["launches_sys"] - a0["launches_empty"] == 1
-    assert a1["system"] == a0["system"] == a1["python_driver"] == a1["repeat"][0] == a1["repeat"][1]
-    assert a1["raw"] == a0["raw"]  # the other three sections are untouched
-    raw = sc.random_raw(12_000, 8, seed=11, adversarial=True)
+    try:
+        eng.load_steps(replay.make_step_replay("balanced", 1, S_BULK, seed=77)[0])
+        eng.load_procs(replay.make_proc_replay("normal", 1, 20_000, seed=5)[0])
+        torch.cuda.synchronize()
+        se = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1,
+                                    system_identity=sc.IDENTITY)
+        l0 = eng.launch_count
+        empty = se.build(W_BULK, 10_000)
+        launches_empty = eng.launch_count - l0
+        assert empty["system"]["diagnosis"]["primary"]["kind"] == "NO_DATA"
+        raw_empty = bytes(empty.raw)
+        raw = sc.random_raw(12_000, 8, seed=11, adversarial=True)
+        eng.load_sys(sc.sys_records(raw))
+        torch.cuda.synchronize()
+        l0 = eng.launch_count
+        res = se.build(W_BULK, 10_000)
+        assert eng.launch_count - l0 - launches_empty == 1
+        assert res["reduce"].fused_rows
+        assert bytes(res.raw) == raw_empty  # the other three sections are untouched
+        system = res["system"]
+        repeat = [se.build(W_BULK, 10_000)["system"] for _ in range(2)]
+        py = sections.SummaryEngine([eng], ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=1,
+                                    system_identity=sc.IDENTITY, native=False).build(W_BULK, 10_000)
+        assert system == py["system"] == repeat[0] == repeat[1]
+    finally:
+        eng.close()
     want = system_oracle.system_section([sc.wire_row(s) for s in raw[-10_000:]], sc.IDENTITY, 10_000)
-    got = json.loads(json.dumps(a1["system"]))
+    got = json.loads(json.dumps(system))
     assert got["aggregate"] == json.loads(json.dumps(want["aggregate"]))
     assert got["diagnosis"] == json.loads(json.dumps(want["diagnosis"]))
 
@@ -299,7 +275,3 @@ def test_training_loop_system_payload_equals_reference_section(cuda, tmp_path):
 
     assert format_system_section_text(mine["system"]) == want.text
 
-
-if __name__ == "__main__":  # child process of test_chained_build_with_system_samples
-    sys.path.insert(0, ROOT)
-    _child(sys.argv[1])

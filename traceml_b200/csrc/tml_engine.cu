@@ -117,7 +117,7 @@ static_assert(sizeof(WinAcc) == WINACC_WORDS * sizeof(u64), "WinAcc is re-armed 
 
 // The chained single-rank build (tml_win_fused_chain_launch_ / _finish_): everything the host
 // reads back, packed so that ONE device-to-host copy fetches it.  Bands and tails have slots of
-// their own: nothing here is shared with the staged path's d_final / d_partials.
+// their own: nothing here is shared with the staged path's results or d_partials.
 struct ChainOut {
   double fin[16];       // k_finalize's columns of k_window_fused: 7 tree sums, 2 byte sums, 2 maxima
   WinAcc acc;           // the pass's integer side results
@@ -797,8 +797,8 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // oldest row of its step id in the window: the two rules differ only where a step id repeats, and
 // such a window is never dense under either.  The host accepts the series only
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
-// otherwise it falls back to the staged path.  In the chained build the extra CTAs of the
-// k_bands launch behind it fold the partials and hand the accumulator over (k_bands).
+// otherwise it falls back to the staged path.  The extra CTAs of the k_bands launch behind it fold
+// the partials and hand the accumulator over (k_bands).
 #define WF_WARP_U4 (2 * 32 * 8)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
 
@@ -1798,6 +1798,44 @@ extern "C" int tml_set_error_(int code, const char* fmt, ...) {
                      __FILE__, __LINE__);                                                \
   } while (0)
 
+// The window stages' results in device memory (tml_ctx::d_final), one member per stage.
+struct WinFinal {   // tml_win_prepare: fetched whole by one copy
+  double exact[7];  // K3e: the window's sums in reference order
+  double fin[11];   // k_finalize of K3a's partials: 7 tree sums, 2 byte sums, 2 maxima
+  WinAcc acc;       // K3a's integer side results
+};
+struct DevFinal {
+  WinFinal win;
+  double sel_fin[16];    // tml_win_select*: k_finalize of k_gather's partials, layout [q][k]
+  double sel_exact[7];   // ... and K3e's reference-order sums of the aligned rows
+  double band_sum[48];   // tml_win_bands: [series][band]
+  ChainOut chain;        // the chained build's results (one copy)
+  WinAcc chain_acc;      // ... and its pass's accumulator: armed at context creation and re-armed
+                         // by the k_bands launch that reads it, so no host copy sits in front of the pass
+};
+
+// The pinned page the result readbacks land in (tml_ctx::h_stage), one member per readback.  The
+// process aggregates' copy is still in flight while the chained build copies its block, so no two
+// members may share bytes.
+struct StagePage {
+  WinFinal prepare;
+  struct {
+    u64 total;  // k_sel_scan: common steps
+    double fin[16], exact[7];
+    u64 bytes[2];  // k_gather's exact byte sums
+    u64 first_step, last_step;
+    u32 noncontig, first_row;
+  } select;
+  double exact_collect[7];
+  struct {
+    double sum[48];
+    u64 cnt[48];
+    double tail[32];  // [series][first, last]
+  } bands;
+  ChainOut chain;
+  double proc[PR_COLS];
+};
+
 struct tml_ctx {
   int device = 0, rank = 0, world = 1;
   int n_sms = 132;
@@ -1849,7 +1887,6 @@ struct tml_ctx {
   u64 cap_blk = 0;
   u32* d_blockcnt = nullptr;
   u64* d_total = nullptr;
-  WinAcc* d_winacc = nullptr;
   double* d_ppartials = nullptr; // proc reduce partials (own buffers: it overlaps the window reduce)
   double* d_pfinal = nullptr;
   bool proc_pending = false;
@@ -1871,15 +1908,11 @@ struct tml_ctx {
   cudaEvent_t xs_gate = nullptr, xs_done = nullptr;
   bool xs_defer = false, xs_pending = false;
   double* d_partials = nullptr;  // max(grid) * 16 doubles
-  double* d_final = nullptr;     // 64 doubles, then d_winacc, d_chain_out, d_chain_acc
+  DevFinal* d_final = nullptr;
   u64* d_bandcnt = nullptr;
-  ChainOut* d_chain_out = nullptr;  // the chained single-rank build's results (one copy), in d_final's allocation
-  // ... and its pass's own accumulator: armed at context creation and re-armed by the k_bands launch
-  // that reads it, so no host copy sits in front of the pass
-  WinAcc* d_chain_acc = nullptr;
   u64 chain_n = 0, chain_window = 0;    // the chained pass in flight: retained rows, window
   bool chain_pending = false;
-  void* h_stage = nullptr;       // pinned 4 KB result staging
+  StagePage* h_stage = nullptr;  // pinned
   std::unordered_map<std::string, void*> peers;
   void* comb[2] = {nullptr, nullptr};  // live step-combined workspaces, per kind (tml_combined.cuh)
   void* run_ws = nullptr;        // tml_reduce_run's workspace (tml_summary.cpp)
@@ -2049,13 +2082,7 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   CK(cudaMalloc(&c->d_xs_out, 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_xs_stats, 8 * sizeof(u64)));
   CK(cudaMalloc(&c->d_partials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
-  // d_final | K3a's WinAcc (one D2H copy fetches both) | the chained build's ChainOut, accumulator
-  const size_t fin_bytes = 64 * sizeof(double) + sizeof(WinAcc);
-  static_assert((64 * sizeof(double) + sizeof(WinAcc)) % 8 == 0 && sizeof(ChainOut) % 8 == 0, "8-B aligned");
-  CK(cudaMalloc(&c->d_final, fin_bytes + sizeof(ChainOut) + sizeof(WinAcc)));
-  c->d_winacc = reinterpret_cast<WinAcc*>(c->d_final + 64);
-  c->d_chain_out = reinterpret_cast<ChainOut*>((char*)c->d_final + fin_bytes);
-  c->d_chain_acc = reinterpret_cast<WinAcc*>((char*)c->d_final + fin_bytes + sizeof(ChainOut));
+  CK(cudaMalloc(&c->d_final, sizeof(DevFinal)));
   CK(cudaMalloc(&c->d_ppartials, (size_t)c->n_sms * 4 * 16 * sizeof(double)));
   CK(cudaMalloc(&c->d_pfinal, 32 * sizeof(double)));
   CK(cudaMalloc(&c->d_bandcnt, 64 * sizeof(u64)));
@@ -2063,9 +2090,9 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
     WinAcc armed;
     memset(&armed, 0, sizeof(armed));
     armed.lo[0] = armed.lo[1] = ~0ull;
-    CK(cudaMemcpy(c->d_chain_acc, &armed, sizeof(armed), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(&c->d_final->chain_acc, &armed, sizeof(armed), cudaMemcpyHostToDevice));
   }
-  CK(cudaHostAlloc(&c->h_stage, 4096, cudaHostAllocDefault));
+  CK(cudaHostAlloc(&c->h_stage, sizeof(StagePage), cudaHostAllocDefault));
   *out = c;
   return TML_OK;
 }
@@ -2510,6 +2537,68 @@ static int ensure(T** p, u64* cap, u64 need, bool exact_alloc = false) {
   return TML_OK;
 }
 
+// What a window pass (K3a or the fused pass: the same counters, timed between ev0 and ev1) reports
+// from its accumulator and the window's seven sums: n rows retained, the last n_win the time window.
+static int win_info(tml_ctx* c, const WinAcc& acc, const double* t_sums, u64 n, u64 n_win, tml_win_info* out) {
+  memcpy(out->t_sums, t_sums, 7 * sizeof(double));
+  out->latest_step = acc.latest_step;
+  out->monotone = acc.violations == 0 ? 1u : 0u;
+  out->dup_rows = (u32)acc.dups;
+  // dense: every window row is a candidate and the candidates' step ids are consecutive, so
+  // row(step) = first_row + (step - lo) and the aligned rows are a contiguous slice
+  const u64 rows_in[2] = {n_win, n};
+  for (int k = 0; k < 2; ++k) {
+    out->n_rows[k] = acc.nrows[k];
+    out->n_cand[k] = acc.ncand[k];
+    out->lo[k] = acc.ncand[k] ? acc.lo[k] : 0;
+    out->hi[k] = acc.ncand[k] ? acc.hi[k] : 0;
+    out->dense[k] = (acc.ncand[k] > 0 && acc.ncand[k] == rows_in[k] &&
+                     (out->hi[k] - out->lo[k] + 1) == acc.ncand[k]) ? 1u : 0u;
+  }
+  out->t_count = acc.t_count;
+  out->n_both = acc.n_both;
+  float ms = 0.f;
+  if (cudaEventElapsedTime(&ms, c->ev0, c->ev1) == cudaSuccess) out->kernel_ms = (double)ms;
+  if (!out->monotone)
+    return set_err(TML_ERR_NONMONOTONIC, "step ids decrease inside the retained ring (%llu places)", acc.violations);
+  return TML_OK;
+}
+
+// The end of an aligned selection (tml_win_select / _select_dense), after k_gather left its
+// partials: k_finalize, K3e's reference-order sums of `exact` (time window, or nullptr), the copies,
+// one wait, and the sums decoded into `out`.  selected: also fetch what tml_win_select reads back of
+// its k_sel_* / k_check_contig results (first and last step, noncontig, first row).
+static int select_finish(tml_ctx* c, int grid, const XsSrc* exact, bool selected, u64 keep, cudaStream_t s,
+                         tml_align_info* out) {
+  k_finalize<<<1, 32 * 16, 0, s>>>(c->d_partials, grid, 16, (1u << 14) | (1u << 15), c->d_final->sel_fin);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  auto& st = c->h_stage->select;
+  if (exact) {
+    int xr = launch_exact_sums(c, *exact, c->d_final->sel_exact, s);
+    if (xr != TML_OK) return xr;
+    CK(cudaMemcpyAsync(st.exact, c->d_final->sel_exact, sizeof(st.exact), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(st.bytes, c->d_gacc, sizeof(st.bytes), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(st.fin, c->d_final->sel_fin, sizeof(st.fin), cudaMemcpyDeviceToHost, s));
+  if (selected) {
+    CK(cudaMemcpyAsync(&st.first_step, c->d_selstep, sizeof(u64), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&st.last_step, c->d_selstep + (keep - 1), sizeof(u64), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&st.noncontig, c->d_noncontig, sizeof(u32), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&st.first_row, c->d_selrow, sizeof(u32), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  const double* f = st.fin;
+  // partial layout [q][k]: q0 {dl} q1 {fwd,bwd} q2 {opt,cpu,traced,total} q3 {alloc,resv,maxa,maxr}
+  out->t_sums[0] = f[0]; out->t_sums[1] = f[4]; out->t_sums[2] = f[5]; out->t_sums[3] = f[8];
+  out->t_sums[4] = f[9]; out->t_sums[5] = f[10]; out->t_sums[6] = f[11];
+  out->m_sums[0] = (double)st.bytes[0]; out->m_sums[1] = (double)st.bytes[1];  // exact integer sums, rounded once
+  out->m_sums[2] = f[14]; out->m_sums[3] = f[15];
+  if (exact) memcpy(out->t_sums, st.exact, sizeof(st.exact));
+  out->n_rows = keep;
+  return TML_OK;
+}
+
 extern "C" {
 
 int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out) {
@@ -2534,7 +2623,6 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
     c->win_ready = true;
     return TML_OK;
   }
-  int rc;
   u64 cap = c->cap_rows;
   if (n > cap) {
     cudaFree(c->d_rows); cudaFree(c->d_steps); cudaFree(c->d_flags);
@@ -2550,7 +2638,7 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
   WinAcc init;
   memset(&init, 0, sizeof(init));
   init.lo[0] = init.lo[1] = ~0ull;
-  CK(cudaMemcpyAsync(c->d_winacc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(&c->d_final->win.acc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
   static bool wr_attr = false;
   if (!wr_attr) {
     CK(cudaFuncSetAttribute(k_window_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, WR_SMEM_BYTES));
@@ -2577,11 +2665,11 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
   }
   CK(cudaEventRecord(c->ev0, s));
   k_window_rows<<<grid, WR_THREADS, WR_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, c->win_tstart,
-                                            c->d_rows, c->d_steps, c->d_flags, c->d_winacc,
+                                            c->d_rows, c->d_steps, c->d_flags, &c->d_final->win.acc,
                                             c->d_partials, d_csum, (u64)(n - 1 + wsrc.pad));
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
-  k_finalize<<<1, 32 * 11, 0, s>>>(c->d_partials, grid, 11, (1u << 9) | (1u << 10), c->d_final + 32);
+  k_finalize<<<1, 32 * 11, 0, s>>>(c->d_partials, grid, 11, (1u << 9) | (1u << 10), c->d_final->win.fin);
   CK(cudaPeekAtLastError());
   c->launches += 2;  // K3a + its finalize
   if (exact_win && c->xs_defer) {
@@ -2602,54 +2690,25 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
     c->xs_pending = true;
     exact_win = false;
   } else if (exact_win) {  // reference-order sums (used instead of the tree sums)
-    int xr = launch_exact_sums(c, wsrc, c->d_final, s, k3a_csum);
+    int xr = launch_exact_sums(c, wsrc, c->d_final->win.exact, s, k3a_csum);
     if (xr != TML_OK) return xr;
   }
-  // d_final[0..7) exact sums | d_final[32..43) tree sums + maxima | d_final[64..] WinAcc: one copy
-  char* st = (char*)c->h_stage;
-  CK(cudaMemcpyAsync(st + 1024, c->d_final, 64 * sizeof(double) + sizeof(WinAcc), cudaMemcpyDeviceToHost, s));
+  const WinFinal& f = c->h_stage->prepare;
+  CK(cudaMemcpyAsync(&c->h_stage->prepare, &c->d_final->win, sizeof(WinFinal), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  memcpy(st, st + 1024 + 64 * sizeof(double), sizeof(WinAcc));
-  memcpy(st + 256, st + 1024 + (exact_win ? 0 : 32) * sizeof(double), 7 * sizeof(double));
-  memcpy(st + 320, st + 1024 + (32 + 7) * sizeof(double), 4 * sizeof(double));
-  WinAcc acc;
-  memcpy(&acc, st, sizeof(acc));
-  memcpy(out->t_sums, st + 256, 7 * sizeof(double));
-  memcpy(c->win_msums, st + 320, 4 * sizeof(double));
-  c->win_msums[0] = (double)acc.msum[0];  // exact integer sums, rounded once (u64 -> f64 is RN)
-  c->win_msums[1] = (double)acc.msum[1];
+  const int rc = win_info(c, f.acc, exact_win ? f.exact : f.fin, n, n - c->win_tstart, out);
   memcpy(c->win_tsums, out->t_sums, 7 * sizeof(double));
-  out->latest_step = acc.latest_step;
-  out->monotone = acc.violations == 0 ? 1u : 0u;
-  out->dup_rows = (u32)acc.dups;
+  c->win_msums[0] = (double)f.acc.msum[0];  // exact integer sums, rounded once (u64 -> f64 is RN)
+  c->win_msums[1] = (double)f.acc.msum[1];
+  c->win_msums[2] = f.fin[9];
+  c->win_msums[3] = f.fin[10];
   for (int k = 0; k < 2; ++k) {
-    out->n_rows[k] = acc.nrows[k];
-    out->n_cand[k] = acc.ncand[k];
-    out->lo[k] = acc.ncand[k] ? acc.lo[k] : 0;
-    out->hi[k] = acc.ncand[k] ? acc.hi[k] : 0;
-  }
-  out->t_count = acc.t_count;
-  out->n_both = acc.n_both;
-  {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, c->ev0, c->ev1) == cudaSuccess) out->kernel_ms = (double)ms;
-  }
-  c->win_ncand[0] = acc.ncand[0]; c->win_ncand[1] = acc.ncand[1];
-  // dense: every window row is a candidate and the candidates' step ids are consecutive, so
-  // row(step) = first_row + (step - lo) and the aligned rows are a contiguous slice
-  const u64 rows_in[2] = {n - c->win_tstart, n};
-  for (int k = 0; k < 2; ++k) {
+    c->win_ncand[k] = out->n_cand[k];
     c->win_lo[k] = out->lo[k]; c->win_hi[k] = out->hi[k];
-    c->win_dense[k] = acc.ncand[k] > 0 && acc.ncand[k] == rows_in[k] &&
-                      (out->hi[k] - out->lo[k] + 1) == acc.ncand[k];
-    out->dense[k] = c->win_dense[k] ? 1u : 0u;
+    c->win_dense[k] = out->dense[k] != 0;
   }
   c->win_ready = true;
-  (void)rc;
-  if (!out->monotone)
-    return set_err(TML_ERR_NONMONOTONIC, "step ids decrease inside the retained ring (%llu places)",
-                   acc.violations);
-  return TML_OK;
+  return rc;
 }
 
 int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_window) {
@@ -2661,20 +2720,14 @@ int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_
 }
 
 // k_window_fused on stream s over the retained ring's last `window` rows (n > 0), between ev0 and
-// ev1; *grid_out: its CTAs.  chained: into d_chain_acc, always armed, and the caller finalises it
-// (k_bands); otherwise d_winacc is armed by a copy in front and k_finalize runs behind.
-static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, bool chained, int* grid_out) {
+// ev1, into the chained build's accumulator (always armed); *grid_out: its CTAs.  The k_bands launch
+// behind it finalises the pass.
+static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, int* grid_out) {
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
   const u64 t_start = n > window ? n - window : 0;
   const u64 n_win = n - t_start;
   if (c->xs_pending) { CK(cudaStreamWaitEvent(s, c->xs_done, 0)); c->xs_pending = false; }
-  if (!chained) {
-    WinAcc init;
-    memset(&init, 0, sizeof(init));
-    init.lo[0] = init.lo[1] = ~0ull;
-    CK(cudaMemcpyAsync(c->d_winacc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
-  }
   static bool wf_attr = false;
   if (!wf_attr) {
     CK(cudaFuncSetAttribute(k_window_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
@@ -2686,44 +2739,20 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t 
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   CK(cudaEventRecord(c->ev0, s));
   k_window_fused<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
-                                                         chained ? c->d_chain_acc : c->d_winacc, c->d_partials);
+                                                         &c->d_final->chain_acc, c->d_partials);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
   c->launches += 1;
-  if (!chained) {
-    k_finalize<<<1, 32 * 11, 0, s>>>(c->d_partials, grid, 11, (1u << 9) | (1u << 10), c->d_final + 32);
-    CK(cudaPeekAtLastError());
-    c->launches += 1;
-  }
   return TML_OK;
 }
 
-// What tml_win_fused reports once the pass has finished: `acc` its accumulator, f[0..11) its
+// What the chained pass reports once it has finished: `acc` its accumulator, f[0..11) its
 // finalised columns.  *ok = 1 and `aligned` when the window is dense.
 static int fused_result(tml_ctx* c, u64 n, u64 window, const WinAcc& acc, const double* f, tml_win_info* out,
                         tml_align_info* aligned, uint32_t* ok) {
   const u64 n_win = n > window ? window : n;
-  memcpy(out->t_sums, f, 7 * sizeof(double));
-  out->latest_step = acc.latest_step;
-  out->monotone = acc.violations == 0 ? 1u : 0u;
-  out->dup_rows = (u32)acc.dups;
-  const u64 rows_in[2] = {n_win, n};
-  for (int k = 0; k < 2; ++k) {
-    out->n_rows[k] = acc.nrows[k];
-    out->n_cand[k] = acc.ncand[k];
-    out->lo[k] = acc.ncand[k] ? acc.lo[k] : 0;
-    out->hi[k] = acc.ncand[k] ? acc.hi[k] : 0;
-    out->dense[k] = (acc.ncand[k] > 0 && acc.ncand[k] == rows_in[k] &&
-                     (out->hi[k] - out->lo[k] + 1) == acc.ncand[k]) ? 1u : 0u;
-  }
-  out->t_count = acc.t_count;
-  out->n_both = acc.n_both;
-  {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, c->ev0, c->ev1) == cudaSuccess) out->kernel_ms = (double)ms;
-  }
-  if (!out->monotone)
-    return set_err(TML_ERR_NONMONOTONIC, "step ids decrease inside the retained ring (%llu places)", acc.violations);
+  const int rc = win_info(c, acc, f, n, n_win, out);
+  if (rc != TML_OK) return rc;
   // dense in both kinds: the last min(n, W) memory candidates are exactly the time window's rows
   if (out->dense[0] && out->dense[1] && out->hi[0] == out->hi[1] && acc.ncand[0] == n_win) {
     *ok = 1;
@@ -2739,9 +2768,71 @@ static int fused_result(tml_ctx* c, u64 n, u64 window, const WinAcc& acc, const 
   return TML_OK;
 }
 
+// The single-rank bulk pass as one device submission with the band sums chained behind it
+// (tml_internal.h).
+int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
+                                void* stream) {
+  if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
+  if (n == 0) return set_err(TML_ERR_STATE, "chained window pass over an empty ring");
+  c->win_ready = false;
+  c->chain_n = n;
+  c->chain_window = window;
+  c->chain_pending = false;
+  int grid = 0;
+  int rc = fused_pass(c, window, series, s, &grid);
+  if (rc != TML_OK) return rc;
+  // k_bands as tml_win_bands launches it, into the packed block's own slots, plus the row of CTAs
+  // that finishes the pass
+  BandParams p;
+  p.series = series; p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
+  memcpy(p.lo, bands->band_lo, sizeof(p.lo));
+  memcpy(p.hi, bands->band_hi, sizeof(p.hi));
+  memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
+  ChainOut* co = &c->d_final->chain;
+  p.fin_partials = c->d_partials; p.fin_nblk = grid; p.fin_acc = &c->d_final->chain_acc; p.fin_out = co;
+  k_bands<<<dim3(16, 5), 256, 0, s>>>(p, co->band_sum, co->band_cnt, co->tail);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  c->chain_pending = true;
+  return TML_OK;
+}
+
+// The launched chain's results: one copy, one wait.
+static int chain_result(tml_ctx* c, cudaStream_t s, tml_win_info* out, tml_align_info* aligned,
+                        tml_band_out* band_out, uint32_t* ok) {
+  c->chain_pending = false;
+  memset(out, 0, sizeof(*out));
+  memset(aligned, 0, sizeof(*aligned));
+  *ok = 0;
+  out->n_retained = c->chain_n;
+  out->monotone = 1;
+  const ChainOut& r = c->h_stage->chain;
+  CK(cudaMemcpyAsync(&c->h_stage->chain, &c->d_final->chain, sizeof(ChainOut), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  memcpy(band_out->sum, r.band_sum, sizeof(band_out->sum));
+  memcpy(band_out->cnt, r.band_cnt, sizeof(band_out->cnt));
+  for (int k = 0; k < 16; ++k) { band_out->tail_first[k] = r.tail[2 * k]; band_out->tail_last[k] = r.tail[2 * k + 1]; }
+  return fused_result(c, c->chain_n, c->chain_window, r.acc, r.fin, out, aligned, ok);
+}
+
+int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
+                                tml_band_out* band_out, uint32_t* ok) {
+  if (!c || !out || !aligned || !band_out || !ok) return TML_ERR_ARG;
+  if (!c->chain_pending) return set_err(TML_ERR_STATE, "tml_win_fused_chain_finish_ without a launch");
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  // the process aggregates (side stream) land in their own staging slot before the one wait
+  if (c->proc_pending && c->proc_pending_n > 0) CK(cudaStreamWaitEvent(s, c->ev_proc, 0));
+  return chain_result(c, s, out, aligned, band_out, ok);
+}
+
 // Single-rank bulk path: ring -> per-step series in ONE pass (k_window_fused).  *ok = 1: the
 // window is dense and `series` ([16][n_window], device) plus `aligned` hold the result; 0: the
-// caller runs the staged path (tml_win_prepare ...).  Leaves no WindowRows behind.
+// caller runs the staged path (tml_win_prepare ...).  Leaves no WindowRows behind.  The chain with
+// no bands: n_common = 0, so its band and tail CTAs read nothing.
 int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml_win_info* out,
                   tml_align_info* aligned, uint32_t* ok) {
   if (!c || !out || !aligned || !ok || !series || window == 0) return TML_ERR_ARG;
@@ -2755,76 +2846,12 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
   out->n_retained = n;
   out->monotone = 1;
   if (n == 0) return TML_OK;
-  int grid = 0;
-  int rc = fused_pass(c, window, series, s, false, &grid);
+  tml_band_args none;
+  memset(&none, 0, sizeof(none));
+  int rc = tml_win_fused_chain_launch_(c, window, series, &none, stream);
   if (rc != TML_OK) return rc;
-  // d_final[32..43) tree sums + maxima | d_final[64..] WinAcc: one copy
-  char* st = (char*)c->h_stage;
-  CK(cudaMemcpyAsync(st + 1024, c->d_final, 64 * sizeof(double) + sizeof(WinAcc), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  WinAcc acc;
-  memcpy(&acc, st + 1024 + 64 * sizeof(double), sizeof(acc));
-  double f[11];
-  memcpy(f, st + 1024 + 32 * sizeof(double), sizeof(f));
-  return fused_result(c, n, window, acc, f, out, aligned, ok);
-}
-
-// The same pass as one device submission with the band sums chained behind it (tml_internal.h).
-int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
-                                void* stream) {
-  if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
-  cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaSetDevice(c->device));
-  const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
-  if (n == 0) return set_err(TML_ERR_STATE, "chained window pass over an empty ring");
-  c->win_ready = false;
-  c->chain_n = n;
-  c->chain_window = window;
-  c->chain_pending = false;
-  int grid = 0;
-  int rc = fused_pass(c, window, series, s, true, &grid);
-  if (rc != TML_OK) return rc;
-  // k_bands as tml_win_bands launches it, into the packed block's own slots, plus the row of CTAs
-  // that finishes the pass
-  BandParams p;
-  p.series = series; p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
-  memcpy(p.lo, bands->band_lo, sizeof(p.lo));
-  memcpy(p.hi, bands->band_hi, sizeof(p.hi));
-  memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
-  p.fin_partials = c->d_partials; p.fin_nblk = grid; p.fin_acc = c->d_chain_acc; p.fin_out = c->d_chain_out;
-  char* co = (char*)c->d_chain_out;
-  k_bands<<<dim3(16, 5), 256, 0, s>>>(p, (double*)(co + offsetof(ChainOut, band_sum)),
-                                      (u64*)(co + offsetof(ChainOut, band_cnt)), (double*)(co + offsetof(ChainOut, tail)));
-  CK(cudaPeekAtLastError());
-  c->launches += 1;
-  c->chain_pending = true;
-  return TML_OK;
-}
-
-int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
-                                tml_band_out* band_out, uint32_t* ok) {
-  if (!c || !out || !aligned || !band_out || !ok) return TML_ERR_ARG;
-  if (!c->chain_pending) return set_err(TML_ERR_STATE, "tml_win_fused_chain_finish_ without a launch");
-  c->chain_pending = false;
-  cudaStream_t s = (cudaStream_t)stream;
-  CK(cudaSetDevice(c->device));
-  memset(out, 0, sizeof(*out));
-  memset(aligned, 0, sizeof(*aligned));
-  *ok = 0;
-  out->n_retained = c->chain_n;
-  out->monotone = 1;
-  // the process aggregates (side stream) land in their own staging slot before the one wait
-  if (c->proc_pending && c->proc_pending_n > 0) CK(cudaStreamWaitEvent(s, c->ev_proc, 0));
-  char* st = (char*)c->h_stage + 1024;
-  static_assert(1024 + sizeof(ChainOut) <= 3072, "the packed block must stay clear of the process slot");
-  CK(cudaMemcpyAsync(st, c->d_chain_out, sizeof(ChainOut), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  ChainOut r;
-  memcpy(&r, st, sizeof(r));
-  memcpy(band_out->sum, r.band_sum, sizeof(band_out->sum));
-  memcpy(band_out->cnt, r.band_cnt, sizeof(band_out->cnt));
-  for (int k = 0; k < 16; ++k) { band_out->tail_first[k] = r.tail[2 * k]; band_out->tail_last[k] = r.tail[2 * k + 1]; }
-  return fused_result(c, c->chain_n, c->chain_window, r.acc, r.fin, out, aligned, ok);
+  tml_band_out dropped;
+  return chain_result(c, s, out, aligned, &dropped, ok);
 }
 
 int tml_win_set_defer(tml_ctx* c, int on) {
@@ -2840,10 +2867,10 @@ int tml_win_exact_collect(tml_ctx* c, void* stream, double t_sums[7]) {
     cudaStream_t s = (cudaStream_t)stream;
     CK(cudaSetDevice(c->device));
     CK(cudaStreamWaitEvent(s, c->xs_done, 0));
-    char* st = (char*)c->h_stage;
-    CK(cudaMemcpyAsync(st + 448, c->d_xs_out, 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    double* st = c->h_stage->exact_collect;
+    CK(cudaMemcpyAsync(st, c->d_xs_out, 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    memcpy(c->win_tsums, st + 448, 7 * sizeof(double));
+    memcpy(c->win_tsums, st, 7 * sizeof(double));
     c->xs_pending = false;
   }
   memcpy(t_sums, c->win_tsums, 7 * sizeof(double));
@@ -2909,11 +2936,9 @@ int tml_win_select(tml_ctx* c, uint32_t kind, uint64_t glo, uint64_t span, const
                                            glo, c->d_rowof[kind], c->d_selrow, c->d_selstep);
   CK(cudaPeekAtLastError());
   c->launches += 3;
-  char* st = (char*)c->h_stage;
-  CK(cudaMemcpyAsync(st, c->d_total, sizeof(u64), cudaMemcpyDeviceToHost, s));
+  u64& total = c->h_stage->select.total;
+  CK(cudaMemcpyAsync(&total, c->d_total, sizeof(u64), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  u64 total = 0;
-  memcpy(&total, st, sizeof(u64));
   const u64 keep = total < window ? total : window;
   c->n_common[kind] = keep;
   out->n_common = keep;
@@ -2928,48 +2953,18 @@ int tml_win_select(tml_ctx* c, uint32_t kind, uint64_t glo, uint64_t span, const
   k_gather<<<grid, GA_THREADS, 0, s>>>(c->d_rows, c->d_selrow, keep, c->d_xrows[kind], c->d_noncontig,
                                        -1ll, c->d_partials, c->d_gacc);
   CK(cudaPeekAtLastError());
-  c->launches += 1;
-  k_finalize<<<1, 32 * 16, 0, s>>>(c->d_partials, grid, 16, (1u << 14) | (1u << 15), c->d_final);
-  CK(cudaPeekAtLastError());
   c->launches += 2;
   const bool exact = (kind == TML_KIND_TIME) && (c->world > 1 || keep <= TML_EXACT_SUM_MAX);
-  if (exact) {
-    XsSrc x;
-    memset(&x, 0, sizeof(x));
-    x.rows = c->d_rows; x.first = 0; x.last = (long long)keep - 1; x.aligned = 1;
-    x.xrows = c->d_xrows[kind]; x.noncontig = c->d_noncontig; x.sel_rows = c->d_selrow; x.dense_first = -1;
-    int xr = launch_exact_sums(c, x, c->d_final + 16, s);
-    if (xr != TML_OK) return xr;
-    CK(cudaMemcpyAsync(st + 320, c->d_final + 16, 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaMemcpyAsync(st + 400, c->d_gacc, 2 * sizeof(u64), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 64, c->d_final, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 256, c->d_selstep, sizeof(u64), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 264, c->d_selstep + (keep - 1), sizeof(u64), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 272, c->d_noncontig, sizeof(u32), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 276, c->d_selrow, sizeof(u32), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  {
-    u32 noncontig = 0, first_row = 0;
-    memcpy(&noncontig, st + 272, sizeof(u32));
-    memcpy(&first_row, st + 276, sizeof(u32));
-    c->rows_ptr[kind] = noncontig ? c->d_xrows[kind] : (c->d_rows + first_row);
-  }
-  double f[16];
-  memcpy(f, st + 64, sizeof(f));
-  // partial layout [q][k]: q0 {dl} q1 {fwd,bwd} q2 {opt,cpu,traced,total} q3 {alloc,resv,maxa,maxr}
-  out->t_sums[0] = f[0]; out->t_sums[1] = f[4]; out->t_sums[2] = f[5]; out->t_sums[3] = f[8];
-  out->t_sums[4] = f[9]; out->t_sums[5] = f[10]; out->t_sums[6] = f[11];
-  out->m_sums[0] = f[12]; out->m_sums[1] = f[13]; out->m_sums[2] = f[14]; out->m_sums[3] = f[15];
-  {
-    u64 g[2];
-    memcpy(g, st + 400, sizeof(g));
-    out->m_sums[0] = (double)g[0]; out->m_sums[1] = (double)g[1];  // exact integer sums, rounded once
-  }
-  if (exact) memcpy(out->t_sums, st + 320, 7 * sizeof(double));
-  memcpy(&out->start_step, st + 256, sizeof(u64));
-  memcpy(&out->end_step, st + 264, sizeof(u64));
-  out->n_rows = keep;
+  XsSrc x;
+  memset(&x, 0, sizeof(x));
+  x.rows = c->d_rows; x.first = 0; x.last = (long long)keep - 1; x.aligned = 1;
+  x.xrows = c->d_xrows[kind]; x.noncontig = c->d_noncontig; x.sel_rows = c->d_selrow; x.dense_first = -1;
+  rc = select_finish(c, grid, exact ? &x : nullptr, true, keep, s, out);
+  if (rc != TML_OK) return rc;
+  const auto& st = c->h_stage->select;
+  c->rows_ptr[kind] = st.noncontig ? c->d_xrows[kind] : (c->d_rows + st.first_row);
+  out->start_step = st.first_step;
+  out->end_step = st.last_step;
   return TML_OK;
 }
 
@@ -3007,37 +3002,16 @@ int tml_win_select_dense(tml_ctx* c, uint32_t kind, uint64_t first_step, uint64_
   k_gather<<<grid, GA_THREADS, 0, s>>>(c->d_rows, nullptr, n_common, nullptr, c->d_noncontig,
                                        (long long)first_row, c->d_partials, c->d_gacc);
   CK(cudaPeekAtLastError());
-  k_finalize<<<1, 32 * 16, 0, s>>>(c->d_partials, grid, 16, (1u << 14) | (1u << 15), c->d_final);
-  CK(cudaPeekAtLastError());
-  c->launches += 2;
+  c->launches += 1;
   const bool exact = (kind == TML_KIND_TIME) && (c->world > 1 || n_common <= TML_EXACT_SUM_MAX);
-  char* st = (char*)c->h_stage;
-  if (exact) {
-    XsSrc x;
-    memset(&x, 0, sizeof(x));
-    x.rows = c->d_rows; x.first = 0; x.last = (long long)n_common - 1; x.aligned = 1;
-    x.dense_first = (long long)first_row;
-    int xr = launch_exact_sums(c, x, c->d_final + 16, s);
-    if (xr != TML_OK) return xr;
-    CK(cudaMemcpyAsync(st + 320, c->d_final + 16, 7 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaMemcpyAsync(st + 400, c->d_gacc, 2 * sizeof(u64), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 64, c->d_final, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  double f[16];
-  memcpy(f, st + 64, sizeof(f));
-  out->t_sums[0] = f[0]; out->t_sums[1] = f[4]; out->t_sums[2] = f[5]; out->t_sums[3] = f[8];
-  out->t_sums[4] = f[9]; out->t_sums[5] = f[10]; out->t_sums[6] = f[11];
-  out->m_sums[0] = f[12]; out->m_sums[1] = f[13]; out->m_sums[2] = f[14]; out->m_sums[3] = f[15];
-  {
-    u64 g[2];
-    memcpy(g, st + 400, sizeof(g));
-    out->m_sums[0] = (double)g[0]; out->m_sums[1] = (double)g[1];  // exact integer sums, rounded once
-  }
-  if (exact) memcpy(out->t_sums, st + 320, 7 * sizeof(double));
+  XsSrc x;
+  memset(&x, 0, sizeof(x));
+  x.rows = c->d_rows; x.first = 0; x.last = (long long)n_common - 1; x.aligned = 1;
+  x.dense_first = (long long)first_row;
+  const int rc = select_finish(c, grid, exact ? &x : nullptr, false, n_common, s, out);
+  if (rc != TML_OK) return rc;
   out->start_step = first_step;
   out->end_step = first_step + n_common - 1;
-  out->n_rows = n_common;
   return TML_OK;
 }
 
@@ -3171,21 +3145,18 @@ int tml_win_bands(tml_ctx* c, const double* series, const tml_band_args* a, void
   memcpy(p.hi, a->band_hi, sizeof(p.hi));
   memcpy(p.tail_first, a->tail_first, sizeof(p.tail_first));
   p.fin_partials = nullptr; p.fin_nblk = 0; p.fin_acc = nullptr; p.fin_out = nullptr;
-  double* d_sum = c->d_final;            // 48 doubles
   double* d_tail = c->d_partials;        // 32 doubles (scratch)
-  k_bands<<<dim3(16, 4), 256, 0, s>>>(p, d_sum, c->d_bandcnt, d_tail);
+  k_bands<<<dim3(16, 4), 256, 0, s>>>(p, c->d_final->band_sum, c->d_bandcnt, d_tail);
   CK(cudaPeekAtLastError());
   c->launches += 1;
-  char* st = (char*)c->h_stage;
-  CK(cudaMemcpyAsync(st, d_sum, 48 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 512, c->d_bandcnt, 48 * sizeof(u64), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(st + 1024, d_tail, 32 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  auto& st = c->h_stage->bands;
+  CK(cudaMemcpyAsync(st.sum, c->d_final->band_sum, sizeof(st.sum), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(st.cnt, c->d_bandcnt, sizeof(st.cnt), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(st.tail, d_tail, sizeof(st.tail), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  memcpy(out->sum, st, 48 * sizeof(double));
-  memcpy(out->cnt, st + 512, 48 * sizeof(u64));
-  double tails[32];
-  memcpy(tails, st + 1024, sizeof(tails));
-  for (int k = 0; k < 16; ++k) { out->tail_first[k] = tails[2 * k]; out->tail_last[k] = tails[2 * k + 1]; }
+  memcpy(out->sum, st.sum, sizeof(st.sum));
+  memcpy(out->cnt, st.cnt, sizeof(st.cnt));
+  for (int k = 0; k < 16; ++k) { out->tail_first[k] = st.tail[2 * k]; out->tail_last[k] = st.tail[2 * k + 1]; }
   return TML_OK;
 }
 
@@ -3211,8 +3182,7 @@ int tml_proc_reduce_launch(tml_ctx* c, uint32_t max_rows, void* stream) {
   k_finalize_dd<<<1, 32, 0, s>>>(c->d_ppartials, grid, PR_COLS, 0, 15, PR_U64MASK, c->d_pfinal);
   CK(cudaPeekAtLastError());
   c->launches += 3;
-  CK(cudaMemcpyAsync((char*)c->h_stage + 3072, c->d_pfinal, PR_COLS * sizeof(double),
-                     cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(c->h_stage->proc, c->d_pfinal, sizeof(c->h_stage->proc), cudaMemcpyDeviceToHost, s));
   if (!c->ev_proc) CK(cudaEventCreateWithFlags(&c->ev_proc, cudaEventDisableTiming));
   CK(cudaEventRecord(c->ev_proc, s));
   return TML_OK;
@@ -3229,8 +3199,7 @@ int tml_proc_reduce_collect(tml_ctx* c, tml_proc_agg* out) {
   // normally complete already (tml_win_prepare synchronised the stream); an empty step
   // ring returns from there without a sync, so wait on the copy itself
   CK(cudaEventSynchronize(c->ev_proc));
-  double f[PR_COLS];
-  memcpy(f, (char*)c->h_stage + 3072, sizeof(f));
+  const double* f = c->h_stage->proc;
   u64 bsum[3];  // columns 1-3 hold the u64 byte sums
   memcpy(bsum, f + 1, sizeof(bsum));
   out->n = n;

@@ -369,14 +369,6 @@ bool trend_layout(u64 n, u64 min_points, double warmup_frac, u64 lo[3], u64 hi[3
 
 // ------------------------------------------------------------------ the run
 constexpr u64 TML_FUSED_MIN_ROWS = 1u << 17;  // == TML_EXACT_SUM_MAX: below it the staged path gives reference-order sums
-
-// TML_FUSED_CHAIN=0: the single-rank bulk build as three host waits (pass + k_finalize, process
-// aggregates, bands) instead of one chained submission.  An A/B switch, never needed for
-// correctness; read once per process.
-bool fused_chain_enabled() {
-  static const bool on = [] { const char* e = getenv("TML_FUSED_CHAIN"); return !e || e[0] != '0'; }();
-  return on;
-}
 constexpr u64 P2P_MIN_ROWS = 1000000;  // reduce.py: the one-shot IPC mapping pays above this
 
 struct KindState {
@@ -392,8 +384,8 @@ u32 mode_for(const Run& r, u32 exchange, u64 n_common) {
   return TML_XCHG_P2P;
 }
 
-int parse_aligns(Run& r, const double* all, int stride, int off, bool handles, u32 kind,
-                 const tml_win_info* infos, const std::vector<int>& part, KindState* ks) {
+int parse_aligns(Run& r, const double* all, int stride, int off, bool handles, const std::vector<int>& part,
+                 KindState* ks) {
   tml_kind_result* res = ks->res;
   ks->blocks.assign(r.world, Aligned());
   u64 n_common = 0;
@@ -413,7 +405,6 @@ int parse_aligns(Run& r, const double* all, int stride, int off, bool handles, u
     memcpy(res->m_sums[i], a.m_sums, sizeof(a.m_sums));
     res->start_step = a.start; res->end_step = a.end;
   }
-  (void)kind; (void)infos;
   return TML_OK;
 }
 
@@ -457,7 +448,7 @@ int align_kind(Run& r, u32 kind, u32 window, u32 exchange, const tml_win_info* i
     for (int p : part) same_window = same_window && infos[p].lo[kind] == glo && infos[p].hi[kind] == ghi;
     if (same_window) {  // every participant speculated on exactly [glo, ghi]
       ks->from_spec = true;
-      return parse_aligns(r, spec_all, spec_stride, spec_off, spec_handles, kind, infos, part, ks);
+      return parse_aligns(r, spec_all, spec_stride, spec_off, spec_handles, part, ks);
     }
     const u64 n_common = span < window ? span : window;
     CKT(tml_win_select_dense(r.c, kind, ghi - n_common + 1, n_common, r.s, &a));
@@ -471,7 +462,7 @@ int align_kind(Run& r, u32 kind, u32 window, u32 exchange, const tml_win_info* i
   }
   CKT(export_block(r, kind, exchange, a, handles, mine.data()));
   CKT(r.xchg(mine.data(), alen, all.data()));
-  return parse_aligns(r, all.data(), alen, 0, handles, kind, infos, part, ks);
+  return parse_aligns(r, all.data(), alen, 0, handles, part, ks);
 }
 
 int reduce_pass(Run& r, u32 kind, u32 mask, u32 mode, KindState* ks, int series_slot) {
@@ -532,9 +523,6 @@ int reduce_pass(Run& r, u32 kind, u32 mask, u32 mode, KindState* ks, int series_
   return TML_OK;
 }
 
-// `extra` (n_extra doubles per rank, may be 0) rides in the band exchange: the deferred
-// reference-order sums of K3e, so that they cost no exchange of their own.  *extra_done tells the
-// caller whether the exchange happened (no aligned window -> no band exchange).
 // what k_bands is asked for over a series of n columns, of which [shard_lo, shard_hi) are here
 void band_args(u64 n, u64 shard_lo, u64 shard_hi, tml_band_args* a) {
   memset(a, 0, sizeof(*a));
@@ -546,22 +534,9 @@ void band_args(u64 n, u64 shard_lo, u64 shard_hi, tml_band_args* a) {
   a->tail_first[1] = n - (n < 1000 ? n : 1000);
 }
 
-int bands_collect(Run& r, tml_kind_result* res, const tml_band_out& bo, const double* extra, int n_extra,
-                  double* extra_all, bool* extra_done);
-
-int bands(Run& r, tml_kind_result* res, const double* extra = nullptr, int n_extra = 0,
-          double* extra_all = nullptr, bool* extra_done = nullptr) {
-  const u64 n = res->n_common;
-  if (extra_done) *extra_done = false;
-  if (n == 0 || !res->series) return TML_OK;
-  tml_band_args a;
-  band_args(n, res->shard_lo, res->shard_hi, &a);
-  tml_band_out bo;
-  CKT(tml_win_bands(r.c, res->series, &a, r.s, &bo));
-  return bands_collect(r, res, bo, extra, n_extra, extra_all, extra_done);
-}
-
-// the band exchange and its rank-order sums, from this rank's k_bands results
+// the band exchange and its rank-order sums, from this rank's k_bands results.  `extra` (n_extra
+// doubles per rank, may be 0) rides in the band exchange: the deferred reference-order sums of K3e,
+// so that they cost no exchange of their own.
 int bands_collect(Run& r, tml_kind_result* res, const tml_band_out& bo, const double* extra, int n_extra,
                   double* extra_all, bool* extra_done) {
   double vec[128 + 16];
@@ -595,6 +570,29 @@ int bands_collect(Run& r, tml_kind_result* res, const tml_band_out& bo, const do
   }
   res->has_bands = 1;
   return TML_OK;
+}
+
+// k_bands over res's series, then bands_collect.  *extra_done tells the caller whether the exchange
+// happened (no aligned window -> no band exchange).
+int bands(Run& r, tml_kind_result* res, const double* extra = nullptr, int n_extra = 0,
+          double* extra_all = nullptr, bool* extra_done = nullptr) {
+  const u64 n = res->n_common;
+  if (extra_done) *extra_done = false;
+  if (n == 0 || !res->series) return TML_OK;
+  tml_band_args a;
+  band_args(n, res->shard_lo, res->shard_hi, &a);
+  tml_band_out bo;
+  CKT(tml_win_bands(r.c, res->series, &a, r.s, &bo));
+  return bands_collect(r, res, bo, extra, n_extra, extra_all, extra_done);
+}
+
+// the memory section's series is the time section's: so are its bands
+void share_bands(tml_kind_result* mem, const tml_kind_result& time) {
+  memcpy(mem->band_sum, time.band_sum, sizeof(time.band_sum));
+  memcpy(mem->band_cnt, time.band_cnt, sizeof(time.band_cnt));
+  memcpy(mem->tail_first, time.tail_first, sizeof(time.tail_first));
+  memcpy(mem->tail_last, time.tail_last, sizeof(time.tail_last));
+  mem->has_bands = time.has_bands;
 }
 
 double now_ms() {
@@ -644,9 +642,8 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   u64 n_win = 0;
   CKT(tml_win_peek(c, window, nullptr, &n_win));
   const bool bulk = world == 1 && n_win > (u64)TML_FUSED_MIN_ROWS;
-  const bool chain = bulk && fused_chain_enabled();
   if (args->proc_rows) CKC(cudaEventRecord(r.w->side_gate, r.s));
-  if (chain) {
+  if (bulk) {
     // the dense series has n_win columns, so the band layout is known before the pass
     CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
     tml_band_args ba;
@@ -660,20 +657,15 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   const double tl = now_ms();
   // ---- single rank, bulk window: ring -> series in ONE pass (k_window_fused); the WindowRows
   // that K3a would write for K4 to re-read never exist.  Falls through to the staged path when the
-  // window is not dense (re-flushed step ids, rows without memory, ...).  Chained (the default):
-  // pass, bands and process aggregates are one device submission with one copy and one wait.
+  // window is not dense (re-flushed step ids, rows without memory, ...).  Pass, bands and process
+  // aggregates are one device submission with one copy and one wait.
   if (bulk) {
     tml_win_info finfo;
     tml_align_info fal;
     tml_band_out cbo;
     uint32_t ok = 0;
-    if (chain) {
-      if (pre) pre->run();  // the GPU is busy with the pass
-      CKT(tml_win_fused_chain_finish_(c, r.s, &finfo, &fal, &cbo, &ok));
-    } else {
-      CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
-      CKT(tml_win_fused(c, window, r.w->d_series[0], r.s, &finfo, &fal, &ok));
-    }
+    if (pre) pre->run();  // the GPU is busy with the pass
+    CKT(tml_win_fused_chain_finish_(c, r.s, &finfo, &fal, &cbo, &ok));
     if (ok) {
       tml_proc_agg pagg0;
       memset(&pagg0, 0, sizeof(pagg0));
@@ -693,13 +685,8 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
       out->exchange_used = TML_XCHG_LOCAL;
       out->fused_pass = 2;  // 2: K3a and K4 fused as well (no WindowRows)
       const double tf = now_ms();
-      if (chain) CKT(bands_collect(r, &out->time, cbo, nullptr, 0, nullptr, nullptr));
-      else CKT(bands(r, &out->time));
-      memcpy(out->mem.band_sum, out->time.band_sum, sizeof(out->time.band_sum));
-      memcpy(out->mem.band_cnt, out->time.band_cnt, sizeof(out->time.band_cnt));
-      memcpy(out->mem.tail_first, out->time.tail_first, sizeof(out->time.tail_first));
-      memcpy(out->mem.tail_last, out->time.tail_last, sizeof(out->time.tail_last));
-      out->mem.has_bands = out->time.has_bands;
+      CKT(bands_collect(r, &out->time, cbo, nullptr, 0, nullptr, nullptr));
+      share_bands(&out->mem, out->time);
       const double te = now_ms();
       out->n_exchanges = r.n_exchanges;
       out->k3a_ms = finfo.kernel_ms;
@@ -814,15 +801,8 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   bool exact_done = false;
   if (deferred) CKT(tml_win_exact_collect(c, r.s, exact_mine));
   CKT(bands(r, &out->time, deferred ? exact_mine : nullptr, deferred ? 7 : 0, exact_all, &exact_done));
-  if (same) {
-    memcpy(out->mem.band_sum, out->time.band_sum, sizeof(out->time.band_sum));
-    memcpy(out->mem.band_cnt, out->time.band_cnt, sizeof(out->time.band_cnt));
-    memcpy(out->mem.tail_first, out->time.tail_first, sizeof(out->time.tail_first));
-    memcpy(out->mem.tail_last, out->time.tail_last, sizeof(out->time.tail_last));
-    out->mem.has_bands = out->time.has_bands;
-  } else {
-    CKT(bands(r, &out->mem));
-  }
+  if (same) share_bands(&out->mem, out->time);
+  else CKT(bands(r, &out->mem));
   if (deferred) {
     if (!exact_done) CKT(r.xchg(exact_mine, 7, exact_all));  // no aligned window: no band exchange to ride in
     for (int p = 0; p < world; ++p) memcpy(out->infos[p].t_sums, exact_all + (size_t)p * 7, 7 * sizeof(double));

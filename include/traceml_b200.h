@@ -456,6 +456,60 @@ int tml_sys_read(tml_ctx* ctx, tml_sys_record* out, uint32_t max_records, uint32
 int tml_sys_reduce_launch(tml_ctx* ctx, uint32_t max_rows, void* stream);
 int tml_sys_reduce_collect(tml_ctx* ctx, tml_sys_agg* out);
 
+/* ---- multi-node System section: each node leader's K6s result crosses the network as one fixed
+ * record; comm index 0 folds them (K6m) into the cluster rollup over all nodes' retained samples.
+ *
+ * The unrounded fold of K6s's sample-level columns: double-double sums (value = hi + lo), exact
+ * u64 sums, extrema and counts.  Folding two of these and rounding once (csrc/tml_sys_sum.h)
+ * gives the window aggregate of the two sample sets together. */
+typedef struct tml_sys_part {
+  double cpu_hi, cpu_lo, cpu_max, ts_min, ts_max;
+  double d_hi[4], d_lo[4], d_max[4];  /* derived util / mem / temp / power: avg sums, peaks */
+  uint64_t ram_sum, ram_max, ram_total_max, n, n_gpu;
+  uint32_t avail, gpu_count, n_gpus, _pad;
+} tml_sys_part;
+
+#define TML_HOSTNAME_MAX 64  /* Linux HOST_NAME_MAX + 1 */
+
+/* The launcher identity of one System source (SystemNodeIdentity, loader.py:78-93). */
+typedef struct tml_sys_node_ident {
+  int32_t global_rank, local_rank;
+  int32_t node_rank;        /* -1: none (the node label is then the global rank)  */
+  int32_t world_size, local_world_size;
+  int32_t _pad;
+  char hostname[TML_HOSTNAME_MAX];  /* NUL-terminated                            */
+} tml_sys_node_ident;
+
+/* One rank's contribution to the gather: valid = 0 for a rank that is not a node leader or whose
+ * system ring is empty (agg and part are then zero). */
+typedef struct tml_sys_node_record {
+  tml_sys_node_ident ident;
+  uint32_t valid, _pad;
+  tml_sys_agg agg;          /* the node's finished K6s aggregates (per-GPU rows included) */
+  tml_sys_part part;        /* its unrounded sample-level fold                            */
+} tml_sys_node_record;
+
+/* K6m's result, in the slot right after the gathered records.  order[0 .. n_nodes) are the indices
+ * of the records folded, in fold order: ascending node label (node_rank, else global_rank) as an
+ * integer, which is the reference's row order.  Records that repeat a label are dropped, keeping
+ * the lowest global rank; n_dup counts them. */
+typedef struct tml_sys_cluster_out {
+  tml_sys_agg agg;          /* the cluster rollup; gpu[] is unused (zero)                 */
+  uint32_t n_nodes, n_dup;
+  int32_t order[TML_MAX_RANKS];
+} tml_sys_cluster_out;
+
+/* Assemble this rank's record at device address d_record on `stream`, after this context's last
+ * K6s (its own event), from the device-resident aggregates: no host round trip.  ident == NULL or a
+ * context without samples writes a record with valid = 0. */
+int tml_sys_node_pack(tml_ctx* ctx, const tml_sys_node_ident* ident, void* d_record, void* stream);
+/* K6m k_sys_cluster over n_records (1 .. TML_MAX_RANKS) consecutive records at d_records; writes a
+ * tml_sys_cluster_out right after them, then copies records + result to pinned memory
+ * (asynchronously, on `stream`).  Collect waits on that copy's own event and writes n_records
+ * records followed by the tml_sys_cluster_out into `out`. */
+int tml_sys_cluster_launch(tml_ctx* ctx, const void* d_records, uint32_t n_records, void* stream);
+int tml_sys_cluster_collect(tml_ctx* ctx, void* out);
+
 /* ---------------------------------------------------------------- WHOLE REDUCE
  * The staged reduce above, sequenced natively for the production layout (one rank
  * per process / GPU): prepare -> bounds exchange (+ process aggregates + the
@@ -665,6 +719,14 @@ typedef struct tml_sys_diag_in {
  * "per_gpu"}: the diagnosis, SystemSummaryAgg and the PerGPUSummary rows (model.py:50-117). */
 int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t cap);
 
+/* diagnose_system over several nodes (api.py:189-209): the same per-node rules, scopes and
+ * samples_used as tml_diag_system for each node with samples; issues sorted across nodes by
+ * priority, severity, score, then node label as a string; without an issue the default primary
+ * from the cluster aggregate.  `nodes` in the order their labels sort as strings.  Writes
+ * {"primary", "issues", "aggregate", "nodes": {label: {"aggregate", "per_gpu"}}}. */
+int tml_diag_system_cluster(const tml_sys_diag_in* nodes, uint32_t n_nodes, const tml_sys_agg* cluster,
+                            char* json_out, size_t cap);
+
 /* ---------------------------------------------------------------- SECTIONS
  * All three sections of one tml_reduce_run as one JSON object
  * {"step_time": {data, diagnosis, global, overview}, "step_memory": {...},
@@ -725,8 +787,12 @@ int tml_xs_host_sum(const double* x, uint64_t n, int planned, double* out_sum, u
 /* Host emulation of k_sys_reduce's float sums (csrc/tml_sys_sum.h), so the CPU suite can fuzz them
  * against CPython's sum().  mode 0: the per-sample restatement of CPython 3.12's compensated loop;
  * mode 1: the window sum -- a TwoSum double-double carried through the kernel's exact reduction
- * tree for a grid of `nblk` CTAs, rounded once.  Never called by the product. */
+ * tree for a grid of `nblk` CTAs, rounded once; mode 2: mode 1 unrounded, the pair (hi, lo) into
+ * out_sum[0], out_sum[1].  Never called by the product. */
 int tml_sys_host_sum(const double* x, uint64_t n, uint32_t mode, uint32_t nblk, double* out_sum);
+/* Host emulation of K6m: the same record selection, fold and finish (csrc/tml_sys_sum.h) on the
+ * CPU.  Never called by the product. */
+int tml_sys_host_cluster(const tml_sys_node_record* records, uint32_t n_records, tml_sys_cluster_out* out);
 
 #ifdef __cplusplus
 }

@@ -141,6 +141,29 @@ class SysDiagIn(C.Structure):
     _fields_ = [("node_rank", i32), ("_pad", i32), ("node_label", C.c_char * 32), ("agg", SysAgg)]
 
 
+TML_HOSTNAME_MAX = 64
+
+
+class SysPart(C.Structure):
+    _fields_ = [("cpu_hi", f64), ("cpu_lo", f64), ("cpu_max", f64), ("ts_min", f64), ("ts_max", f64),
+                ("d_hi", f64 * 4), ("d_lo", f64 * 4), ("d_max", f64 * 4),
+                ("ram_sum", u64), ("ram_max", u64), ("ram_total_max", u64), ("n", u64), ("n_gpu", u64),
+                ("avail", u32), ("gpu_count", u32), ("n_gpus", u32), ("_pad", u32)]
+
+
+class SysNodeIdent(C.Structure):
+    _fields_ = [("global_rank", i32), ("local_rank", i32), ("node_rank", i32), ("world_size", i32),
+                ("local_world_size", i32), ("_pad", i32), ("hostname", C.c_char * TML_HOSTNAME_MAX)]
+
+
+class SysNodeRecord(C.Structure):
+    _fields_ = [("ident", SysNodeIdent), ("valid", u32), ("_pad", u32), ("agg", SysAgg), ("part", SysPart)]
+
+
+class SysClusterOut(C.Structure):
+    _fields_ = [("agg", SysAgg), ("n_nodes", u32), ("n_dup", u32), ("order", i32 * TML_MAX_RANKS)]
+
+
 class Comm(C.Structure):
     _fields_ = [("nccl_comm", vp), ("rank", i32), ("world", i32)]
 
@@ -275,6 +298,11 @@ SIGNATURES = {
     "tml_sys_reduce_collect": (C.c_int, [vp, C.POINTER(SysAgg)]),
     "tml_diag_system": (C.c_int, [C.POINTER(SysDiagIn), C.c_char_p, C.c_size_t]),
     "tml_sys_host_sum": (C.c_int, [vp, u64, u32, u32, C.POINTER(f64)]),
+    "tml_sys_node_pack": (C.c_int, [vp, C.POINTER(SysNodeIdent), vp, vp]),
+    "tml_sys_cluster_launch": (C.c_int, [vp, vp, u32, vp]),
+    "tml_sys_cluster_collect": (C.c_int, [vp, vp]),
+    "tml_diag_system_cluster": (C.c_int, [C.POINTER(SysDiagIn), u32, C.POINTER(SysAgg), C.c_char_p, C.c_size_t]),
+    "tml_sys_host_cluster": (C.c_int, [C.POINTER(SysNodeRecord), u32, C.POINTER(SysClusterOut)]),
     # private (csrc/tml_internal.h): tml_reduce_run that emits an earlier reduce's sections meanwhile
     "tml_summary_run_": (C.c_int, [vp, C.POINTER(Comm), C.POINTER(ReduceRunArgs), vp, C.POINTER(ReduceRunOut),
                                    C.POINTER(ReduceRunOut), C.POINTER(SectionsArgs), vp, C.c_size_t,
@@ -337,6 +365,21 @@ def diag_json(fn_name: str, arg: C.Structure, cap: int = 1 << 16) -> Any:
         return diag_json(fn_name, arg, len(buf) * 8)
     check(rc, fn_name)
     return json.loads(buf.value)
+
+
+def diag_system_cluster(nodes, n_nodes: int, cluster: SysAgg) -> Any:
+    """tml_diag_system_cluster over ``nodes`` (a ctypes array of SysDiagIn) -> dict."""
+    global _DIAG_BUF
+    cap = 1 << 16
+    while True:
+        if _DIAG_BUF is None or len(_DIAG_BUF) < cap:
+            _DIAG_BUF = C.create_string_buffer(cap)
+        rc = lib().tml_diag_system_cluster(nodes, int(n_nodes), C.byref(cluster), _DIAG_BUF, len(_DIAG_BUF))
+        if rc != -8:  # TML_ERR_SMALL
+            break
+        cap = len(_DIAG_BUF) * 8
+    check(rc, "tml_diag_system_cluster")
+    return json.loads(_DIAG_BUF.value)
 
 
 _SEC_BUF = None

@@ -1056,13 +1056,11 @@ extern "C" int tml_diag_process(const tml_proc_diag_in* in, char* json_out, size
 }
 
 // ================================================================== system
-// diagnose_system over the engine's one node (diagnostics/system/api.py:189-209): the node's
-// rules (context.py:285-373, rules.py:55-310, policy.py:22-36), scoped to the node
-// (api.py:106-170); without an issue the cluster-level default primary (api.py:68-103).  Also
-// emits SystemSummaryAgg and the PerGPUSummary rows (reporting/sections/system/model.py:50-117).
-extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t cap) {
-  tml_json::Scope json_scope;
-  if (!in) return TML_ERR_ARG;
+namespace {
+
+// One node's issues (context.py:285-373, rules.py:55-310, policy.py:22-36) in DEFAULT_SYSTEM_RULES
+// order, each scoped to the node (api.py:106-170) with samples_used = the node's samples.
+void sys_node_issues(const tml_sys_diag_in* in, std::vector<Issue>& issues) {
   const tml_sys_agg& a = in->agg;
   const bool have = a.n > 0, hg = a.n_gpu > 0;
   const int n_gpus = have ? (int)std::min<uint32_t>(a.n_gpus, TML_SYS_MAX_GPUS) : 0;
@@ -1104,7 +1102,6 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
   const double mem_pct = mem_frac * 100.0, pow_pct = pow_frac * 100.0;
 
   // ---- rules, in DEFAULT_SYSTEM_RULES order; SYSTEM_ISSUE_PRIORITY is that same order
-  std::vector<Issue> issues;
   auto pct_s = [](double v) { return fmt("%.1f%%", v); };  // rules.py:13-14
   auto mk = [&](const char* kind, const char* status, const char* sev, S summary, const char* action,
                 const char* metric, const char* phase, double score, int gpu, const S& ev_head) {
@@ -1189,8 +1186,12 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
          Obj().kv("gpu_util_avg_percent", jnum(a.gpu_util_avg))
              .kv("lowest_util_gpu_idx", jopt_int(lo_util_idx, lo_util_idx >= 0)).done());
   }
+}
 
-  // ---- primary (api.py:68-103, 173-186)
+// The diagnosis primary (api.py:68-103, 173-186): the first issue, scoped, with the samples of its
+// node; without one, the default from the cluster aggregate `a`.
+S sys_primary(const std::vector<Issue>& issues, long long issue_samples, const tml_sys_agg& a) {
+  const bool have = a.n > 0, hg = a.n_gpu > 0;
   auto pd = [&](const S& kind, const S& sev, const S& status, const S& reason, const S& action, long long used,
                 const S& scope) {
     return Obj().kv("severity", jstr(sev)).kv("status", jstr(status)).kv("reason", jstr(reason))
@@ -1201,7 +1202,7 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
     const Issue& t = issues[0];
     const size_t at = t.evidence.find("\"scope\":");
     const size_t end = t.evidence.find('}', at);
-    primary = pd(t.kind, t.severity, t.status, t.summary, t.action, (long long)a.n,
+    primary = pd(t.kind, t.severity, t.status, t.summary, t.action, issue_samples,
                  t.evidence.substr(at + 8, end + 1 - (at + 8)));
   } else if (!have) {
     primary = pd("NO_DATA", "info", "NO DATA", "No system telemetry was recorded.",
@@ -1213,9 +1214,13 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
                  "Use training diagnostics for model-level bottlenecks.", (long long)a.n,
                  Obj().kv("level", jstr("cluster")).done());
   }
+  return primary;
+}
 
-  // ---- SystemSummaryAgg and PerGPUSummary (model.py:50-117, loader.py:97-156)
-  S agg = Obj().kv("first_ts", jopt_num(a.first_ts, have)).kv("last_ts", jopt_num(a.last_ts, have))
+// SystemSummaryAgg (model.py:50-81, loader.py:97-125) of `a`.
+S sys_agg_json(const tml_sys_agg& a) {
+  const bool have = a.n > 0, hg = a.n_gpu > 0;
+  return Obj().kv("first_ts", jopt_num(a.first_ts, have)).kv("last_ts", jopt_num(a.last_ts, have))
       .kv("system_samples", jint((long long)a.n))
       .kv("cpu_avg_percent", jopt_num(a.cpu_avg, have)).kv("cpu_peak_percent", jopt_num(a.cpu_peak, have))
       .kv("ram_avg_bytes", jopt_num(a.ram_avg, have)).kv("ram_peak_bytes", jopt_num(a.ram_peak, have))
@@ -1227,6 +1232,11 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
       .kv("gpu_temp_avg_c", jopt_num(a.gpu_temp_avg, hg)).kv("gpu_temp_peak_c", jopt_num(a.gpu_temp_peak, hg))
       .kv("gpu_power_avg_w", jopt_num(a.gpu_power_avg, hg)).kv("gpu_power_peak_w", jopt_num(a.gpu_power_peak, hg))
       .done();
+}
+
+// The PerGPUSummary rows (model.py:84-117, loader.py:128-156) of a node's aggregates.
+S sys_per_gpu_json(const tml_sys_agg& a) {
+  const int n_gpus = a.n > 0 ? (int)std::min<uint32_t>(a.n_gpus, TML_SYS_MAX_GPUS) : 0;
   Obj per_gpu;
   for (int g = 0; g < n_gpus; ++g) {
     const tml_sys_gpu_agg& q = a.gpu[g];
@@ -1237,9 +1247,71 @@ extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t
             .kv("temp_peak_c", jnum(q.temp_peak)).kv("power_avg_w", jnum(q.power_avg))
             .kv("power_peak_w", jnum(q.power_peak)).kv("power_limit_w", jnum(q.power_limit)).done());
   }
+  return per_gpu.done();
+}
+
+int sys_priority(const S& kind) {  // SYSTEM_ISSUE_PRIORITY (rules.py:273-281)
+  static const char* const order[] = {"VERY_HIGH_GPU_MEMORY", "HIGH_GPU_TEMPERATURE", "HIGH_GPU_MEMORY",
+                                      "HIGH_GPU_POWER", "HIGH_HOST_MEMORY", "HIGH_CPU", "LOW_GPU_UTILIZATION"};
+  for (int k = 0; k < 7; ++k)
+    if (kind == order[k]) return k;
+  return 999;
+}
+
+int sys_severity(const S& sev) { return sev == "crit" ? 2 : sev == "warn" ? 1 : 0; }  // common.py:98-102
+
+}  // namespace
+
+// diagnose_system over the engine's one node (diagnostics/system/api.py:189-209): the node's
+// rules, scoped to the node; without an issue the cluster-level default primary.  Also emits
+// SystemSummaryAgg and the PerGPUSummary rows (reporting/sections/system/model.py:50-117).
+extern "C" int tml_diag_system(const tml_sys_diag_in* in, char* json_out, size_t cap) {
+  tml_json::Scope json_scope;
+  if (!in) return TML_ERR_ARG;
+  std::vector<Issue> issues;
+  sys_node_issues(in, issues);
+  const S primary = sys_primary(issues, (long long)in->agg.n, in->agg);
   std::vector<S> is;
   for (const Issue& i : issues) is.push_back(i.json());
-  return emit(Obj().kv("primary", primary).kv("issues", jarr(is)).kv("aggregate", agg)
-                  .kv("per_gpu", per_gpu.done()).done(),
+  return emit(Obj().kv("primary", primary).kv("issues", jarr(is)).kv("aggregate", sys_agg_json(in->agg))
+                  .kv("per_gpu", sys_per_gpu_json(in->agg)).done(),
+              json_out, cap);
+}
+
+// The same over several nodes (api.py:189-209): every node's issues, sorted by _issue_sort_key
+// (priority, severity, score, node label as a string); a stable sort over the nodes in label
+// order, as the reference sorts its list built in that order.
+extern "C" int tml_diag_system_cluster(const tml_sys_diag_in* nodes, uint32_t n_nodes, const tml_sys_agg* cluster,
+                                       char* json_out, size_t cap) {
+  tml_json::Scope json_scope;
+  if ((!nodes && n_nodes) || !cluster || n_nodes > TML_MAX_RANKS) return TML_ERR_ARG;
+  struct Tagged { Issue issue; S label; long long samples; };
+  std::vector<Tagged> all;
+  Obj per_node;
+  for (uint32_t k = 0; k < n_nodes; ++k) {
+    const tml_sys_diag_in& in = nodes[k];
+    char label_buf[33];
+    memcpy(label_buf, in.node_label, 32);
+    label_buf[32] = 0;
+    std::vector<Issue> issues;
+    sys_node_issues(&in, issues);
+    for (Issue& i : issues) all.push_back({i, S(label_buf), (long long)in.agg.n});
+    per_node.kv(label_buf, Obj().kv("aggregate", sys_agg_json(in.agg)).kv("per_gpu", sys_per_gpu_json(in.agg)).done());
+  }
+  std::stable_sort(all.begin(), all.end(), [](const Tagged& x, const Tagged& y) {
+    const int px = sys_priority(x.issue.kind), py = sys_priority(y.issue.kind);
+    if (px != py) return px < py;
+    const int sx = sys_severity(x.issue.severity), sy = sys_severity(y.issue.severity);
+    if (sx != sy) return sx > sy;
+    if (x.issue.score != y.issue.score) return x.issue.score > y.issue.score;
+    return strcmp(x.label.c_str(), y.label.c_str()) < 0;
+  });
+  std::vector<Issue> issues;
+  for (const Tagged& t : all) issues.push_back(t.issue);
+  const S primary = sys_primary(issues, all.empty() ? 0 : all[0].samples, *cluster);
+  std::vector<S> is;
+  for (const Issue& i : issues) is.push_back(i.json());
+  return emit(Obj().kv("primary", primary).kv("issues", jarr(is)).kv("aggregate", sys_agg_json(*cluster))
+                  .kv("nodes", per_node.done()).done(),
               json_out, cap);
 }

@@ -14,6 +14,8 @@
 //   K6  k_proc_reduce                 per-rank process aggregates
 //   K5s k_sys_commit                  576-B host / all-GPU sample into the system ring
 //   K6s k_sys_reduce                  System section window aggregates (one launch)
+//   K6p k_sys_node_pack               one node's System record, assembled in HBM for the gather
+//   K6m k_sys_cluster                 the gathered node records -> the cluster System rollup
 //
 // Nothing here is a dense contraction: no tensor-core path.  Every bulk kernel
 // is HBM-bound; accesses are 16-byte vectorised and warp-coalesced, tiles are
@@ -1573,37 +1575,16 @@ __global__ void k_finalize_dd(const double* __restrict__ partials, int nblk, int
 //   pass B  one thread per (record, GPU index), GPU = tid % 16: the per-GPU columns.
 // Each CTA folds its threads in a fixed tree (warp butterfly, then warps in order) into one
 // partial; the last CTA to finish folds the partials in CTA order and writes the finished
-// tml_sys_agg.  Every float sum is a TwoSum double-double until that last fold; integer columns
+// tml_sys_agg, and beside it that fold unrounded (tml_sys_part) for the multi-node rollup.  Every float sum is a TwoSum double-double until that last fold; integer columns
 // are exact u64 sums.  The result does not depend on which CTA finishes last.
 
-struct SysPartA {
-  double cpu_hi, cpu_lo, cpu_max, ts_min, ts_max;
-  double d_hi[4], d_lo[4], d_max[4];  // derived util / mem / temp / power: avg sums, peaks
-  u64 ram_sum, ram_max, ram_total_max, n, n_gpu;
-  u32 avail, gpu_count, n_gpus, _pad;
-};
+typedef tml_sys_part SysPartA;  // the sample-level fold (tml_sys_sum.h)
 struct SysPartG {
   double p_hi, p_lo;  // watts
   u64 n, util_sum, mem_sum, temp_sum, mem_max, mem_total_max;
   u32 util_max, temp_max, power_max, plimit_max;  // power in mW: mW / 1000.0 is monotone
 };
 
-__device__ __forceinline__ void sysa_init(SysPartA& a) {
-  a.cpu_hi = a.cpu_lo = 0.0; a.cpu_max = -INFINITY; a.ts_min = INFINITY; a.ts_max = -INFINITY;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) { a.d_hi[k] = 0.0; a.d_lo[k] = 0.0; a.d_max[k] = -INFINITY; }
-  a.ram_sum = a.ram_max = a.ram_total_max = a.n = a.n_gpu = 0;
-  a.avail = a.gpu_count = a.n_gpus = a._pad = 0;
-}
-__device__ __forceinline__ void sysa_merge(SysPartA& a, const SysPartA& b) {
-  sys_dd_add(a.cpu_hi, a.cpu_lo, b.cpu_hi, b.cpu_lo);
-  a.cpu_max = fmax(a.cpu_max, b.cpu_max); a.ts_min = fmin(a.ts_min, b.ts_min); a.ts_max = fmax(a.ts_max, b.ts_max);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) { sys_dd_add(a.d_hi[k], a.d_lo[k], b.d_hi[k], b.d_lo[k]); a.d_max[k] = fmax(a.d_max[k], b.d_max[k]); }
-  a.ram_sum += b.ram_sum; a.ram_max = max(a.ram_max, b.ram_max); a.ram_total_max = max(a.ram_total_max, b.ram_total_max);
-  a.n += b.n; a.n_gpu += b.n_gpu;
-  a.avail |= b.avail; a.gpu_count = max(a.gpu_count, b.gpu_count); a.n_gpus = max(a.n_gpus, b.n_gpus);
-}
 __device__ __forceinline__ SysPartA sysa_shfl(const SysPartA& a, int m) {
   SysPartA o;
   o.cpu_hi = shfl_xor_f64(a.cpu_hi, m); o.cpu_lo = shfl_xor_f64(a.cpu_lo, m); o.cpu_max = shfl_xor_f64(a.cpu_max, m);
@@ -1647,14 +1628,15 @@ __device__ __forceinline__ T sys_ld_cg(const T* p) {
 __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record* __restrict__ ring, u32 slots,
                                                             u64 first_k, u64 n, SysPartA* pa,
                                                             SysPartG* pg, unsigned int* ticket,
-                                                            tml_sys_agg* __restrict__ out) {
+                                                            tml_sys_agg* __restrict__ out,
+                                                            tml_sys_part* __restrict__ out_part) {
   __shared__ SysPartA s_a[SYS_THREADS / 32];
   __shared__ SysPartG s_g[SYS_THREADS / 32][TML_SYS_MAX_GPUS];
   __shared__ bool s_last;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // ---- pass A: samples
   SysPartA a;
-  sysa_init(a);
+  sys_part_init(a);
   for (u64 i = (u64)blockIdx.x * SYS_THREADS + tid; i < n; i += (u64)gridDim.x * SYS_THREADS) {
     const tml_sys_record* r = &ring[(first_k + i) % slots];
     const double ts = __ldg(&r->ts), cpu = __ldg(&r->cpu_pct);
@@ -1664,7 +1646,7 @@ __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record
     if (ng > TML_SYS_MAX_GPUS) ng = TML_SYS_MAX_GPUS;
     sys_dd_add(a.cpu_hi, a.cpu_lo, cpu, 0.0);
     a.cpu_max = fmax(a.cpu_max, cpu); a.ts_min = fmin(a.ts_min, ts); a.ts_max = fmax(a.ts_max, ts);
-    a.ram_sum += ram; a.ram_max = max(a.ram_max, ram); a.ram_total_max = max(a.ram_total_max, ram_total);
+    a.ram_sum += ram; a.ram_max = sys_max_u64(a.ram_max, ram); a.ram_total_max = sys_max_u64(a.ram_total_max, ram_total);
     a.n += 1; a.avail |= (fl & TML_SYS_GPU_AVAILABLE) ? 1u : 0u;
     a.gpu_count = max(a.gpu_count, gc); a.n_gpus = max(a.n_gpus, ng);
     if (ng > 0) {
@@ -1681,7 +1663,7 @@ __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record
 #pragma unroll
   for (int m = 16; m >= 1; m >>= 1) {
     const SysPartA o = sysa_shfl(a, m);
-    sysa_merge(a, o);
+    sys_part_merge(a, o);
   }
   if (lane == 0) s_a[warp] = a;
   // ---- pass B: (sample, GPU index) pairs
@@ -1717,8 +1699,8 @@ __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record
   __syncthreads();
   if (tid == 0) {
     SysPartA b;
-    sysa_init(b);
-    for (int w = 0; w < SYS_THREADS / 32; ++w) sysa_merge(b, s_a[w]);
+    sys_part_init(b);
+    for (int w = 0; w < SYS_THREADS / 32; ++w) sys_part_merge(b, s_a[w]);
     pa[blockIdx.x] = b;
   } else if (tid >= 32 && tid < 32 + (int)TML_SYS_MAX_GPUS) {
     SysPartG b;
@@ -1736,21 +1718,10 @@ __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record
   const int nb = (int)gridDim.x;
   if (tid == 0) {
     SysPartA b;
-    sysa_init(b);
-    for (int k = 0; k < nb; ++k) sysa_merge(b, sys_ld_cg(pa + k));
-    const double cnt = (double)b.n;
-    out->n = b.n; out->n_gpu = b.n_gpu;
-    out->first_ts = b.ts_min; out->last_ts = b.ts_max;
-    out->cpu_avg = (b.cpu_hi + b.cpu_lo) / cnt; out->cpu_peak = b.cpu_max;
-    out->ram_avg = (double)b.ram_sum / cnt; out->ram_peak = (double)b.ram_max;
-    out->ram_total = (double)b.ram_total_max;
-    const double cg = (double)b.n_gpu;
-    const bool hg = b.n_gpu > 0;
-    out->gpu_util_avg = hg ? (b.d_hi[0] + b.d_lo[0]) / cg : 0.0; out->gpu_util_peak = hg ? b.d_max[0] : 0.0;
-    out->gpu_mem_avg = hg ? (b.d_hi[1] + b.d_lo[1]) / cg : 0.0; out->gpu_mem_peak = hg ? b.d_max[1] : 0.0;
-    out->gpu_temp_avg = hg ? (b.d_hi[2] + b.d_lo[2]) / cg : 0.0; out->gpu_temp_peak = hg ? b.d_max[2] : 0.0;
-    out->gpu_power_avg = hg ? (b.d_hi[3] + b.d_lo[3]) / cg : 0.0; out->gpu_power_peak = hg ? b.d_max[3] : 0.0;
-    out->gpu_available = b.avail; out->gpu_count = b.gpu_count; out->n_gpus = b.n_gpus; out->_pad = 0;
+    sys_part_init(b);
+    for (int k = 0; k < nb; ++k) sys_part_merge(b, sys_ld_cg(pa + k));
+    sys_part_finish(b, out);
+    *out_part = b;
     *ticket = 0u;  // re-armed for the next launch (every other CTA has taken its ticket)
   } else if (tid >= 32 && tid < 32 + (int)TML_SYS_MAX_GPUS) {
     const int gx = tid - 32;
@@ -1768,6 +1739,34 @@ __global__ void __launch_bounds__(SYS_THREADS) k_sys_reduce(const tml_sys_record
     o.power_avg = h ? (b.p_hi + b.p_lo) / cnt : 0.0; o.power_peak = (double)b.power_max / 1000.0;
     o.power_limit = (double)b.plimit_max / 1000.0;
   }
+}
+
+// ------------------------------------------------------------------ multi-node System
+// The node record is assembled where the gather reads it: identity from the kernel argument, the
+// node's aggregates and part from K6s's device outputs (absent: a record with valid = 0).
+__global__ void k_sys_node_pack(const __grid_constant__ tml_sys_node_ident id, const tml_sys_agg* __restrict__ agg,
+                                const tml_sys_part* __restrict__ part, tml_sys_node_record* __restrict__ dst) {
+  static_assert(sizeof(tml_sys_agg) % 8 == 0 && sizeof(tml_sys_part) % 8 == 0, "8-B words");
+  const bool valid = agg != nullptr;
+  if (threadIdx.x == 0) { dst->ident = id; dst->valid = valid ? 1u : 0u; dst->_pad = 0; }
+  u64* da = reinterpret_cast<u64*>(&dst->agg);
+  const u64* sa = reinterpret_cast<const u64*>(agg);
+  for (int k = threadIdx.x; k < (int)(sizeof(tml_sys_agg) / 8); k += blockDim.x) da[k] = valid ? sa[k] : 0ull;
+  u64* dp = reinterpret_cast<u64*>(&dst->part);
+  const u64* sp = reinterpret_cast<const u64*>(part);
+  for (int k = threadIdx.x; k < (int)(sizeof(tml_sys_part) / 8); k += blockDim.x) dp[k] = valid ? sp[k] : 0ull;
+}
+
+// K6m: at most TML_MAX_RANKS records, so one thread runs the selection, fold and finish
+// (sys_cluster_fold, shared with the host emulation) and the block copies the result out.
+__global__ void k_sys_cluster(const tml_sys_node_record* __restrict__ rec, u32 n, tml_sys_cluster_out* __restrict__ out) {
+  __shared__ tml_sys_cluster_out s;
+  if (threadIdx.x == 0) sys_cluster_fold(rec, n, &s);
+  __syncthreads();
+  static_assert(sizeof(tml_sys_cluster_out) % 8 == 0, "8-B words");
+  const u64* src = reinterpret_cast<const u64*>(&s);
+  u64* dst = reinterpret_cast<u64*>(out);
+  for (int k = threadIdx.x; k < (int)(sizeof(tml_sys_cluster_out) / 8); k += blockDim.x) dst[k] = src[k];
 }
 
 // =================================================================== host side
@@ -1920,15 +1919,22 @@ struct tml_ctx {
   tml_sys_record* d_sring = nullptr;
   u64 sys_commits = 0;
   std::mutex sys_mu;
-  void* d_sys_ws = nullptr;         // SysPartA[grid cap] | SysPartG[grid cap][16] | ticket | tml_sys_agg
+  void* d_sys_ws = nullptr;         // SysPartA[grid cap] | SysPartG[grid cap][16] | ticket | tml_sys_agg | tml_sys_part
   SysPartA* d_sys_pa = nullptr;
   SysPartG* d_sys_pg = nullptr;
   unsigned int* d_sys_ticket = nullptr;
   tml_sys_agg* d_sys_out = nullptr;
   tml_sys_agg* h_sys_out = nullptr; // pinned: the result's copy lands here
+  tml_sys_part* d_sys_part = nullptr;  // K6s's unrounded sample-level fold, beside d_sys_out
   cudaEvent_t ev_sys = nullptr;
   bool sys_pending = false;
   u64 sys_pending_n = 0;
+  u64 sys_last_n = 0;               // samples the last K6s launch covered (0: none launched)
+  // K6m (tml_sys_cluster_*): pinned landing of the gathered records + result, allocated on first use
+  void* h_sys_cluster = nullptr;
+  cudaEvent_t ev_sys_cluster = nullptr;
+  u32 sys_cluster_n = 0;
+  bool sys_cluster_pending = false;
 };
 
 static void comb_free(tml_ctx* c);
@@ -2121,6 +2127,8 @@ int tml_shutdown(tml_ctx* c) {
   cudaFree(c->d_sring); cudaFree(c->d_sys_ws);
   if (c->h_sys_out) cudaFreeHost(c->h_sys_out);
   if (c->ev_sys) cudaEventDestroy(c->ev_sys);
+  if (c->h_sys_cluster) cudaFreeHost(c->h_sys_cluster);
+  if (c->ev_sys_cluster) cudaEventDestroy(c->ev_sys_cluster);
   cudaFreeHost(c->h_stage);
   comb_free(c);
   tml_run_ws_free_(c->run_ws);
@@ -2444,10 +2452,12 @@ static int sys_ensure(tml_ctx* c) {
   const u64 cap = (u64)c->n_sms * 4ull;  // grid_for's cap
   const size_t o_pg = cap * sizeof(SysPartA), o_t = o_pg + cap * TML_SYS_MAX_GPUS * sizeof(SysPartG);
   const size_t o_out = (o_t + sizeof(unsigned int) + 255) & ~(size_t)255;
-  CK(cudaMalloc(&c->d_sys_ws, o_out + sizeof(tml_sys_agg)));
+  const size_t o_part = o_out + sizeof(tml_sys_agg);  // 8-B aligned: tml_sys_agg is a multiple of 8 B
+  CK(cudaMalloc(&c->d_sys_ws, o_part + sizeof(tml_sys_part)));
   char* base = (char*)c->d_sys_ws;
   c->d_sys_pa = (SysPartA*)base; c->d_sys_pg = (SysPartG*)(base + o_pg);
   c->d_sys_ticket = (unsigned int*)(base + o_t); c->d_sys_out = (tml_sys_agg*)(base + o_out);
+  c->d_sys_part = (tml_sys_part*)(base + o_part);
   CK(cudaMemset(c->d_sys_ticket, 0, sizeof(unsigned int)));
   CK(cudaHostAlloc(&c->h_sys_out, sizeof(tml_sys_agg), cudaHostAllocDefault));
   CK(cudaEventCreateWithFlags(&c->ev_sys, cudaEventDisableTiming));
@@ -2512,7 +2522,7 @@ int tml_ring_reset(tml_ctx* c) {
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   memset(c->h_page, 0, sizeof(HostPage));
   c->commits = 0; c->proc_commits.store(0); c->next_slot = 0;
-  c->sys_commits = 0;
+  c->sys_commits = 0; c->sys_last_n = 0;
   c->drain_tail = 0; c->pdrain_tail = 0; c->mirror_copied = 0;
   memset(c->host_dur, 0, sizeof(c->host_dur));
   memset(c->host_calls, 0, sizeof(c->host_calls));
@@ -3227,11 +3237,12 @@ int tml_sys_reduce_launch(tml_ctx* c, uint32_t max_rows, void* stream) {
   if (n > max_rows) n = max_rows;
   c->sys_pending_n = n;
   c->sys_pending = true;
+  c->sys_last_n = n;
   if (n == 0) return TML_OK;
   CK(cudaSetDevice(c->device));
   const int grid = grid_for(c, n, SYS_THREADS);
   k_sys_reduce<<<grid, SYS_THREADS, 0, s>>>(c->d_sring, c->proc_slots, total - n, n, c->d_sys_pa, c->d_sys_pg,
-                                            c->d_sys_ticket, c->d_sys_out);
+                                            c->d_sys_ticket, c->d_sys_out, c->d_sys_part);
   CK(cudaPeekAtLastError());
   c->launches += 1;
   CK(cudaMemcpyAsync(c->h_sys_out, c->d_sys_out, sizeof(tml_sys_agg), cudaMemcpyDeviceToHost, s));
@@ -3248,6 +3259,64 @@ int tml_sys_reduce_collect(tml_ctx* c, tml_sys_agg* out) {
   if (c->sys_pending_n == 0) return TML_OK;
   CK(cudaEventSynchronize(c->ev_sys));  // normally landed already: the build's own wait covered it
   memcpy(out, c->h_sys_out, sizeof(*out));
+  return TML_OK;
+}
+
+// Behind this context's last K6s (its event) on `stream`; a context without a launch that covered
+// samples contributes valid = 0.
+int tml_sys_node_pack(tml_ctx* c, const tml_sys_node_ident* ident, void* d_record, void* stream) {
+  if (!c || !d_record) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  tml_sys_node_ident id;
+  memset(&id, 0, sizeof(id));
+  id.node_rank = -1;
+  const bool valid = ident != nullptr && c->sys_last_n > 0;
+  if (ident) {
+    id = *ident;
+    id.hostname[TML_HOSTNAME_MAX - 1] = 0;
+  }
+  if (valid) CK(cudaStreamWaitEvent(s, c->ev_sys, 0));
+  k_sys_node_pack<<<1, 32, 0, s>>>(id, valid ? c->d_sys_out : nullptr, valid ? c->d_sys_part : nullptr,
+                                   (tml_sys_node_record*)d_record);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  return TML_OK;
+}
+
+int tml_sys_cluster_launch(tml_ctx* c, const void* d_records, uint32_t n_records, void* stream) {
+  if (!c || !d_records || n_records == 0 || n_records > TML_MAX_RANKS) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  cudaStream_t s = (cudaStream_t)stream;
+  CK(cudaSetDevice(c->device));
+  const size_t bytes = (size_t)TML_MAX_RANKS * sizeof(tml_sys_node_record) + sizeof(tml_sys_cluster_out);
+  if (!c->h_sys_cluster) {
+    CK(cudaHostAlloc(&c->h_sys_cluster, bytes, cudaHostAllocDefault));
+    CK(cudaEventCreateWithFlags(&c->ev_sys_cluster, cudaEventDisableTiming));
+  }
+  const tml_sys_node_record* rec = (const tml_sys_node_record*)d_records;
+  tml_sys_cluster_out* out = (tml_sys_cluster_out*)(rec + n_records);
+  k_sys_cluster<<<1, 64, 0, s>>>(rec, n_records, out);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  CK(cudaMemcpyAsync(c->h_sys_cluster, d_records,
+                     (size_t)n_records * sizeof(tml_sys_node_record) + sizeof(tml_sys_cluster_out),
+                     cudaMemcpyDeviceToHost, s));
+  CK(cudaEventRecord(c->ev_sys_cluster, s));
+  c->sys_cluster_n = n_records;
+  c->sys_cluster_pending = true;
+  return TML_OK;
+}
+
+int tml_sys_cluster_collect(tml_ctx* c, void* out) {
+  if (!c || !out) return TML_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->sys_mu);
+  if (!c->sys_cluster_pending) return set_err(TML_ERR_STATE, "tml_sys_cluster_collect without a launch");
+  c->sys_cluster_pending = false;
+  CK(cudaEventSynchronize(c->ev_sys_cluster));
+  memcpy(out, c->h_sys_cluster,
+         (size_t)c->sys_cluster_n * sizeof(tml_sys_node_record) + sizeof(tml_sys_cluster_out));
   return TML_OK;
 }
 

@@ -102,7 +102,7 @@ extern "C" int tml_xs_host_sum(const double* x, uint64_t n, int planned, double*
 #include "tml_sys_sum.h"
 
 extern "C" int tml_sys_host_sum(const double* x, uint64_t n, uint32_t mode, uint32_t nblk, double* out_sum) {
-  if ((!x && n) || !out_sum || mode > 1) return TML_ERR_ARG;
+  if ((!x && n) || !out_sum || mode > 2) return TML_ERR_ARG;
   if (mode == 0) { *out_sum = sys_cpython_sum(x, n); return TML_OK; }
   if (nblk == 0) return TML_ERR_ARG;
   double gh = 0.0, gl = 0.0;
@@ -126,6 +126,13 @@ extern "C" int tml_sys_host_sum(const double* x, uint64_t n, uint32_t mode, uint
     }
     sys_dd_add(gh, gl, bh, bl);
   }
+  if (mode == 2) { out_sum[0] = gh; out_sum[1] = gl; return TML_OK; }
   *out_sum = gh + gl;
+  return TML_OK;
+}
+
+extern "C" int tml_sys_host_cluster(const tml_sys_node_record* records, uint32_t n_records, tml_sys_cluster_out* out) {
+  if ((!records && n_records) || !out || n_records > TML_MAX_RANKS) return TML_ERR_ARG;
+  sys_cluster_fold(records, n_records, out);
   return TML_OK;
 }

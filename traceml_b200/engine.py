@@ -333,6 +333,27 @@ class Engine:
         _abi.check(self._lib.tml_sys_reduce_collect(self._h, C.byref(out)), "tml_sys_reduce_collect")
         return out
 
+    # ---- multi-node System section: header "multi-node System"
+    def sys_node_pack(self, ident: Optional[_abi.SysNodeIdent], d_record, stream: int = 0) -> None:
+        """This rank's node record at device address ``d_record`` (an int or a tensor), behind the
+        last K6s, on ``stream``.  ``ident`` None, or no samples: a record with valid = 0."""
+        _abi.check(self._lib.tml_sys_node_pack(self._h, C.byref(ident) if ident is not None else None,
+                                               _p(d_record), stream), "tml_sys_node_pack")
+
+    def sys_cluster_launch(self, d_records, n_records: int, stream: int = 0) -> None:
+        """K6m over ``n_records`` gathered records at ``d_records``; its result goes right after them."""
+        _abi.check(self._lib.tml_sys_cluster_launch(self._h, _p(d_records), int(n_records), stream),
+                   "tml_sys_cluster_launch")
+
+    def sys_cluster_collect(self, n_records: int):
+        """(the gathered records, in slot order; the ``_abi.SysClusterOut``) of the last K6m."""
+        class _Out(C.Structure):
+            _fields_ = [("records", _abi.SysNodeRecord * int(n_records)), ("cluster", _abi.SysClusterOut)]
+
+        out = _Out()
+        _abi.check(self._lib.tml_sys_cluster_collect(self._h, C.byref(out)), "tml_sys_cluster_collect")
+        return list(out.records), out.cluster
+
     def proc_reduce(self, max_rows: int, stream: int = 0) -> _abi.ProcAgg:
         out = _abi.ProcAgg()
         _abi.check(self._lib.tml_proc_reduce(self._h, int(max_rows), stream, C.byref(out)),

@@ -300,6 +300,66 @@ def build_system(agg: Optional[_abi.SysAgg], identity: Dict[str, Any]) -> Dict[s
             "diagnosis": {"primary": d["primary"], "issues": d["issues"]}}
 
 
+def multi_node_run(comm) -> bool:
+    """Is the System section gathered across nodes?  Only when the run has more than one process
+    and, by the launcher's environment, more than one node: ``ceil(WORLD_SIZE / LOCAL_WORLD_SIZE)
+    > 1``.  Every rank reads the same two variables, so every rank takes the same branch of what
+    is a collective."""
+    if int(getattr(comm, "world", 1)) <= 1:
+        return False
+    try:
+        world, lws = int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_WORLD_SIZE"])
+    except (KeyError, ValueError):
+        return False
+    return lws > 0 and math.ceil(world / lws) > 1
+
+
+def node_ident(identity: Dict[str, Any]) -> _abi.SysNodeIdent:
+    """The record identity of a System source (``reporting.default_identity`` fields)."""
+    i = _abi.SysNodeIdent()
+    i.global_rank = int(identity.get("global_rank") or 0)
+    i.local_rank = int(identity.get("local_rank") or 0)
+    i.node_rank = int(identity["node_rank"]) if identity.get("node_rank") is not None else -1
+    i.world_size = int(identity.get("world_size") or 0)
+    i.local_world_size = int(identity.get("local_world_size") or 0)
+    i.hostname = str(identity.get("hostname") or "").encode()[: _abi.TML_HOSTNAME_MAX - 1]
+    return i
+
+
+def _record_identity(rec: _abi.SysNodeRecord) -> Dict[str, Any]:
+    i = rec.ident
+    ident = {"node_rank": int(i.node_rank) if i.node_rank >= 0 else None,
+             "hostname": i.hostname.decode("utf-8", "replace"), "global_rank": int(i.global_rank),
+             "local_rank": int(i.local_rank), "local_world_size": int(i.local_world_size),
+             "world_size": int(i.world_size)}
+    return dict({"label": system_node_label(ident)}, **ident)
+
+
+def build_system_cluster(host_records: Sequence[_abi.SysNodeRecord], cluster: _abi.SysClusterOut) -> Dict[str, Any]:
+    """The System section of every node from the gathered records and K6m's result: the same
+    shape as ``build_system``, with one entry per node in ``nodes`` (in the string order of their
+    labels, loader.py:300-359), the cluster aggregate over all their samples, the reference's
+    ``expected_nodes`` (loader.py:159-167) and the cluster-wide diagnosis of
+    ``tml_diag_system_cluster``."""
+    kept = [host_records[int(k)] for k in cluster.order[: int(cluster.n_nodes)]]
+    idents = [_record_identity(r) for r in kept]
+    by_label = sorted(zip(idents, kept), key=lambda p: p[0]["label"])
+    din = (_abi.SysDiagIn * max(1, len(by_label)))()
+    for k, (ident, rec) in enumerate(by_label):
+        din[k].node_rank = ident["node_rank"] if ident["node_rank"] is not None else -1
+        din[k].node_label = ident["label"].encode()[:31]
+        din[k].agg = rec.agg
+    d = _abi.diag_system_cluster(din, len(by_label), cluster.agg)
+    nodes = {ident["label"]: {"identity": ident, "aggregate": d["nodes"][ident["label"]]["aggregate"],
+                              "per_gpu": {int(k): v for k, v in d["nodes"][ident["label"]]["per_gpu"].items()}}
+             for ident, _ in by_label}
+    cands = {int(math.ceil(float(i["world_size"]) / float(i["local_world_size"])))
+             for i in idents if i["world_size"] and i["local_world_size"]}
+    expected = max(1, cands.pop()) if len(cands) == 1 else max(1, len(nodes))
+    return {"aggregate": d["aggregate"], "nodes": nodes, "expected_nodes": expected,
+            "diagnosis": {"primary": d["primary"], "issues": d["issues"]}}
+
+
 # ----------------------------------------------------------------------------- driver
 class SummaryEngine:
     """All three sections for the local engines of this process."""
@@ -320,22 +380,70 @@ class SummaryEngine:
         self.ram_total = ram_total
         self.gpu_count = gpu_count
         self._unemitted: Optional[_abi.Sections] = None  # the last native build's sections
-        # the System section has one source: the engine of local rank 0 (comm index 0), whose
-        # system ring the sampler fills; its node identity comes from the launcher's environment
+        # the System section has one source per node: the engine of local rank 0, whose system
+        # ring the sampler fills; its node identity comes from the launcher's environment.  On one
+        # node that is comm index 0; on several, every node leader reduces its own ring and the
+        # records meet on comm index 0 (multi_node_run).
         self.system_identity = system_identity
         self._ident: Optional[Dict[str, Any]] = None
         self._no_system: Optional[Dict[str, Any]] = None
+        self.multi_node = multi_node_run(self.comm)
+        self._node_ident: Optional[Dict[str, Any]] = None
+
+    def _leader_identity(self) -> Dict[str, Any]:
+        if self._node_ident is None:
+            from .reporting import default_identity
+
+            self._node_ident = self.system_identity or default_identity(
+                self.comm.index, max(1, int(self.comm.world)) * max(1, len(self.engines)))
+        return self._node_ident
 
     def _system_launch(self, rows: int):
         """K6s beside the window pass on the engine holding the system ring; None (and nothing
-        launched) when this process has no ring or the ring is empty."""
+        launched) when this process is not its node's source or its ring is empty."""
         eng = self.engines[0] if self.engines else None
-        if self.comm.index != 0 or not hasattr(eng, "sys_reduce_beside") or eng.sys_count == 0:
+        if self.multi_node:
+            source = int(self._leader_identity().get("local_rank") or 0) == 0
+        else:
+            source = self.comm.index == 0
+        if not source or not hasattr(eng, "sys_reduce_beside") or eng.sys_count == 0:
             return None
         eng.sys_reduce_beside(rows, _stream_of(self.reducer.device))
         return eng
 
-    def _system_section(self, eng) -> Dict[str, Any]:
+    def _system_gather(self, eng) -> Optional[Dict[str, Any]]:
+        """Every rank packs its node record in device memory (valid only on a node leader with
+        samples); one all-gather brings them to comm index 0, which folds them (K6m), copies the
+        records and the cluster rollup back in one transfer and runs the cluster rules.  None on
+        every other rank."""
+        import ctypes as C
+
+        import torch
+
+        if eng is not None:
+            eng.sys_reduce_collect()  # ends the launch; the node's aggregates stay in HBM for the pack
+        dev, world = self.reducer.device, int(self.comm.world)
+        rec = C.sizeof(_abi.SysNodeRecord)
+        mine = torch.empty(rec, dtype=torch.uint8, device=dev)
+        gathered = torch.empty(world * rec + C.sizeof(_abi.SysClusterOut), dtype=torch.uint8, device=dev)
+        stream = _stream_of(dev)
+        ident = node_ident(self._leader_identity()) if eng is not None else None
+        self.engines[0].sys_node_pack(ident, mine, stream)
+        self.comm.all_gather_into(gathered[: world * rec], mine)
+        if self.comm.index != 0:
+            return None
+        self.engines[0].sys_cluster_launch(gathered, world, stream)
+        records, cluster = self.engines[0].sys_cluster_collect(world)
+        if cluster.n_dup:
+            import sys
+
+            print(f"[TraceML] System section: {int(cluster.n_dup)} node record(s) repeat a node label; "
+                  "each label keeps the record of its lowest global rank", file=sys.stderr)
+        return build_system_cluster(records, cluster)
+
+    def _system_section(self, eng) -> Optional[Dict[str, Any]]:
+        if self.multi_node:
+            return self._system_gather(eng)
         if self._ident is None:
             from .reporting import default_identity
 
@@ -405,6 +513,6 @@ class SummaryEngine:
 
 
 __all__ = ["SummaryEngine", "build_step_time", "build_step_memory", "build_process", "build_system",
-           "system_node_label",
+           "build_system_cluster", "multi_node_run", "node_ident", "system_node_label",
            "proc_agg_dict", "closest_rank_to_median", "step_time_global", "step_time_overview",
            "step_memory_global", "wait_avg_ms"]

@@ -548,14 +548,19 @@ typedef struct tml_kind_result {
   double t_sums[TML_MAX_RANKS][7];
   double m_sums[TML_MAX_RANKS][4];
   uint32_t has_bands;
-  uint32_t _pad;
+  uint32_t series_paired;            /* 1: rows 2m and 2m+1 are one physical row  */
   double band_sum[TML_SERIES_PER_STEP][3];   /* summed over ranks, rank order     */
   uint64_t band_cnt[TML_SERIES_PER_STEP][3];
   double tail_first[TML_SERIES_PER_STEP];
   double tail_last[TML_SERIES_PER_STEP];
   uint64_t shard_lo, shard_hi;       /* this rank's columns of the series         */
-  const double* series;              /* device, [16][n_common]; owned by the ctx  */
+  const double* series;              /* device, 16 rows of n_common; owned by the ctx */
+  uint64_t series_ld;                /* row stride of `series` in doubles, >= n_common */
 } tml_kind_result;
+/* series row s starts at series + s * series_ld.  The single-rank bulk build stores each
+ * median / worst pair once (one rank: the two are the same value) and maps that row at both
+ * row addresses, series_paired = 1: a write into one row of a pair shows in the other.  Every
+ * other result has series_paired = 0 and series_ld = n_common (16 separate rows). */
 
 typedef struct tml_reduce_run_out {
   uint32_t n_ranks;

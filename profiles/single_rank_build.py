@@ -14,8 +14,9 @@ line:
     Python after it;
   * ``kernel_ms``: device time per build of each kernel (torch.profiler, a run of its own), and
     ``device_idle_ms``: ``build_ms`` minus the pass and the band kernel;
-  * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved, the fused pass's
-    bytes at W = 4e6), CUDA events, median of 25 after warm-up; the fused pass against it;
+  * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved), CUDA events,
+    median of 25 after warm-up; the fused pass against it, counting the bytes it moves: W * 192 when
+    each median / worst series pair is stored once (``series_paired``), W * 256 otherwise;
   * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
 """
 from __future__ import annotations
@@ -167,6 +168,7 @@ def measure(steps: int, window: int, warmup: int) -> dict:
     build_ms = e0.elapsed_time(e1) / steps
     launches = (eng.launch_count - l0) / steps
     fused = bool(getattr(res["reduce"], "fused_rows", False))
+    paired = bool(getattr(res["reduce"], "series_paired", False))
     # (2) host clock around single builds, and the JSON emitter alone on a fresh result
     wall = []
     for _ in range(steps):
@@ -186,11 +188,13 @@ def measure(steps: int, window: int, warmup: int) -> dict:
     med = {k: statistics.median(v) for k, v in stage.items() if not k.startswith("host_")}
     wall_ms, sj_ms = statistics.median(wall), statistics.median(sj)
     ceil = copy_ceiling(torch)
-    fused_bytes = W * 256.0
+    # 128 B record read per step, plus 8 series x 8 B written when the pairs are mapped twice
+    # (series_paired), 16 x 8 B otherwise
+    fused_bytes = W * (192.0 if paired else 256.0)
     k3a = med.get("k3a") or 0.0
     fused_gbps = fused_bytes / (k3a * 1e-3) / 1e9 if k3a else None
     return {
-        "window": W, "steps": steps, "fused_rows": fused,
+        "window": W, "steps": steps, "fused_rows": fused, "series_paired": paired,
         "build_ms": build_ms, "build_wall_ms": wall_ms, "launches_per_build": launches,
         "stage_ms": med, "sections_json_ms": sj_ms,
         "python_rest_ms": wall_ms - med.get("total", 0.0) - sj_ms,

@@ -180,10 +180,10 @@ class KindResultC(C.Structure):
     _fields_ = [("observed", u32), ("n_used", u32), ("used", i32 * TML_MAX_RANKS),
                 ("n_common", u64), ("start_step", u64), ("end_step", u64),
                 ("n_rows", u64 * TML_MAX_RANKS), ("t_sums", (f64 * 7) * TML_MAX_RANKS),
-                ("m_sums", (f64 * 4) * TML_MAX_RANKS), ("has_bands", u32), ("_pad", u32),
+                ("m_sums", (f64 * 4) * TML_MAX_RANKS), ("has_bands", u32), ("series_paired", u32),
                 ("band_sum", (f64 * 3) * 16), ("band_cnt", (u64 * 3) * 16),
                 ("tail_first", f64 * 16), ("tail_last", f64 * 16),
-                ("shard_lo", u64), ("shard_hi", u64), ("series", vp)]
+                ("shard_lo", u64), ("shard_hi", u64), ("series", vp), ("series_ld", u64)]
 
 
 class ReduceRunOut(C.Structure):

@@ -801,12 +801,15 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
 // otherwise it falls back to the staged path.  The extra CTAs of the k_bands launch behind it fold
 // the partials and hand the accumulator over (k_bands).
+// Series row s starts at series + s * ld.  PAIRED: rows 2m and 2m+1 are one physical row mapped
+// twice (tml_summary.cpp), so only the even rows are stored: 64 B out per step instead of 128.
 #define WF_WARP_U4 (2 * 32 * 8)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
 
+template <bool PAIRED>
 __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
     const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
-    double* __restrict__ series, u64 n_ser, WinAcc* acc, double* partials) {
+    double* __restrict__ series, u64 ld, WinAcc* acc, double* partials) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint4* w_in0 = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
@@ -904,14 +907,12 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
         const double wait = fmax(0.0, traced - compute);  // model.py:247
         const double va = (double)pa, vr = (double)pr;
         double* S = series + j;
-        S[0 * n_ser] = dl;     S[1 * n_ser] = dl;
-        S[2 * n_ser] = fwd;    S[3 * n_ser] = fwd;
-        S[4 * n_ser] = bwd;    S[5 * n_ser] = bwd;
-        S[6 * n_ser] = opt;    S[7 * n_ser] = opt;
-        S[8 * n_ser] = traced; S[9 * n_ser] = traced;
-        S[10 * n_ser] = wait;  S[11 * n_ser] = wait;
-        S[12 * n_ser] = va;    S[13 * n_ser] = va;
-        S[14 * n_ser] = vr;    S[15 * n_ser] = vr;
+        auto put = [&](int m, double v) {  // metric m: median row 2m, worst row 2m+1
+          S[(u64)(2 * m) * ld] = v;
+          if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
+        };
+        put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
+        put(4, traced); put(5, wait); put(6, va); put(7, vr);
       }
     }
     __syncwarp();  // `cur` is free again
@@ -1383,6 +1384,7 @@ __global__ void __launch_bounds__(RD_THREADS) k_window_reduce_any(const __grid_c
 
 struct BandParams {
   const double* series;
+  u64 ld;  // row stride of `series` in doubles
   u64 n_common, shard_lo, shard_hi;
   u64 lo[2][3], hi[2][3];
   u64 tail_first[2];
@@ -1412,7 +1414,7 @@ __global__ void __launch_bounds__(256) k_bands(const __grid_constant__ BandParam
     return;
   }
   const int kind = (s >= 12) ? 1 : 0;
-  const double* v = p.series + (u64)s * p.n_common;
+  const double* v = p.series + (u64)s * p.ld;
   if (b == 3) {
     if (threadIdx.x == 0) {
       u64 f = p.tail_first[kind], l = p.n_common ? p.n_common - 1 : 0;
@@ -2731,16 +2733,20 @@ int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_
 
 // k_window_fused on stream s over the retained ring's last `window` rows (n > 0), between ev0 and
 // ev1, into the chained build's accumulator (always armed); *grid_out: its CTAs.  The k_bands launch
-// behind it finalises the pass.
-static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t s, int* grid_out) {
+// behind it finalises the pass.  `ld`: the series' row stride (>= the window's rows); `paired`:
+// store the even rows only (tml_kind_result::series_paired).
+static int fused_pass(tml_ctx* c, uint32_t window, double* series, u64 ld, bool paired, cudaStream_t s,
+                      int* grid_out) {
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
   const u64 t_start = n > window ? n - window : 0;
-  const u64 n_win = n - t_start;
+  if (ld < n - t_start) return set_err(TML_ERR_ARG, "series row stride %llu below the window's %llu rows",
+                                       (unsigned long long)ld, (unsigned long long)(n - t_start));
   if (c->xs_pending) { CK(cudaStreamWaitEvent(s, c->xs_done, 0)); c->xs_pending = false; }
   static bool wf_attr = false;
   if (!wf_attr) {
-    CK(cudaFuncSetAttribute(k_window_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
     wf_attr = true;
   }
   int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
@@ -2748,8 +2754,9 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, cudaStream_t 
   *grid_out = grid;
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   CK(cudaEventRecord(c->ev0, s));
-  k_window_fused<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, n_win,
-                                                         &c->d_final->chain_acc, c->d_partials);
+  auto* kern = paired ? k_window_fused<true> : k_window_fused<false>;
+  kern<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, ld,
+                                               &c->d_final->chain_acc, c->d_partials);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
   c->launches += 1;
@@ -2780,8 +2787,8 @@ static int fused_result(tml_ctx* c, u64 n, u64 window, const WinAcc& acc, const 
 
 // The single-rank bulk pass as one device submission with the band sums chained behind it
 // (tml_internal.h).
-int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
-                                void* stream) {
+int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uint64_t ld, uint32_t paired,
+                                const tml_band_args* bands, void* stream) {
   if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
@@ -2792,12 +2799,13 @@ int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, con
   c->chain_window = window;
   c->chain_pending = false;
   int grid = 0;
-  int rc = fused_pass(c, window, series, s, &grid);
+  int rc = fused_pass(c, window, series, ld, paired != 0, s, &grid);
   if (rc != TML_OK) return rc;
   // k_bands as tml_win_bands launches it, into the packed block's own slots, plus the row of CTAs
   // that finishes the pass
   BandParams p;
-  p.series = series; p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
+  p.series = series; p.ld = ld;
+  p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
   memcpy(p.lo, bands->band_lo, sizeof(p.lo));
   memcpy(p.hi, bands->band_hi, sizeof(p.hi));
   memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
@@ -2858,7 +2866,7 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
   if (n == 0) return TML_OK;
   tml_band_args none;
   memset(&none, 0, sizeof(none));
-  int rc = tml_win_fused_chain_launch_(c, window, series, &none, stream);
+  int rc = tml_win_fused_chain_launch_(c, window, series, n > window ? window : n, 0, &none, stream);
   if (rc != TML_OK) return rc;
   tml_band_out dropped;
   return chain_result(c, s, out, aligned, &dropped, ok);
@@ -3150,7 +3158,8 @@ int tml_win_bands(tml_ctx* c, const double* series, const tml_band_args* a, void
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
   BandParams p;
-  p.series = series; p.n_common = a->n_common; p.shard_lo = a->shard_lo; p.shard_hi = a->shard_hi;
+  p.series = series; p.ld = a->n_common;
+  p.n_common = a->n_common; p.shard_lo = a->shard_lo; p.shard_hi = a->shard_hi;
   memcpy(p.lo, a->band_lo, sizeof(p.lo));
   memcpy(p.hi, a->band_hi, sizeof(p.hi));
   memcpy(p.tail_first, a->tail_first, sizeof(p.tail_first));

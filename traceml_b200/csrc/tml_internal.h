@@ -17,9 +17,10 @@ void tml_run_ws_free_(void* ws);
 // launch: k_window_fused, then k_bands over `series` with `bands` (the host knows n_window, so the
 // band layout, before the pass) and one more row of CTAs that finalises the pass.  finish: one
 // device-to-host copy, one stream wait; then reports what tml_win_fused and tml_win_bands would.
-// *ok = 0: not dense, drop the bands.
-int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, const tml_band_args* bands,
-                                void* stream);
+// *ok = 0: not dense, drop the bands.  Series row s starts at series + s * ld (ld >= the window's
+// rows); paired = 1: rows 2m and 2m+1 share their memory and only the even rows are stored.
+int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uint64_t ld, uint32_t paired,
+                                const tml_band_args* bands, void* stream);
 int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
                                 tml_band_out* band_out, uint32_t* ok);
 

@@ -31,6 +31,8 @@
 #include <mutex>
 #include <vector>
 
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_runtime.h>
 
 #include "../../include/traceml_b200.h"
@@ -106,6 +108,14 @@ struct RunWs {
   u64 cap_presence = 0;
   double* d_series[2] = {nullptr, nullptr};
   u64 cap_series[2] = {0, 0};
+  // the single-rank bulk path's series (see "paired series" below): 8 physical rows of pair_ld
+  // doubles, row m mapped at rows 2m and 2m+1 of a 16-row address range at d_pair
+  int pair_ok = -1;  // -1: not asked yet; 0: plain 16-row buffer (d_series[0]); 1: paired
+  u64 pair_gran = 0;  // mapping granularity, bytes
+  double* d_pair = nullptr;  // reserved address range, 16 * pair_ld doubles
+  u64 pair_ld = 0;
+  CUmemGenericAllocationHandle pair_mem[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  int pair_mapped = 0;  // rows of the range mapped so far
   char* d_recv_rows = nullptr;  // a2a: my shard of every rank's rows
   u64 cap_recv_rows = 0;
   char* d_zero_rows = nullptr;  // a2a: what a rank outside `used` sends
@@ -168,6 +178,158 @@ int grow(T** p, u64* cap, u64 need) {
   u64 n = need + need / 4 + 64;
   CKC(cudaMalloc(p, (size_t)n * sizeof(T)));
   *cap = n;
+  return TML_OK;
+}
+
+// ------------------------------------------------------------------ paired series
+// With one rank the median and the worst series of a metric hold the same values.  The bulk path
+// stores each pair once: 8 physical rows, row m mapped at rows 2m and 2m+1 of a 16-row address
+// range.  Each row is an allocation of its own, since cuMemMap maps a handle from offset 0 only.
+// Every consumer still reads a 16-row series (row stride pair_ld), while the
+// window pass writes 64 B per step instead of 128 -- a quarter of its HBM traffic.  The mapping
+// takes the driver's virtual memory management; its entry points are resolved once through the
+// runtime, so the library keeps no link-time dependency on libcuda.  A device without it, or
+// TML_SERIES_ALIAS=0 (read once per process, for A/B measurements), keeps the plain 16-row buffer.
+struct Vmm {
+  PFN_cuDeviceGetAttribute_v2000 attr = nullptr;
+  PFN_cuMemGetAllocationGranularity_v10020 granularity = nullptr;
+  PFN_cuMemCreate_v10020 create = nullptr;
+  PFN_cuMemRelease_v10020 release = nullptr;
+  PFN_cuMemAddressReserve_v10020 reserve = nullptr;
+  PFN_cuMemAddressFree_v10020 addr_free = nullptr;
+  PFN_cuMemMap_v10020 map = nullptr;
+  PFN_cuMemUnmap_v10020 unmap = nullptr;
+  PFN_cuMemSetAccess_v10020 set_access = nullptr;
+  PFN_cuGetErrorString_v6000 error_string = nullptr;
+  bool ok = false;
+};
+
+Vmm g_vmm;
+std::once_flag g_vmm_once;
+
+void load_vmm() {
+  auto sym = [](const char* name, void* fn) {
+    void** p = (void**)fn;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPointByVersion(name, p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess) {
+      cudaGetLastError();  // not sticky: keep it from surfacing at the next launch check
+      *p = nullptr;
+    }
+    return *p != nullptr;
+  };
+  bool ok = sym("cuDeviceGetAttribute", &g_vmm.attr);
+  ok = sym("cuMemGetAllocationGranularity", &g_vmm.granularity) && ok;
+  ok = sym("cuMemCreate", &g_vmm.create) && ok;
+  ok = sym("cuMemRelease", &g_vmm.release) && ok;
+  ok = sym("cuMemAddressReserve", &g_vmm.reserve) && ok;
+  ok = sym("cuMemAddressFree", &g_vmm.addr_free) && ok;
+  ok = sym("cuMemMap", &g_vmm.map) && ok;
+  ok = sym("cuMemUnmap", &g_vmm.unmap) && ok;
+  ok = sym("cuMemSetAccess", &g_vmm.set_access) && ok;
+  ok = sym("cuGetErrorString", &g_vmm.error_string) && ok;
+  g_vmm.ok = ok;
+}
+
+#define CKD(call)                                                                                      \
+  do {                                                                                                 \
+    CUresult r_ = (call);                                                                              \
+    if (r_ != CUDA_SUCCESS) {                                                                          \
+      const char* s_ = nullptr;                                                                        \
+      g_vmm.error_string(r_, &s_);                                                                     \
+      return tml_set_error_(r_ == CUDA_ERROR_OUT_OF_MEMORY ? TML_ERR_NOMEM : TML_ERR_CUDA,             \
+                            "%s failed: %s (%s:%d)", #call, s_ ? s_ : "unknown error", __FILE__, __LINE__); \
+    }                                                                                                  \
+  } while (0)
+
+CUmemAllocationProp pair_prop(int dev) {
+  CUmemAllocationProp prop;
+  memset(&prop, 0, sizeof(prop));
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = dev;
+  return prop;
+}
+
+// decides w->pair_ok once per workspace (the current device is the context's)
+int pair_mode(RunWs* w) {
+  if (w->pair_ok >= 0) return TML_OK;
+  static const bool off = [] { const char* e = getenv("TML_SERIES_ALIAS"); return e && e[0] == '0'; }();
+  w->pair_ok = 0;
+  if (off) return TML_OK;
+  std::call_once(g_vmm_once, load_vmm);
+  if (!g_vmm.ok) return TML_OK;
+  int dev = 0, vmm = 0;
+  CKC(cudaGetDevice(&dev));
+  CKD(g_vmm.attr(&vmm, CU_DEVICE_ATTRIBUTE_VIRTUAL_MEMORY_MANAGEMENT_SUPPORTED, (CUdevice)dev));
+  if (!vmm) return TML_OK;
+  const CUmemAllocationProp prop = pair_prop(dev);
+  size_t gran = 0;
+  CKD(g_vmm.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM));
+  if (gran == 0 || gran % sizeof(double) != 0) return TML_OK;
+  w->pair_gran = gran;
+  w->pair_ok = 1;
+  return TML_OK;
+}
+
+// unmap, free the address range, release the memory; safe on a partial allocation
+void pair_free(RunWs* w) {
+  const size_t row = (size_t)w->pair_ld * sizeof(double);
+  for (int r = 0; r < w->pair_mapped; ++r) g_vmm.unmap((CUdeviceptr)w->d_pair + r * row, row);
+  if (w->d_pair) g_vmm.addr_free((CUdeviceptr)w->d_pair, 16 * row);
+  for (CUmemGenericAllocationHandle& h : w->pair_mem) {
+    if (h) g_vmm.release(h);
+    h = 0;
+  }
+  w->d_pair = nullptr; w->pair_mapped = 0; w->pair_ld = 0;
+}
+
+int pair_alloc(RunWs* w, u64 ld) {
+  int dev = 0;
+  CKC(cudaGetDevice(&dev));
+  w->pair_ld = ld;
+  const size_t row = (size_t)ld * sizeof(double);
+  const CUmemAllocationProp prop = pair_prop(dev);
+  for (CUmemGenericAllocationHandle& h : w->pair_mem) {
+    CUmemGenericAllocationHandle mem = 0;
+    CKD(g_vmm.create(&mem, row, &prop, 0));
+    h = mem;
+  }
+  CUdeviceptr va = 0;
+  CKD(g_vmm.reserve(&va, 16 * row, w->pair_gran, 0, 0));
+  w->d_pair = (double*)va;
+  for (int r = 0; r < 16; ++r) {
+    CKD(g_vmm.map(va + r * row, row, 0, w->pair_mem[r / 2], 0));
+    w->pair_mapped = r + 1;
+  }
+  CUmemAccessDesc acc;
+  memset(&acc, 0, sizeof(acc));
+  acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  acc.location.id = dev;
+  acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+  CKD(g_vmm.set_access(va, 16 * row, &acc, 1));
+  return TML_OK;
+}
+
+// The bulk path's series for an n-step window: *ld its row stride, *paired whether the rows pair up.
+// The paired range only grows (row stride n rounded up to the granularity); the plain one is
+// d_series[0], which the staged path also uses.
+int bulk_series(RunWs* w, u64 n, double** series, u64* ld, u32* paired) {
+  CKT(pair_mode(w));
+  if (w->pair_ok != 1) {
+    CKT(grow(&w->d_series[0], &w->cap_series[0], (u64)TML_SERIES_PER_STEP * n));
+    *series = w->d_series[0]; *ld = n; *paired = 0;
+    return TML_OK;
+  }
+  const u64 g = w->pair_gran / sizeof(double);
+  const u64 need = (n + g - 1) / g * g;
+  if (!w->d_pair || need > w->pair_ld) {
+    if (w->d_pair) CKC(cudaDeviceSynchronize());  // nothing in flight still touches the old range
+    pair_free(w);
+    const int rc = pair_alloc(w, need);
+    if (rc != TML_OK) { pair_free(w); return rc; }
+  }
+  *series = w->d_pair; *ld = w->pair_ld; *paired = 1;
   return TML_OK;
 }
 
@@ -471,6 +633,7 @@ int reduce_pass(Run& r, u32 kind, u32 mask, u32 mode, KindState* ks, int series_
   RunWs* w = r.w;
   CKT(grow(&w->d_series[series_slot], &w->cap_series[series_slot], (u64)TML_SERIES_PER_STEP * n));
   res->series = w->d_series[series_slot];
+  res->series_ld = n;
   const int W = r.world, g = r.rank;
   const u64 lo = (n * (u64)g) / (u64)W, hi = (n * (u64)(g + 1)) / (u64)W;
   res->shard_lo = lo; res->shard_hi = hi;
@@ -643,12 +806,15 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   CKT(tml_win_peek(c, window, nullptr, &n_win));
   const bool bulk = world == 1 && n_win > (u64)TML_FUSED_MIN_ROWS;
   if (args->proc_rows) CKC(cudaEventRecord(r.w->side_gate, r.s));
+  double* bulk_ser = nullptr;
+  u64 bulk_ld = 0;
+  u32 bulk_paired = 0;
   if (bulk) {
     // the dense series has n_win columns, so the band layout is known before the pass
-    CKT(grow(&r.w->d_series[0], &r.w->cap_series[0], (u64)TML_SERIES_PER_STEP * n_win));
+    CKT(bulk_series(r.w, n_win, &bulk_ser, &bulk_ld, &bulk_paired));
     tml_band_args ba;
     band_args(n_win, 0, n_win, &ba);
-    CKT(tml_win_fused_chain_launch_(c, window, r.w->d_series[0], &ba, r.s));
+    CKT(tml_win_fused_chain_launch_(c, window, bulk_ser, bulk_ld, bulk_paired, &ba, r.s));
   }
   if (args->proc_rows) {
     CKC(cudaStreamWaitEvent(r.w->side, r.w->side_gate, 0));
@@ -679,7 +845,7 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
         res->n_rows[0] = fal.n_rows;
         memcpy(res->t_sums[0], fal.t_sums, sizeof(fal.t_sums));
         memcpy(res->m_sums[0], fal.m_sums, sizeof(fal.m_sums));
-        res->series = r.w->d_series[0];
+        res->series = bulk_ser; res->series_ld = bulk_ld; res->series_paired = bulk_paired;
         res->shard_lo = 0; res->shard_hi = fal.n_common;
       }
       out->exchange_used = TML_XCHG_LOCAL;
@@ -788,7 +954,7 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   out->fused_pass = same ? 1u : 0u;
   if (same) {
     CKT(reduce_pass(r, TML_KIND_TIME, TML_MASK_TIME | TML_MASK_MEM, mode, &kt, 0));
-    out->mem.series = out->time.series;
+    out->mem.series = out->time.series; out->mem.series_ld = out->time.series_ld;
     out->mem.shard_lo = out->time.shard_lo; out->mem.shard_hi = out->time.shard_hi;
   } else {
     if (t.n_common && t.n_used) CKT(reduce_pass(r, TML_KIND_TIME, TML_MASK_TIME, mode_for(r, exchange, t.n_common), &kt, 0));
@@ -862,6 +1028,7 @@ extern "C" void tml_run_ws_free_(void* p) {
   if (!w) return;
   cudaFree(w->d_send); cudaFree(w->d_recv); cudaFreeHost(w->h_send); cudaFreeHost(w->h_recv);
   cudaFree(w->d_presence); cudaFree(w->d_series[0]); cudaFree(w->d_series[1]);
+  pair_free(w);
   cudaFree(w->d_recv_rows); cudaFree(w->d_zero_rows);
   if (w->mbox) munmap(w->mbox, w->mbox_bytes);
   if (w->side) cudaStreamDestroy(w->side);

@@ -251,14 +251,17 @@ class NativeReduceOutput:
     """What ``SummaryEngine.build`` returns as ``"reduce"`` on the native path: the cheap
     facts eagerly, the full ``ReduceOutput`` (per-rank windows, band sums, series view) only
     if somebody asks -- the sections no longer need it.  ``time.series`` / ``mem.series`` are
-    zero-copy views of the engine's own workspace: valid until the engine's next reduce or its
-    ``close()``; ``clone()`` them to keep them."""
+    zero-copy, read-only views of the engine's own workspace: valid until the engine's next reduce
+    or its ``close()``; ``clone()`` them to keep them.  Their row stride may exceed ``n_common``,
+    and when ``series_paired`` is set (the single-rank bulk path) rows 2m and 2m+1 are the same
+    memory mapped twice, so a write into one row would change its partner."""
 
     def __init__(self, reducer: "WindowReducer", o, window: int, proc_rows: Optional[int]):
         self.window = window
         self.exchange = _abi.XCHG_NAME[int(o.exchange_used)]
         self.fused_pass = bool(o.fused_pass)
         self.fused_rows = int(o.fused_pass) == 2  # single-rank bulk path: ring -> series in one kernel
+        self.series_paired = bool(o.time.series_paired)
         self.timings_ms = reducer.native_timings(o)
         self.n_exchanges = int(o.n_exchanges)
         self.ranks = list(range(int(o.n_ranks)))
@@ -555,8 +558,9 @@ class WindowReducer:
                             trend_layout(n, min_points=50, warmup_frac=0.0))
             if k.series and n:
                 from .engine import _DevView
-                res.series = torch.as_tensor(_DevView(int(k.series), _abi.TML_SERIES_PER_STEP * n),
-                                             device=self.device).view(_abi.TML_SERIES_PER_STEP, n)
+                ld = int(k.series_ld)
+                res.series = torch.as_tensor(_DevView(int(k.series), _abi.TML_SERIES_PER_STEP * ld),
+                                             device=self.device).view(_abi.TML_SERIES_PER_STEP, ld)[:, :n]
             res.shard = (int(k.shard_lo), int(k.shard_hi))
             return res
 

@@ -156,6 +156,25 @@ int tml_step_commit(tml_ctx* ctx, uint64_t step, uint64_t peak_alloc,
 /* Drop whatever the open step accumulated (TRACEML_DISABLED / failed setup). */
 int tml_step_discard(tml_ctx* ctx);
 
+/* ------------------------------------------------- GRAPH-CAPTURED REGIONS
+ * tml_phase_begin / _end return TML_ERR_CAPTURE on a capturing stream.  These
+ * capture the same stamp kernels into the graph `stream` is capturing, so the
+ * region is timed on every replay and adds to the step that is open on the
+ * device when the replay runs (the end stamp reads the epoch from the device's
+ * commit head).  They need a capturing stream (else TML_ERR_STATE).  The begin
+ * returns the region's graph slot, its nesting depth at capture time; at most
+ * 64 graph regions are open at once (else TML_ERR_STATE), and an end must close
+ * the innermost one (else TML_ERR_ARG).  The first stamp of each capture moves
+ * a CUDA user object into the graph: while that graph or an exec made from it
+ * lives, tml_shutdown keeps the context's device state allocated (and returns
+ * the number of such graphs instead of TML_OK), and tml_layer_init returns
+ * TML_ERR_STATE if the graph holds layer stamps. */
+int tml_graph_phase_begin(tml_ctx* ctx, uint32_t phase, void* stream);
+int tml_graph_phase_end(tml_ctx* ctx, uint32_t phase, int slot, void* stream);
+/* Graphs (and execs) in this process still holding some context's device
+ * state.  Takes no context: it stays readable after tml_shutdown. */
+uint64_t tml_graph_refs(void);
+
 /* ------------------------------------------------------- SAMPLER-SIDE (host)
  * Called from the sampler thread; never touches the training stream. */
 
@@ -778,6 +797,11 @@ int tml_layer_end(tml_ctx* ctx, uint32_t layer, uint32_t direction, int slot, ui
 int tml_layer_commit(tml_ctx* ctx, uint64_t step, void* stream);
 int tml_layer_drain(tml_ctx* ctx, tml_layer_record* out, uint32_t max_steps, uint32_t* n_steps,
                     uint32_t* n_layers, uint64_t* n_dropped);
+/* Graph-captured layer regions: tml_layer_begin / _end for a capturing stream, with the
+ * rules of tml_graph_phase_begin / _end (own 64 graph slots, LIFO). */
+int tml_graph_layer_begin(tml_ctx* ctx, void* stream);
+int tml_graph_layer_end(tml_ctx* ctx, uint32_t layer, uint32_t direction, int slot, uint64_t bytes,
+                        void* stream);
 
 /* ---------------------------------------------------------------- TEST HOOK
  * Host emulation of K3e -- the reference-order window sums (``s += x`` per row:

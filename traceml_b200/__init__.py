@@ -25,6 +25,7 @@ _LAZY = {
     "init": ("traceml_b200.sdk", "init"),
     "start": ("traceml_b200.sdk", "start"),
     "trace_step": ("traceml_b200.sdk", "trace_step"),
+    "trace_graph": ("traceml_b200.sdk", "trace_graph"),
     "trace_time": ("traceml_b200.sdk", "trace_time"),
     "trace_model_instance": ("traceml_b200.sdk", "trace_model_instance"),
     "wrap_dataloader_fetch": ("traceml_b200.sdk", "wrap_dataloader_fetch"),

@@ -243,6 +243,11 @@ SIGNATURES = {
     "tml_phase_host": (C.c_int, [vp, u32, u64]),
     "tml_step_commit": (C.c_int, [vp, u64, u64, u64, u32, f64, vp]),
     "tml_step_discard": (C.c_int, [vp]),
+    "tml_graph_phase_begin": (C.c_int, [vp, u32, vp]),
+    "tml_graph_phase_end": (C.c_int, [vp, u32, C.c_int, vp]),
+    "tml_graph_layer_begin": (C.c_int, [vp, vp]),
+    "tml_graph_layer_end": (C.c_int, [vp, u32, u32, C.c_int, u64, vp]),
+    "tml_graph_refs": (u64, []),
     "tml_drain": (C.c_int, [vp, vp, u32, C.POINTER(u32), C.POINTER(u64)]),
     "tml_live": (C.c_int, [vp, C.POINTER(LiveStats)]),
     "tml_proc_commit": (C.c_int, [vp, C.POINTER(ProcRecord), vp]),

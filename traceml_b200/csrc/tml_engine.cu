@@ -50,7 +50,11 @@ static_assert(sizeof(tml_proc_record) == 64, "ProcRecord must be 64 B");
 static_assert(sizeof(tml_sys_gpu) == 32 && sizeof(tml_sys_record) == 576, "SysRecord must be 64 + 16 x 32 B");
 
 #define TML_N_SLOTS 64u      // begin-timestamp slots (regions in flight)
+#define TML_N_GSLOTS 64u     // begin slots of graph-captured regions, after the host-launched ones
 #define TML_N_EPOCHS 8u      // in-flight accumulator sets (steps in flight)
+// k_stamp_end epoch of a graph-captured stamp: its launch arguments are frozen at capture, so it
+// takes the epoch from the device's commit head (head == host commits in stream order)
+#define TML_EPOCH_FROM_HEAD 0xffffffffu
 #define TML_HIST_BINS 256u
 
 // row flags written by k_window_rows
@@ -70,7 +74,8 @@ struct DevAcc {
 };
 
 struct DevState {
-  u64 begin_ts[TML_N_SLOTS];
+  u64 begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // host-launched regions rotate through the first bank;
+                                             // graph regions own slot TML_N_SLOTS + capture depth
   DevAcc acc[TML_N_EPOCHS];
   u64 head;       // step records committed
   u64 proc_head;  // proc records committed
@@ -78,8 +83,9 @@ struct DevState {
   u64 live_max[TML_MAX_PHASES];
   u32 hist[TML_N_PHASES][TML_HIST_BINS];
   tml_live_stats live;  // running count / sum / worst / median per phase (k_mirror copies it out)
-  u64 layer_begin_ts[TML_N_SLOTS];  // deep profile: its own begin slots (hundreds of layer regions
-                                    // open and close while ONE phase region stays open)
+  u64 layer_begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // deep profile: its own begin slots (hundreds of layer
+                                                   // regions open and close while ONE phase region stays
+                                                   // open), same two banks as begin_ts
 };
 
 // host-mapped page: written by kernels, read by the sampler thread with no CUDA call
@@ -164,11 +170,14 @@ __global__ void k_stamp_begin(DevState* st, u32 slot) {
   if (threadIdx.x == 0) st->begin_ts[slot] = globaltimer_ns();
 }
 
-__global__ void k_stamp_end(DevState* st, u32 slot, u32 phase, u32 epoch) {
+// With a register cap (24 is the lowest ptxas accepts) ptxas keeps the 16 registers the kernel had
+// before the graph epoch, with no spills; left to itself it takes 18 to hoist the head load's address.
+__global__ void __maxnreg__(24) k_stamp_end(DevState* st, u32 slot, u32 phase, u32 epoch) {
   if (threadIdx.x == 0) {
     u64 t1 = globaltimer_ns();
     u64 t0 = st->begin_ts[slot];
     u64 d = (t1 > t0) ? (t1 - t0) : 0ull;
+    if (epoch == TML_EPOCH_FROM_HEAD) epoch = (u32)(st->head % TML_N_EPOCHS);  // graph replay
     DevAcc* a = &st->acc[epoch];
     atomicAdd(&a->dur_ns[phase], d);
     atomicAdd(&a->n_calls[phase], 1u);
@@ -1837,6 +1846,33 @@ struct StagePage {
   double proc[PR_COLS];
 };
 
+// Graph-captured stamps hold raw pointers to a context's DevState and layer accumulators for as long
+// as the graph (or any exec instantiated from it) lives.  Each capture that records a stamp moves one
+// CUDA user object into its graph; CUDA runs graph_release once the graph, every exec and their
+// in-flight work are gone.  GraphRefs counts those objects for the context, which keeps its device
+// state while the count is not zero.  It is freed by whichever of the context and the last user
+// object goes last.
+struct GraphRefs {
+  std::atomic<u64> graphs{0};        // live user objects holding this context's device state
+  std::atomic<u64> layer_graphs{0};  // ... of which hold layer stamps too
+  std::atomic<u32> owners{1};        // the context + each live user object
+};
+struct GraphCapture {  // one user object's payload
+  GraphRefs* refs;
+  bool layers;         // the capture recorded a layer stamp (set at capture time, under graph_mu)
+};
+static std::atomic<u64> g_graph_refs{0};  // process-wide: tml_graph_refs
+
+static void graph_release(void* p) {  // CUDA user-object destructor: it may make no CUDA call
+  GraphCapture* gc = static_cast<GraphCapture*>(p);
+  GraphRefs* r = gc->refs;
+  if (gc->layers) r->layer_graphs.fetch_sub(1);
+  r->graphs.fetch_sub(1);
+  g_graph_refs.fetch_sub(1);
+  if (r->owners.fetch_sub(1) == 1) delete r;
+  delete gc;
+}
+
 struct tml_ctx {
   int device = 0, rank = 0, world = 1;
   int n_sms = 132;
@@ -1855,6 +1891,12 @@ struct tml_ctx {
   u64 commits = 0;
   u64 launches = 0;  // kernels this context has launched (bench: gpu_launches)
   u32 next_slot = 0;
+  // graph-captured regions (tml_graph_*): capture-time host state, behind graph_mu
+  std::mutex graph_mu;
+  u32 graph_depth = 0, graph_layer_depth = 0;  // open regions = the next graph slot (LIFO)
+  unsigned long long graph_capture = 0;        // capture sequence that holds graph_cur
+  GraphCapture* graph_cur = nullptr;
+  GraphRefs* graph_refs = nullptr;
   u64 host_dur[TML_MAX_PHASES] = {0};
   u32 host_calls[TML_MAX_PHASES] = {0};
   // sampler-thread state
@@ -2073,6 +2115,8 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   c->n_sms = sms > 0 ? sms : 132;
+  c->graph_refs = new (std::nothrow) GraphRefs();
+  if (!c->graph_refs) { delete c; return set_err(TML_ERR_NOMEM, "tml_init: host allocation failed"); }
   CK(cudaMalloc(&c->d_state, sizeof(DevState)));
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   CK(cudaMalloc(&c->d_ring, (size_t)ring_slots * sizeof(tml_step_record)));
@@ -2110,14 +2154,19 @@ int tml_shutdown(tml_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   for (auto& kv : c->peers) cudaIpcCloseMemHandle(kv.second);
-  cudaFree(c->d_state); cudaFree(c->d_ring); cudaFree(c->d_pring);
+  // a live graph's stamps still write into the DevState and the layer accumulators: those few KB
+  // stay allocated for the rest of the process
+  const u64 graphs_live = c->graph_refs->graphs.load();
+  if (!graphs_live) { cudaFree(c->d_state); cudaFree(c->d_layer_acc); }
+  if (c->graph_refs->owners.fetch_sub(1) == 1) delete c->graph_refs;
+  cudaFree(c->d_ring); cudaFree(c->d_pring);
   cudaFreeHost(c->h_page); cudaFreeHost(c->h_mirror); cudaFreeHost(c->h_pmirror);
   cudaFree(c->d_rows); cudaFree(c->d_steps); cudaFree(c->d_flags);
   for (int k = 0; k < 2; ++k) { cudaFree(c->d_rowof[k]); cudaFree(c->d_xrows[k]); }
   cudaFree(c->d_selrow); cudaFree(c->d_selstep); cudaFree(c->d_blockcnt); cudaFree(c->d_total);
   cudaFree(c->d_noncontig); cudaFree(c->d_gacc);
   cudaFree(c->d_xs_buf); cudaFree(c->d_xs_out); cudaFree(c->d_xs_stats);
-  cudaFree(c->d_layer_acc); cudaFree(c->d_layer_ring); cudaFree(c->d_layer_head);
+  cudaFree(c->d_layer_ring); cudaFree(c->d_layer_head);
   if (c->h_layer_stage) cudaFreeHost(c->h_layer_stage);
   if (c->drain_stream) cudaStreamDestroy(c->drain_stream);
   if (c->xs_stream) cudaStreamDestroy(c->xs_stream);
@@ -2135,7 +2184,7 @@ int tml_shutdown(tml_ctx* c) {
   comb_free(c);
   tml_run_ws_free_(c->run_ws);
   delete c;
-  return TML_OK;
+  return graphs_live ? (int)(graphs_live < 0x7fffffffull ? graphs_live : 0x7fffffffull) : TML_OK;
 }
 
 // ---------------------------------------------------------------- step path
@@ -2183,9 +2232,93 @@ int tml_phase_end(tml_ctx* c, uint32_t phase, int slot, void* stream) {
   return TML_OK;
 }
 
+// ---------------------------------------------------------------- graph-captured regions
+// The stamps are captured into the graph that `stream` is capturing and run on every replay.  They
+// use the second bank of begin slots (slot = nesting depth at capture time, handed out LIFO) and
+// k_stamp_end reads the epoch from the device head.  Capture time is not a hot path: the host state
+// sits behind graph_mu.
+
+}  // extern "C"
+
+// The graph that `s` is capturing holds this context's device state: one user object per capture
+// sequence, created by its first stamp.  `layers`: the stamp writes the layer accumulators.
+// Caller holds graph_mu.
+static int graph_hold(tml_ctx* c, cudaStream_t s, bool layers, const char* what) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  unsigned long long id = 0;
+  cudaGraph_t g = nullptr;
+  if (cudaStreamGetCaptureInfo(s, &st, &id, &g) != cudaSuccess) {
+    return set_err(TML_ERR_STATE, "%s: capture info: %s", what, cudaGetErrorString(cudaGetLastError()));
+  }
+  if (st != cudaStreamCaptureStatusActive || !g) return set_err(TML_ERR_STATE, "%s: stream is not capturing", what);
+  if (id != c->graph_capture || !c->graph_cur) {
+    GraphCapture* gc = new (std::nothrow) GraphCapture{c->graph_refs, false};
+    if (!gc) return set_err(TML_ERR_NOMEM, "%s: host allocation failed", what);
+    cudaUserObject_t obj;
+    if (cudaUserObjectCreate(&obj, gc, graph_release, 1, cudaUserObjectNoDestructorSync) != cudaSuccess) {
+      delete gc;
+      return set_err(TML_ERR_CUDA, "%s: user object: %s", what, cudaGetErrorString(cudaGetLastError()));
+    }
+    c->graph_refs->owners.fetch_add(1);
+    c->graph_refs->graphs.fetch_add(1);
+    g_graph_refs.fetch_add(1);
+    if (cudaGraphRetainUserObject(g, obj, 1, cudaGraphUserObjectMove) != cudaSuccess) {
+      const cudaError_t e = cudaGetLastError();
+      cudaUserObjectRelease(obj, 1);  // graph_release undoes the counts
+      return set_err(TML_ERR_CUDA, "%s: retain user object: %s", what, cudaGetErrorString(e));
+    }
+    c->graph_capture = id;
+    c->graph_cur = gc;  // alive while capture `id` is active: its graph holds the object
+  }
+  if (layers && !c->graph_cur->layers) {
+    c->graph_cur->layers = true;
+    c->graph_refs->layer_graphs.fetch_add(1);
+  }
+  return TML_OK;
+}
+
+extern "C" {
+
+int tml_graph_phase_begin(tml_ctx* c, uint32_t phase, void* stream) {
+  if (!c || phase >= TML_MAX_PHASES) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  if (c->graph_depth >= TML_N_GSLOTS)
+    return set_err(TML_ERR_STATE, "tml_graph_phase_begin: %u graph regions already open", TML_N_GSLOTS);
+  int rc = graph_hold(c, s, false, "tml_graph_phase_begin");
+  if (rc != TML_OK) return rc;
+  const u32 slot = c->graph_depth;
+  k_stamp_begin<<<1, 32, 0, s>>>(c->d_state, TML_N_SLOTS + slot);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph stamp_begin capture: %s", cudaGetErrorString(cudaGetLastError()));
+  c->graph_depth = slot + 1u;
+  return (int)slot;
+}
+
+int tml_graph_phase_end(tml_ctx* c, uint32_t phase, int slot, void* stream) {
+  if (!c || phase >= TML_MAX_PHASES || slot < 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  if ((u32)slot + 1u != c->graph_depth)
+    return set_err(TML_ERR_ARG, "tml_graph_phase_end: slot %d is not the innermost open graph region", slot);
+  c->graph_depth = (u32)slot;  // the region is closed on the host whatever the capture does below
+  int rc = graph_hold(c, s, false, "tml_graph_phase_end");
+  if (rc != TML_OK) return rc;
+  k_stamp_end<<<1, 32, 0, s>>>(c->d_state, TML_N_SLOTS + (u32)slot, phase, TML_EPOCH_FROM_HEAD);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph stamp_end capture: %s", cudaGetErrorString(cudaGetLastError()));
+  return TML_OK;
+}
+
+uint64_t tml_graph_refs(void) { return g_graph_refs.load(); }
+
 // ---------------------------------------------------------------- deep profile
 int tml_layer_init(tml_ctx* c, uint32_t n_layers, uint32_t steps) {
   if (!c || n_layers == 0 || steps == 0) return TML_ERR_ARG;
+  if (c->graph_refs->layer_graphs.load() > 0)
+    return set_err(TML_ERR_STATE, "tml_layer_init: a live CUDA graph holds layer stamps into the current accumulators");
   DeviceGuard dg(c);
   cudaFree(c->d_layer_acc); cudaFree(c->d_layer_ring); cudaFree(c->d_layer_head);
   if (c->h_layer_stage) cudaFreeHost(c->h_layer_stage);
@@ -2224,6 +2357,41 @@ int tml_layer_end(tml_ctx* c, uint32_t layer, uint32_t direction, int slot, uint
   c->launches += 1;
   if (cudaPeekAtLastError() != cudaSuccess)
     return set_err(TML_ERR_CUDA, "layer_end launch: %s", cudaGetErrorString(cudaGetLastError()));
+  return TML_OK;
+}
+
+// graph-captured layer regions: the second bank of layer begin slots, LIFO by capture depth
+int tml_graph_layer_begin(tml_ctx* c, void* stream) {
+  if (!c) return TML_ERR_ARG;
+  if (!c->n_layers) return TML_ERR_STATE;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  if (c->graph_layer_depth >= TML_N_GSLOTS)
+    return set_err(TML_ERR_STATE, "tml_graph_layer_begin: %u graph layer regions already open", TML_N_GSLOTS);
+  int rc = graph_hold(c, s, true, "tml_graph_layer_begin");
+  if (rc != TML_OK) return rc;
+  const u32 slot = c->graph_layer_depth;
+  k_layer_begin<<<1, 32, 0, s>>>(c->d_state, TML_N_SLOTS + slot);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph layer_begin capture: %s", cudaGetErrorString(cudaGetLastError()));
+  c->graph_layer_depth = slot + 1u;
+  return (int)slot;
+}
+
+int tml_graph_layer_end(tml_ctx* c, uint32_t layer, uint32_t direction, int slot, uint64_t bytes, void* stream) {
+  if (!c || !c->n_layers || layer >= c->n_layers || direction > 1 || slot < 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  if ((u32)slot + 1u != c->graph_layer_depth)
+    return set_err(TML_ERR_ARG, "tml_graph_layer_end: slot %d is not the innermost open graph layer region", slot);
+  c->graph_layer_depth = (u32)slot;
+  int rc = graph_hold(c, s, true, "tml_graph_layer_end");
+  if (rc != TML_OK) return rc;
+  k_layer_end<<<1, 32, 0, s>>>(c->d_state, c->d_layer_acc, TML_N_SLOTS + (u32)slot, layer, direction, bytes);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph layer_end capture: %s", cudaGetErrorString(cudaGetLastError()));
   return TML_OK;
 }
 

@@ -46,6 +46,8 @@ class Engine:
         self._end = self._lib.tml_phase_end
         self._host = self._lib.tml_phase_host
         self._commit = self._lib.tml_step_commit
+        self._gbegin = self._lib.tml_graph_phase_begin  # regions captured into a CUDA graph
+        self._gend = self._lib.tml_graph_phase_end
         self._drain_buf = np.zeros(4096, dtype=STEP_RECORD_DTYPE)
         self._pdrain_buf = np.zeros(8192, dtype=PROC_RECORD_DTYPE)
         self._run_out = _abi.ReduceRunOut()
@@ -55,7 +57,9 @@ class Engine:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def close(self) -> None:
+    def close(self) -> int:
+        """Free the context.  Returns the number of live CUDA graphs whose captured stamps still
+        hold its device state, which then stays allocated (0: everything was freed)."""
         if getattr(self, "_h", None) is not None and self._h.value:
             # the step glue / native sampler hold this context's raw pointer: unbind them first
             import sys
@@ -63,8 +67,10 @@ class Engine:
             timing = sys.modules.get("traceml_b200.utils.timing")
             if timing is not None and getattr(timing, "_ENG", None) is self:
                 timing._reset()
-            self._lib.tml_shutdown(self._h)
+            rc = self._lib.tml_shutdown(self._h)
             self._h = C.c_void_p()
+            return max(0, int(rc))
+        return 0
 
     def __del__(self):  # best effort
         try:

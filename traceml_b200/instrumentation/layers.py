@@ -9,6 +9,9 @@ a layer id: a layer call is two 1-warp ``%globaltimer`` stamps on the current st
 output bytes into the layer's device accumulators; ``tml_layer_commit`` at the step boundary
 snapshots all layers into a device ring, ``tml_layer_drain`` (sampler side, own stream) brings
 finished steps to the host.  No events, no queues, no host synchronisation on the training thread.
+While a ``trace_graph`` scope is open, a layer call on a capturing stream captures its stamps into
+the graph (``tml_graph_layer_begin`` / ``_end``), so every replay adds to the layer's records; the
+scope is checked process-wide because backward hooks run on autograd's device thread.
 
 Which modules are hooked is the reference's decision logic (``utils/shared_utils.py:11-37``): leaf
 modules by default, ``include_names`` / ``exclude_names`` substring filters.  Hooks are attached
@@ -25,6 +28,7 @@ import torch
 import torch.nn as nn
 
 from .. import _abi
+from ..utils.timing import GRAPH_SCOPES_OPEN, GRAPH_SLOT0
 
 LAYER_RECORD_DTYPE = np.dtype([("step", "<u8"), ("fwd_ns", "<u8"), ("bwd_ns", "<u8"), ("fwd_calls", "<u4"),
                                ("bwd_calls", "<u4"), ("fwd_bytes", "<u8"), ("bwd_bytes", "<u8")])
@@ -80,27 +84,45 @@ class LayerProfile:
         raw_stream = torch._C._cuda_getCurrentRawStream
         dev = engine.device
         h, begin, end = engine._h, self._lib.tml_layer_begin, self._lib.tml_layer_end
+        gbegin, gend = self._lib.tml_graph_layer_begin, self._lib.tml_graph_layer_end
+
+        def graph_begin(status, stream):
+            """A capturing stream inside trace_graph: the layer's stamps go into the graph."""
+            if status == _abi.TML_ERR_CAPTURE and GRAPH_SCOPES_OPEN[0]:
+                g = gbegin(h, stream)
+                if g >= 0:
+                    return GRAPH_SLOT0 - g
+            return status
+
         for lid, (_, m) in enumerate(mods):
             slots: List[int] = []   # a module may be re-entered (shared layers): FIFO like the reference's deque
             bslots: List[int] = []
 
             def pre(mod, args, _s=slots):
-                _s.append(begin(h, raw_stream(dev)))
+                stream = raw_stream(dev)
+                slot = begin(h, stream)
+                _s.append(slot if slot >= 0 else graph_begin(slot, stream))
 
             def post(mod, args, out, _s=slots, _lid=lid):
                 if _s:
                     slot = _s.pop(0)
                     if slot >= 0:
                         end(h, _lid, 0, slot, _tensor_bytes(out), raw_stream(dev))
+                    elif slot <= GRAPH_SLOT0:
+                        gend(h, _lid, 0, GRAPH_SLOT0 - slot, _tensor_bytes(out), raw_stream(dev))
 
             def bpre(mod, gout, _s=bslots):
-                _s.append(begin(h, raw_stream(dev)))
+                stream = raw_stream(dev)
+                slot = begin(h, stream)
+                _s.append(slot if slot >= 0 else graph_begin(slot, stream))
 
             def bpost(mod, gin, gout, _s=bslots, _lid=lid):
                 if _s:
                     slot = _s.pop(0)
                     if slot >= 0:
                         end(h, _lid, 1, slot, _tensor_bytes(gout), raw_stream(dev))
+                    elif slot <= GRAPH_SLOT0:
+                        gend(h, _lid, 1, GRAPH_SLOT0 - slot, _tensor_bytes(gout), raw_stream(dev))
 
             if forward:
                 self.handles.append(m.register_forward_pre_hook(pre, prepend=outermost))

@@ -164,6 +164,61 @@ class trace_step:
         return False
 
 
+class trace_graph:
+    """``with trace_graph(model): ...`` around a CUDA-graph capture of training work::
+
+        g = torch.cuda.CUDAGraph()
+        with traceml.trace_graph(model), torch.cuda.graph(g):
+            loss = model(static_x).loss; loss.backward(); opt.step()
+        for batch in loader:
+            with traceml.trace_step(model):
+                static_x.copy_(batch); g.replay()
+
+    Arms the forward / backward / h2d openers of ``trace_step`` for the capture, and lets every
+    device-timed region opened on a capturing stream (those, the optimizer hooks, ``trace_time``
+    regions, deep-profile layers) capture its stamps into the graph.  Each replay then adds those
+    regions' durations and calls to the step open on the device when it runs.  Opens no step and
+    commits nothing.  Do not wrap ``torch.cuda.make_graphed_callables`` in it: its replays already
+    run through the module and backward openers, so their regions would count twice."""
+
+    __slots__ = ("model", "flags")
+
+    def __init__(self, model=None):
+        self.model = model
+        self.flags = None
+
+    def __enter__(self):
+        if disabled():
+            return self
+        if _timing._ENG is None:
+            # the engine's first region allocates device memory: never inside the capture
+            try:
+                _timing._resolve()
+            except _timing._Quiet:
+                pass  # reported once by _resolve
+            except Exception as exc:
+                _log("engine start failed", exc)
+        self.flags = _patches.step_auto_timers(self.model)
+        self.flags.__enter__()
+        _timing.GRAPH_SCOPE.depth += 1
+        _timing.GRAPH_SCOPES_OPEN[0] += 1
+        try:
+            if _auto_optimizer():
+                _patches.ensure_optimizer_timing_installed()
+        except Exception as exc:
+            _log("optimizer hook install failed", exc)
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        if self.flags is None:
+            return False
+        _timing.GRAPH_SCOPES_OPEN[0] -= 1
+        _timing.GRAPH_SCOPE.depth -= 1
+        self.flags.__exit__(exc_type, exc, tb)
+        self.flags = None
+        return False
+
+
 def trace_model_instance(model, sample_layer_memory: bool = True, trace_layer_forward_memory: bool = True,
                          trace_layer_backward_memory: bool = True, trace_layer_forward_time: bool = True,
                          trace_layer_backward_time: bool = True, trace_execution: bool = True,
@@ -228,4 +283,4 @@ class TraceState(metaclass=_TraceStateMeta):
         return get_trace_session_state().advance_step(delta)
 
 
-__all__ = ["trace_step", "trace_model_instance", "trace_time", "TraceState"]
+__all__ = ["trace_step", "trace_graph", "trace_model_instance", "trace_time", "TraceState"]

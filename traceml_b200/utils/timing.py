@@ -12,16 +12,23 @@ Semantics kept (SURVEY 8a): repeated regions within a step sum and count
 ``n_calls``; ``use_gpu=False`` regions are host-clock; GLOBAL-scope regions run
 but are not recorded (``utils/timing.py:123-134`` drops them too); telemetry
 errors never reach user code.
+
+Under CUDA-graph capture the stamp entry points return ``TML_ERR_CAPTURE`` and the
+region takes the host clock, unless a ``trace_graph`` scope is open on this thread:
+then the stamps are captured into the graph (``tml_graph_phase_begin`` / ``_end``)
+and time the region on every replay.
 """
 from __future__ import annotations
 
 import os
 import sys
+import threading
 import time
 from dataclasses import dataclass
 from enum import Enum
 from typing import Any, Optional
 
+from .._abi import TML_ERR_CAPTURE
 from ..records import (PHASE_BACKWARD, PHASE_DATALOADER, PHASE_EVENT_NAMES, PHASE_FORWARD,
                        PHASE_OPTIMIZER, PHASE_STEP)
 from ..runtime import disabled, get_engine
@@ -36,6 +43,19 @@ _FAST = None        # traceml_b200._tml_step bound to that engine (None: ctypes 
 
 
 _RESOLVE_FAILED: Optional[str] = None  # a failed engine resolution is cached and printed once
+
+# A region captured into a CUDA graph (tml_graph_phase_begin) keeps its graph slot g in ``slot`` as
+# GRAPH_SLOT0 - g: below every status code, so the plain path's ``slot >= 0`` test is unchanged.
+GRAPH_SLOT0 = -(1 << 16)
+
+
+class _GraphScope(threading.local):
+    depth = 0   # open trace_graph scopes on this thread
+
+
+GRAPH_SCOPE = _GraphScope()
+GRAPH_SCOPES_OPEN = [0]  # open trace_graph scopes in the process (layer backward hooks run on
+                         # autograd's device thread, not on the thread that opened the scope)
 
 
 def _resolve():
@@ -171,6 +191,11 @@ class timed_region:
                 else:
                     self.slot = eng._begin(eng._h, self.phase, _raw_stream(_cur_dev()))
                 if self.slot < 0:
+                    if self.slot == TML_ERR_CAPTURE and GRAPH_SCOPE.depth:  # inside trace_graph
+                        g = eng._gbegin(eng._h, self.phase, _raw_stream(_cur_dev()))
+                        if g >= 0:
+                            self.slot = GRAPH_SLOT0 - g
+                            return self
                     self.t0 = _perf_ns()  # graph capture / launch failure: host clock
             else:
                 self.t0 = _perf_ns()
@@ -189,17 +214,27 @@ class timed_region:
             if fast is not None:
                 if self.slot >= 0:
                     fast.end(self.phase, self.slot)
-                else:
+                elif self.slot > GRAPH_SLOT0:
                     fast.host(self.phase, _perf_ns() - self.t0)
+                else:
+                    self._graph_end()
             else:
                 eng = self.eng
                 if self.slot >= 0:
                     eng._end(eng._h, self.phase, self.slot, _raw_stream(_cur_dev()))
-                else:
+                elif self.slot > GRAPH_SLOT0:
                     eng._host(eng._h, self.phase, _perf_ns() - self.t0)
+                else:
+                    self._graph_end()
         except Exception as e:  # nothing here may break training
             print(f"[TraceML] timed_region teardown failed: {e}", file=sys.stderr)
         return False
+
+    def _graph_end(self):
+        eng = self.eng
+        rc = eng._gend(eng._h, self.phase, GRAPH_SLOT0 - self.slot, _raw_stream(_cur_dev()))
+        if rc < 0:
+            print(f"[TraceML] graph region not closed (status {rc})", file=sys.stderr)
 
 
 def record_event(evt: TimeEvent) -> None:

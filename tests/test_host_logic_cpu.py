@@ -6,7 +6,6 @@ import numpy as np
 import pytest
 
 from oracle import step_time_oracle, trend_oracle
-from traceml_b200 import sections
 from traceml_b200.reduce import WindowReducer, trend_layout
 
 
@@ -34,21 +33,38 @@ def test_info_pack_roundtrip():
     assert WindowReducer._info_unpack([float(x) for x in v]) == d
 
 
-def test_rollups_match_oracle_on_random_ranks():
+def _step_time_of_sums(sums_by_rank, n):
+    """The Step-Time section tml_sections_json emits for a reduce whose aligned window holds ``n``
+    steps of every rank in ``sums_by_rank`` with these seven per-metric sums."""
+    from traceml_b200 import _abi
+
+    o = _abi.ReduceRunOut()
+    o.n_ranks = max(1, len(sums_by_rank))
+    k = o.time
+    k.observed = k.n_used = len(sums_by_rank)
+    k.n_common = n
+    for i, (r, s) in enumerate(sorted(sums_by_rank.items())):
+        k.used[i], k.n_rows[i] = r, n
+        k.t_sums[i][:] = s
+    return _abi.sections_json(o, 1.0e9, 1, 10_000, 0)["step_time"]
+
+
+def test_emitted_rollups_match_oracle_on_random_ranks():
     rnd = random.Random(3)
     for R in (1, 2, 3, 4, 7, 8):
-        summ = {}
+        n = rnd.randint(1, 500)
+        sums = {}
         for r in range(R):
-            f, b, o = rnd.uniform(5, 15), rnd.uniform(10, 30), rnd.uniform(1, 5)
-            traced = f + b + o + rnd.uniform(0, 10)
-            dl = rnd.uniform(1, 50)
-            summ[r] = {"steps_analyzed": 100, "avg_dataloader_ms": dl, "avg_forward_ms": f,
-                       "avg_backward_ms": b, "avg_optimizer_ms": o, "avg_step_cpu_ms": traced,
-                       "avg_traced_step_ms": traced, "avg_gpu_compute_ms": (f + b) + o,
-                       "avg_total_step_ms": dl + traced}
-        assert sections.step_time_global(summ) == step_time_oracle.global_points(summ)
-        assert sections.step_time_overview(summ) == step_time_oracle.overview(summ)
-    assert sections.step_time_overview({})["rank_comparison"] == "no_data"
+            f, b, o = rnd.uniform(5, 15) * n, rnd.uniform(10, 30) * n, rnd.uniform(1, 5) * n
+            traced = f + b + o + rnd.uniform(0, 10) * n
+            dl = rnd.uniform(1, 50) * n
+            sums[r] = [dl, f, b, o, traced, traced, dl + traced]
+        got = _step_time_of_sums(sums, n)
+        summ = {r: step_time_oracle._summary(n, *s) for r, s in sums.items()}
+        assert got["global"] == step_time_oracle.global_points(summ)
+        assert got["overview"] == step_time_oracle.overview(summ)
+    none = _step_time_of_sums({}, 0)["overview"]
+    assert none["rank_comparison"] == "no_data" and none == step_time_oracle.overview({})
 
 
 def test_b_reduce_formula():

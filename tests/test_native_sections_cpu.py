@@ -1,61 +1,27 @@
-"""tml_sections_json (csrc/tml_sections.cpp, host C++: no GPU needed) against
-traceml_b200/sections.py on every golden case: the native section objects must equal the
-Python-assembled ones exactly, and both equal the reference's golden outputs."""
+"""tml_sections_json (csrc/tml_sections.cpp, host C++: no GPU needed) on every golden case, with
+the Python reduce driver over engine doubles feeding it (``WindowReducer.run_out``): the section
+objects must equal the reference's golden outputs, the oracle's rollups and, for the Process
+section, the rule engine run directly on the same aggregates."""
 import json
 import os
 
 import pytest
 import torch
 
-from helpers import assert_struct, golden_cases, plain, proc_replay_for, step_replay_for
+from helpers import (assert_struct, golden_cases, oracle_mem_rows, plain, proc_replay_for, step_replay_for,
+                     strip_device)
+from traceml_b200.sections import build_process
 
 STEP = golden_cases("step")
 PROC = golden_cases("process")
 
 
-def fill_run_out(red, window, proc_rows):
-    """ReduceOutput (Python driver) -> the struct tml_reduce_run would have produced."""
-    from traceml_b200 import _abi
-
-    o = _abi.ReduceRunOut()
-    R = len(red.ranks)
-    o.n_ranks = R
-    for r in red.ranks:
-        d, i = red.infos[r], o.infos[r]
-        i.n_retained, i.latest_step, i.monotone, i.dup_rows = d["n_retained"], d["latest_step"], d["monotone"], d["dup_rows"]
-        for q in range(2):
-            i.n_rows[q], i.n_cand[q], i.lo[q], i.hi[q] = d["n_rows"][q], d["n_cand"][q], d["lo"][q], d["hi"][q]
-            i.dense[q] = d["dense"][q]
-        for q in range(7):
-            i.t_sums[q] = d["t_sums"][q]
-        i.t_count, i.n_both = d["t_count"], d["n_both"]
-        if proc_rows and r in red.proc_aggs:
-            for f, _ in _abi.ProcAgg._fields_:
-                setattr(o.procs[r], f, red.proc_aggs[r][f])
-    for k, res in ((o.time, red.time), (o.mem, red.mem)):
-        k.observed, k.n_common = res.observed, res.n_common
-        k.n_used = len(res.used)
-        k.start_step, k.end_step = res.start_step or 0, res.end_step or 0
-        for idx, r in enumerate(res.used):
-            w = res.windows[r]
-            k.used[idx], k.n_rows[idx] = r, w.n_rows
-            for q in range(7):
-                k.t_sums[idx][q] = w.t_sums[q]
-            for q in range(4):
-                k.m_sums[idx][q] = w.m_sums[q]
-        if res.band_sum is not None:
-            k.has_bands = 1
-            for s in range(16):
-                for b in range(3):
-                    k.band_sum[s][b], k.band_cnt[s][b] = res.band_sum[s][b], res.band_cnt[s][b]
-                k.tail_first[s], k.tail_last[s] = res.tail_first[s], res.tail_last[s]
-    return o
-
-
-def both(records, procs, window):
+def build_sections(records, procs, window):
+    """The sections of one build over engine doubles, and the per-rank process aggregates
+    (with the host constants) they were built from."""
     from fake_engine import FakeEngine
     import replay
-    from traceml_b200 import _abi, sections
+    from traceml_b200 import sections
 
     R = len(records) if records is not None else len(procs)
     empty = replay.make_step_replay("balanced", 1, 0, 0)[0]
@@ -63,31 +29,60 @@ def both(records, procs, window):
                           procs[r] if procs is not None else None) for r in range(R)]
     se = sections.SummaryEngine(engines, ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=R)
     se.reducer.device = torch.device("cpu")
-    py = se.build(window, window)
-    red = py.pop("reduce")
-    nat = _abi.sections_json(fill_run_out(red, window, window), replay.PROC_RAM_TOTAL_BYTES, R, window, window)
-    return py, nat
+    res = se.build(window, window)
+    red = res.pop("reduce")
+    aggs = {r: dict(a, ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=R) for r, a in red.proc_aggs.items()}
+    return res, aggs
+
+
+def _assert_step_memory_golden(got, ref):
+    """The step-memory object against the reference's (as test_gpu_parity checks it on the GPU)."""
+    assert got["training_steps"] == ref["training_steps"]
+    assert got["latest_step_observed"] == ref["latest_step_observed"]
+    assert_struct(plain(got["window"]), ref["window"], "golden.mem.window")
+    assert_struct(plain(got["metrics"]), ref["metrics"], "golden.mem.metrics")
+    assert_struct(plain(got["per_global_rank"]), ref["per_global_rank"], "golden.mem.rows")
+    gd, rd = strip_device(plain(got["diagnosis"])), strip_device(ref["diagnosis"])
+    assert_struct(gd["primary"], rd["primary"], "golden.mem.primary")
+    assert_struct(gd["issues"], rd["issues"], "golden.mem.issues")
+    for k, sig in rd["metric_attribution"].items():
+        assert_struct({x: gd["metric_attribution"][k][x] for x in sig}, sig, f"golden.mem.attr.{k}")
+    if ref["payload"].get("global") and ref["window"]["n_steps"]:
+        for k in ("average", "median", "worst"):
+            assert_struct(plain(got["global"][k]), ref["payload"]["global"][k], f"golden.mem.global.{k}")
 
 
 @pytest.mark.parametrize("g", STEP, ids=[g["case"] for g in STEP])
 def test_native_sections_equal_python_sections(g):
+    """The Python driver's reduce through the native emitter against the reference's own step-time
+    and step-memory objects (data / diagnosis / rollups), with and without a GPU total."""
+    import replay
+
     recs = step_replay_for(g)
-    py, nat = both(recs, None, g["window"])
-    for sec in ("step_time", "step_memory"):
-        assert_struct(plain(nat[sec]), plain(py[sec]), sec, rel=0.0)
-    # and the golden: the reference's own data / diagnosis
+    nat, _ = build_sections(recs, None, g["window"])
     assert_struct(plain(nat["step_time"]["data"]), g["step_time"]["data"], "golden.data")
     assert_struct(plain(nat["step_time"]["diagnosis"]), g["step_time"]["diagnosis"], "golden.diagnosis")
     for k in ("average", "median", "worst"):
         assert_struct(plain(nat["step_time"]["global"][k]), g["step_time"]["payload"]["global"][k], f"golden.global.{k}")
     assert isinstance(next(iter(nat["step_time"]["data"]["aligned_summary"]), 0), int)
+    _assert_step_memory_golden(nat["step_memory"], g["step_memory"])
+    if "step_memory_with_total" in g:  # process samples give the GPU total: the pressure rules
+        procs = replay.make_proc_replay("normal", g["ranks"], 50, g["seed"])
+        got = build_sections(recs, procs, g["window"])[0]["step_memory"]
+        t = g["step_memory_with_total"]
+        assert got["gpu_total_bytes"] == t["gpu_total_bytes"]
+        gd, rd = strip_device(plain(got["diagnosis"])), strip_device(t["diagnosis"])
+        assert_struct(gd["primary"], rd["primary"], "golden.pressure.primary")
+        assert_struct(gd["issues"], rd["issues"], "golden.pressure.issues")
 
 
 @pytest.mark.parametrize("g", PROC, ids=[g["case"] for g in PROC])
 def test_native_process_section_equals_python(g):
+    """The Process section: the rule engine run directly on the reduce's aggregates, and the
+    reference's own diagnosis."""
     procs = proc_replay_for(g)
-    py, nat = both(None, procs, g["max_rows"])
-    assert_struct(plain(nat["process"]), plain(py["process"]), "process", rel=0.0)
+    nat, aggs = build_sections(None, procs, g["max_rows"])
+    assert_struct(plain(nat["process"]), plain(build_process(aggs)), "process", rel=0.0)
     assert_struct(plain(nat["process"]["primary"]), g["process"]["diagnosis"]["primary"], "golden.primary")
     assert_struct(plain(nat["process"]["issues"]), g["process"]["diagnosis"]["issues"], "golden.issues")
 
@@ -96,24 +91,29 @@ def test_native_process_section_equals_python(g):
 def test_tie_breaks_with_identical_ranks(pattern):
     """Ranks holding identical records: every per-rank value ties, so median / worst ranks are
     decided purely by the tie-break rules (|delta|, value, rank / lowest rank wins) -- the
-    native rollups must make the same choices as sections.py."""
+    native rollups must make the oracle's (the reference's) choices."""
     import replay
+    from helpers import oracle_time_rows
+    from oracle import step_memory_oracle, step_time_oracle
 
     base = replay.make_step_replay("input_straggler", 3, 260, seed=5)
     recs = {r: base[p].copy() for r, p in enumerate(pattern)}
     pbase = replay.make_proc_replay("imbalance", 3, 120, seed=5)
     procs = {r: pbase[p].copy() for r, p in enumerate(pattern)}
-    py, nat = both(recs, procs, 10_000)
-    for sec in ("step_time", "step_memory", "process"):
-        assert_struct(plain(nat[sec]), plain(py[sec]), sec, rel=0.0)
-    # and against the oracle (the reference's arithmetic) for the public rollup
-    from helpers import oracle_time_rows
-    from oracle import step_time_oracle
-
+    nat, aggs = build_sections(recs, procs, 10_000)
     o = step_time_oracle.step_time_section(oracle_time_rows(recs, 10_000), max_rows=10_000)
+    st = nat["step_time"]
+    assert_struct(plain(st["data"]), plain({k: o["data"][k] for k in st["data"]}), "oracle.data")
     for k in ("average", "median", "worst"):
-        assert_struct(plain(nat["step_time"]["global"][k]), plain(o["global"][k]), f"oracle.global.{k}", rel=0.0)
-    assert_struct(plain(nat["step_time"]["diagnosis"]), plain(o["diagnosis"]), "oracle.diagnosis", rel=0.0)
+        assert_struct(plain(st["global"][k]), plain(o["global"][k]), f"oracle.global.{k}", rel=0.0)
+    assert_struct(plain(st["overview"]), plain(o["overview"]), "oracle.overview", rel=0.0)
+    assert_struct(plain(st["diagnosis"]), plain(o["diagnosis"]), "oracle.diagnosis", rel=0.0)
+    mo = step_memory_oracle.step_memory_section(oracle_mem_rows(recs), window_size=10_000)
+    sm = nat["step_memory"]
+    assert_struct(plain(sm["per_global_rank"]), plain(mo["per_global_rank"]), "oracle.mem.rows", rel=0.0)
+    assert_struct(plain(sm["global"]), plain(step_memory_oracle.rollup_points(mo["per_global_rank"])),
+                  "oracle.mem.global", rel=0.0)
+    assert_struct(plain(nat["process"]), plain(build_process(aggs)), "process", rel=0.0)
 
 
 def test_sections_json_from_several_threads():
@@ -126,6 +126,7 @@ def test_sections_json_from_several_threads():
     from fake_engine import FakeEngine
     import replay
     from traceml_b200 import _abi, sections
+    from traceml_b200.reduce import WindowReducer
 
     outs = {}
     for R in (1, 3, 8):
@@ -136,7 +137,7 @@ def test_sections_json_from_several_threads():
                                     ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=R)
         se.reducer.device = torch.device("cpu")
         red = se.build(W, W).pop("reduce")
-        outs[R] = (fill_run_out(red, W, W), R, W)
+        outs[R] = (WindowReducer.run_out(red), R, W)
     lib = _abi.lib()
     want = {}
     for R, (o, _, W) in outs.items():
@@ -161,3 +162,23 @@ def test_sections_json_from_several_threads():
     for t in threads:
         t.join()
     assert not bad, bad
+
+
+def test_sections_pickle_as_their_text():
+    """A build's sections pickle (to hand them to another process) as their text and what the
+    caller attached, unparsed or parsed and changed; the emitter's input does not travel."""
+    import pickle
+
+    import replay
+
+    recs = replay.make_step_replay("input_straggler", 3, 120, seed=2)
+    procs = replay.make_proc_replay("normal", 3, 60, seed=2)
+    for parse_first in (False, True):
+        res, _ = build_sections(recs, procs, 100)
+        res["system"] = {"nodes": {}}
+        if parse_first:
+            res.pop("process")
+        back = pickle.loads(pickle.dumps(res))
+        assert back.raw == res.raw and back["system"] == {"nodes": {}}
+        assert plain(back) == plain(res)
+        assert ("process" in back) is not parse_first

@@ -258,10 +258,9 @@ def test_single_rank_fixture_median_total_11():
     mem = {0: [(s, 100.0 + s, 200.0 + s) for s in range(1, 5)]}
     m = step_memory_oracle.step_memory_section(mem, window_size=4)
     assert len(m["window"]["steps"]) == 4 and m["window"]["global_ranks_used"] == 1
-    res = _sections_from_records({0: _records(range(1, 5), 1.0, 2.0, 3.0, 1.0, 10.0, 101.0, 201.0)}, 4)
-    for sec in res:   # python driver + native section emitter, host code only
-        assert sec["step_time"]["global"]["median"]["total_step_ms"]["value"] == 11.0
-        assert sec["step_memory"]["window"]["n_steps"] == 4
+    sec = _sections_from_records({0: _records(range(1, 5), 1.0, 2.0, 3.0, 1.0, 10.0, 101.0, 201.0)}, 4)
+    assert sec["step_time"]["global"]["median"]["total_step_ms"]["value"] == 11.0
+    assert sec["step_memory"]["window"]["n_steps"] == 4
 
 
 def _records(steps, dl, fwd, bwd, opt, wall, alloc0, resv0):
@@ -286,19 +285,16 @@ def _records(steps, dl, fwd, bwd, opt, wall, alloc0, resv0):
 
 def _sections_from_records(recs_by_rank, window):
     """The product's host code on CPU: the Python reduce driver over fake engines (numpy stand-ins
-    for the kernels), then the same reduce output through the native section emitter."""
+    for the kernels), then its output through the native section emitter."""
     import torch
     from fake_engine import FakeEngine
-    from test_native_sections_cpu import fill_run_out
     from traceml_b200 import sections
 
     engines = [FakeEngine(recs_by_rank[r], None) for r in sorted(recs_by_rank)]
     se = sections.SummaryEngine(engines, ram_total=1.0e9, gpu_count=len(engines))
     se.reducer.device = torch.device("cpu")
-    py = se.build(window, window)
-    red = py.pop("reduce")
-    nat = _abi.sections_json(fill_run_out(red, window, 0), 1.0e9, len(engines), window, 0)
-    return plain(py), plain({k: nat[k] for k in ("step_time", "step_memory")})
+    res = se.build(window, window)
+    return plain({k: res[k] for k in ("step_time", "step_memory")})
 
 
 def test_two_rank_fixture_aligned_window_5():
@@ -316,14 +312,13 @@ def test_two_rank_fixture_aligned_window_5():
     assert set(m["per_global_rank"]) == {"0", "1"}
     assert m["global"]["median"]["peak_allocated_bytes"]["idx"] in {"0", "1"}
     assert m["global"]["median"]["peak_reserved_bytes"]["idx"] in {"0", "1"}
-    res = _sections_from_records({r: _records(range(1, 6), 1.0, 2.0 + r, 3.0 + r, 1.0, 10.0 + r,
+    sec = _sections_from_records({r: _records(range(1, 6), 1.0, 2.0 + r, 3.0 + r, 1.0, 10.0 + r,
                                               101.0 + r * 20.0, 201.0 + r * 30.0) for r in (0, 1)}, 5)
-    for sec in res:
-        w = sec["step_time"]["data"]["aligned_window"]
-        assert (w["steps_analyzed"], w["window_size"], w["global_ranks_used"]) == (5, 5, 2)
-        assert sec["step_memory"]["window"]["n_steps"] == 5
-        assert sec["step_memory"]["window"]["global_ranks_used"] == 2
-        assert sec["step_memory"]["global"]["median"]["peak_allocated_bytes"]["idx"] in {"0", "1"}
+    w = sec["step_time"]["data"]["aligned_window"]
+    assert (w["steps_analyzed"], w["window_size"], w["global_ranks_used"]) == (5, 5, 2)
+    assert sec["step_memory"]["window"]["n_steps"] == 5
+    assert sec["step_memory"]["window"]["global_ranks_used"] == 2
+    assert sec["step_memory"]["global"]["median"]["peak_allocated_bytes"]["idx"] in {"0", "1"}
 
 
 # ------------------------------------------------------------------------------ step memory

@@ -26,8 +26,7 @@ def test_sections_vs_oracle_random(scenario, pscenario, R, S, seed, W):
     from fake_engine import FakeEngine
     from oracle import process_oracle, step_memory_oracle, step_time_oracle
     import replay
-    from traceml_b200 import _abi, sections
-    from test_native_sections_cpu import fill_run_out
+    from traceml_b200 import sections
 
     recs = replay.make_step_replay(scenario, R, S, seed)
     cut = random.Random(seed)
@@ -40,21 +39,23 @@ def test_sections_vs_oracle_random(scenario, pscenario, R, S, seed, W):
     se.reducer.device = torch.device("cpu")
     got = se.build(W, W)
     red = got.pop("reduce")
-    nat = _abi.sections_json(fill_run_out(red, W, W), replay.PROC_RAM_TOTAL_BYTES, R, W, W)
-    for sec in ("step_time", "step_memory", "process"):
-        assert_struct(plain(nat[sec]), plain(got[sec]), f"native.{sec}", rel=0.0)
     o = step_time_oracle.step_time_section(oracle_time_rows(recs, W), max_rows=W)
     g = got["step_time"]
     assert_struct(plain(g["data"]), plain({k: o["data"][k] for k in g["data"]}), "time.data")
     assert_struct(plain(g["diagnosis"]), plain(o["diagnosis"]), "time.diagnosis")
     for k in ("average", "median", "worst"):
         assert_struct(plain(g["global"][k]), plain(o["global"][k]), f"time.global.{k}")
+    assert_struct(plain(g["overview"]), plain(o["overview"]), "time.overview")
     mo = step_memory_oracle.step_memory_section(oracle_mem_rows(recs), window_size=W,
                                                 gpu_total_bytes=got["step_memory"]["gpu_total_bytes"])
     gd, od = strip_device(plain(got["step_memory"]["diagnosis"])), strip_device(plain(mo["diagnosis"]))
     assert_struct(gd["primary"], od["primary"], "mem.primary")
     assert_struct(gd["issues"], od["issues"], "mem.issues")
     assert_struct(plain(got["step_memory"]["per_global_rank"]), plain(mo["per_global_rank"]), "mem.rows")
+    assert_struct(plain(got["step_memory"]["global"]), plain(mo["global"]), "mem.global")
+    # the whole Process section: the rule engine on the same aggregates, one host's constants
+    aggs = {r: dict(a, ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=R) for r, a in red.proc_aggs.items()}
+    assert_struct(plain(got["process"]), plain(sections.build_process(aggs)), "process", rel=0.0)
     po = process_oracle.process_section(oracle_proc_rows(procs, R), max_rows=W)
     assert_struct(plain(got["process"]["primary"]), plain(po["diagnosis"]["primary"]), "proc.primary")
     assert_struct(plain(got["process"]["issues"]), plain(po["diagnosis"]["issues"]), "proc.issues")

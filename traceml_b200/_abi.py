@@ -494,3 +494,15 @@ class Sections:
 
     def to_dict(self):
         return dict(self.items())
+
+    def __reduce__(self):
+        """Pickles as the text, the parsed sections if there are any (the caller may have changed
+        them) and what the caller attached.  The emitter's input stays behind: it has a pointer
+        field, which ctypes cannot pickle, and is not needed once the text exists."""
+        return (_sections_restore, (self.raw, self._parsed, self._extra))
+
+
+def _sections_restore(raw, parsed, extra) -> Sections:
+    s = Sections(raw)
+    s._parsed, s._extra = parsed, extra
+    return s

@@ -1,9 +1,9 @@
 // tml_sections_json: Step-Time / Step-Memory / Process sections of one reduce, as JSON.
 //
-// The native counterpart of traceml_b200/sections.py (build_step_time / build_step_memory /
-// build_process + the O(R) public rollups): it consumes tml_reduce_run's output, runs the
-// three rule engines (tml_diag_*) and emits exactly the objects sections.py builds, so the
-// host does one JSON parse per final_summary() instead of interpreter work per section.
+// The one builder of these three sections, for both reduce drivers: it consumes tml_reduce_run's
+// output (the Python staging converts its result to the same struct, reduce.py run_out), fills
+// the three rule engines' inputs (tml_diag_*), computes the O(R) public rollups and emits the
+// section objects, so the host does one JSON parse per final_summary().
 // Reference arithmetic followed (file:line under src/traceml/):
 //   RankStepSummary from sums        reporting/sections/step_time/model.py:108-120,270-281
 //   closest_rank_to_median           reporting/sections/step_time/model.py:77-105
@@ -11,7 +11,8 @@
 //   global average / median / worst  reporting/sections/step_time/model.py:310-403
 //   overview                         reporting/sections/step_time/model.py:445-498
 //   step-memory rows / rollup        reporting/sections/step_memory/model.py:224-246,322-412
-// sections.py stays as the specification; tests hold the two identical.
+// Its parity evidence is the reference's own outputs (tests/golden) and the oracle (oracle/), which
+// is pinned bit-exactly to the reference.
 
 #include <algorithm>
 #include <charconv>

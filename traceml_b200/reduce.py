@@ -18,7 +18,8 @@ Two drivers sequence the same C-ABI stages:
     the native driver; the two are held bit-identical by the tests.
 
 All per-step arithmetic is in ``csrc/tml_engine.cu``, all rank-level rules in
-``csrc/tml_diag.cpp``.
+``csrc/tml_diag.cpp``; the results of both drivers become sections in
+``csrc/tml_sections.cpp`` (``WindowReducer.run_out`` hands it this module's).
 """
 
 from __future__ import annotations
@@ -333,10 +334,8 @@ class WindowReducer:
                 "lo": [i(v[8]), i(v[9])], "hi": [i(v[10]), i(v[11])],
                 "t_sums": [float(x) for x in v[12:19]], "t_count": i(v[19]), "n_both": i(v[20]), "dense": [i(v[21]), i(v[22])]}
 
-    def reduce(self, window: int, *, proc_rows: Optional[int] = None, overlap=None, stage_timings: bool = False) -> ReduceOutput:
-        """``overlap(proc_aggs)``: host work that needs only the process aggregates; it
-        runs after K4 has been launched and before the first wait on it.
-        ``stage_timings``: per-stage CUDA-event / host-clock breakdown (a diagnostic: a dozen torch
+    def reduce(self, window: int, *, proc_rows: Optional[int] = None, stage_timings: bool = False) -> ReduceOutput:
+        """``stage_timings``: per-stage CUDA-event / host-clock breakdown (a diagnostic: a dozen torch
         events per call).  Without it ``timings_ms`` still carries ``k3a`` / ``k4``, the
         two kernels' device times from the library's own events."""
         window = max(1, int(window))
@@ -442,8 +441,6 @@ class WindowReducer:
                                   self._exchange_mode(m_res.n_common))
         if mode == "p2p":
             self._p2p_warm = True
-        if overlap is not None:  # the GPU is busy with K4: free host time
-            overlap(proc_aggs)
         hw.append(_time.perf_counter())
         if ev:
             ev[3].record()
@@ -554,8 +551,6 @@ class WindowReducer:
                 res.band_sum = [k.band_sum[s][:] for s in range(16)]
                 res.band_cnt = [k.band_cnt[s][:] for s in range(16)]
                 res.tail_first, res.tail_last = k.tail_first[:], k.tail_last[:]
-                res._lay = (trend_layout(n, min_points=200, warmup_frac=0.10),
-                            trend_layout(n, min_points=50, warmup_frac=0.0))
             if k.series and n:
                 from .engine import _DevView
                 ld = int(k.series_ld)
@@ -569,6 +564,40 @@ class WindowReducer:
         return ReduceOutput(window=window, ranks=list(range(R)), infos=infos, time=kind(o.time), mem=kind(o.mem),
                             exchange=_abi.XCHG_NAME[int(o.exchange_used)], fused_pass=bool(o.fused_pass),
                             timings_ms=timings, proc_aggs=proc_aggs)
+
+    @staticmethod
+    def run_out(out: ReduceOutput) -> _abi.ReduceRunOut:
+        """The inverse of ``convert_native``: the result ``tml_reduce_run`` would have produced for
+        ``out``, in every field the section emitter (``tml_sections_json``) reads -- so the Python
+        staging and the native driver share one emitter."""
+        o = _abi.ReduceRunOut()
+        o.n_ranks = len(out.ranks)
+        for r in out.ranks:
+            d, i = out.infos[r], o.infos[r]
+            i.n_retained, i.latest_step, i.monotone, i.dup_rows = d["n_retained"], d["latest_step"], d["monotone"], d["dup_rows"]
+            for q in range(2):
+                i.n_rows[q], i.n_cand[q], i.lo[q], i.hi[q] = d["n_rows"][q], d["n_cand"][q], d["lo"][q], d["hi"][q]
+                i.dense[q] = d["dense"][q]
+            i.t_sums[:] = d["t_sums"]
+            i.t_count, i.n_both = d["t_count"], d["n_both"]
+            if r in out.proc_aggs:
+                for f in _PROC_FIELDS:
+                    setattr(o.procs[r], f, out.proc_aggs[r][f])
+        for k, res in ((o.time, out.time), (o.mem, out.mem)):
+            k.observed, k.n_common = res.observed, res.n_common
+            k.n_used = len(res.used)
+            k.start_step, k.end_step = res.start_step or 0, res.end_step or 0
+            for idx, r in enumerate(res.used):
+                w = res.windows[r]
+                k.used[idx], k.n_rows[idx] = r, w.n_rows
+                k.t_sums[idx][:] = w.t_sums
+                k.m_sums[idx][:] = w.m_sums
+            if res.band_sum is not None:
+                k.has_bands = 1
+                for s in range(16):
+                    k.band_sum[s][:], k.band_cnt[s][:] = res.band_sum[s], res.band_cnt[s]
+                k.tail_first[:], k.tail_last[:] = res.tail_first, res.tail_last
+        return o
 
     # ------------------------------------------------------------------ alignment
     def _spec_len(self) -> int:
@@ -803,13 +832,11 @@ class WindowReducer:
 
             res.tail_first = [pick("tf", s) for s in range(16)]
             res.tail_last = [pick("tl", s) for s in range(16)]
-            res._lay = (lay_t, lay_m)
 
         run(t_res, (0,))
         if same:
             m_res.band_sum, m_res.band_cnt = t_res.band_sum, t_res.band_cnt
             m_res.tail_first, m_res.tail_last = t_res.tail_first, t_res.tail_last
-            m_res._lay = getattr(t_res, "_lay", (None, None))
         else:
             run(m_res, (1,))
 

@@ -183,6 +183,31 @@ def test_large_window_properties(cuda):
 
 
 # ---------------------------------------------------------------------------- native sequencing
+def _run_out_fields(o):
+    """What both reduce drivers must fill alike in a ReduceRunOut, as plain values: ``n_ranks``,
+    ``fused_pass``, ``infos`` (but the kernel time each rank reports), ``procs``, and all of
+    ``time`` / ``mem`` but where the series live.  A separate pass per section writes only that
+    section's series rows, so the band sums and tails of the other rows are undefined and left
+    out.  NaNs compare equal."""
+    import ctypes as C
+
+    def val(x, skip=()):
+        if isinstance(x, C.Structure):
+            return {f: val(getattr(x, f)) for f, _ in x._fields_ if f not in skip}
+        if isinstance(x, C.Array):
+            return [val(v) for v in x]
+        return "nan" if isinstance(x, float) and x != x else x
+
+    got = {"n_ranks": o.n_ranks, "fused_pass": o.fused_pass, "infos": [val(i, ("kernel_ms",)) for i in o.infos],
+           "procs": val(o.procs)}
+    for name, rows in (("time", slice(0, 12)), ("mem", slice(12, 16))):
+        k = val(getattr(o, name), ("series",))
+        for f in ("band_sum", "tail_first", "tail_last"):
+            k[f] = k[f][rows]
+        got[name] = k
+    return got
+
+
 @pytest.mark.parametrize("scenario,S,W,slots", [
     ("balanced", 300, 10_000, None), ("wait_heavy", 300, 128, None), ("duplicates", 240, 10_000, None),
     ("trend_worsening", 600, 10_000, None), ("mem_creep_confirmed", 300, 100, None),
@@ -192,14 +217,14 @@ def test_large_window_properties(cuda):
 ])
 def test_native_driver_equals_python_driver(cuda, scenario, S, W, slots):
     """tml_reduce_run (csrc/tml_summary.cpp) against the Python staging of the same C-ABI
-    stages, one rank: every section identical, bit for bit."""
+    stages, one rank: every section, and the result struct both fill, identical bit for bit."""
     import replay
     from traceml_b200 import sections
     from traceml_b200.engine import Engine
 
     recs = replay.make_step_replay(scenario, 1, S, seed=31)[0]
     procs = replay.make_proc_replay("overhang", 1, 300, seed=31)[0]
-    out, series, facts = {}, {}, {}
+    out, series, facts, fields = {}, {}, {}, {}
     for native in (True, False):
         e = Engine(device=0, rank=0, world=1, ring_slots=slots or max(64, S + 8), proc_slots=512)
         e.load_steps(recs)
@@ -217,12 +242,14 @@ def test_native_driver_equals_python_driver(cuda, scenario, S, W, slots):
             series[native] = (red.time.series.clone() if red.time.n_common else None,
                               red.mem.series.clone() if red.mem.n_common else None)
             facts[native] = (red.exchange, red.fused_pass, red.time.n_common, red.mem.n_common)
+            fields[native] = _run_out_fields(red.out)
         finally:
             e.close()
     a, b = out[True], out[False]
     a.pop("reduce"), b.pop("reduce")
     assert_struct(plain(a), plain(b), "native == python", rel=0.0)
     assert facts[True] == facts[False] and facts[True][0] == "local"
+    assert fields[True] == fields[False]
     if series[True][0] is not None:
         assert torch.equal(series[True][0][:12], series[False][0][:12])
     if series[True][1] is not None:

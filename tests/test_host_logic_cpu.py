@@ -24,13 +24,22 @@ def test_trend_layout_matches_reference_bands(min_points, warm):
             assert math.isclose(a[lo:hi].sum() / (hi - lo), ev[key], rel_tol=1e-13), (n, key)
 
 
-def test_info_pack_roundtrip():
-    d = {"n_retained": 12345, "latest_step": 2 ** 40 + 7, "monotone": 1, "dup_rows": 3,
-         "n_rows": [100, 200], "n_cand": [99, 198], "lo": [5, 6], "hi": [2 ** 40, 2 ** 40 + 7],
-         "t_sums": [1.5, 2.5, 3.5, 4.5, 5.5, 6.5, 7.5], "t_count": 99, "n_both": 98, "dense": [1, 0]}
-    v = WindowReducer._info_pack(d)
+def test_win_info_pack_roundtrip():
+    """A rank's ``WinInfo`` through the exchange layout and back into a ``WinInfo``, with the
+    memory candidate bounds it advertises."""
+    from traceml_b200 import _abi
+
+    w = _abi.WinInfo(n_retained=12345, latest_step=2 ** 40 + 7, monotone=1, dup_rows=3, n_rows=(100, 200),
+                     n_cand=(99, 198), lo=(5, 6), hi=(2 ** 40, 2 ** 40 + 7),
+                     t_sums=(1.5, 2.5, 3.5, 4.5, 5.5, 6.5, 7.5), t_count=99, n_both=98, dense=(1, 0))
+    v = WindowReducer._info_pack(w, (w.lo[1], w.n_cand[1]))
     assert len(v) == 23
-    assert WindowReducer._info_unpack([float(x) for x in v]) == d
+    got = _abi.WinInfo()
+    WindowReducer._info_unpack([float(x) for x in v], got)
+    assert bytes(got) == bytes(w)
+    WindowReducer._info_unpack([float(x) for x in WindowReducer._info_pack(w, (2 ** 40 - 3, 4))], got)
+    assert (got.lo[1], got.n_cand[1]) == (2 ** 40 - 3, 4)  # the advertised memory candidates
+    assert (got.lo[0], got.n_cand[0], got.hi[1]) == (5, 99, 2 ** 40 + 7)
 
 
 def _step_time_of_sums(sums_by_rank, n):

@@ -1,5 +1,5 @@
 """tml_sections_json (csrc/tml_sections.cpp, host C++: no GPU needed) on every golden case, with
-the Python reduce driver over engine doubles feeding it (``WindowReducer.run_out``): the section
+the Python reduce driver over engine doubles feeding it (the ``ReduceRunOut`` it fills): the section
 objects must equal the reference's golden outputs, the oracle's rollups and, for the Process
 section, the rule engine run directly on the same aggregates."""
 import json
@@ -116,17 +116,16 @@ def test_tie_breaks_with_identical_ranks(pattern):
     assert_struct(plain(nat["process"]), plain(build_process(aggs)), "process", rel=0.0)
 
 
-def test_sections_json_from_several_threads():
+def test_sections_json_of_reduce_results_from_several_threads():
     """The JSON strings of one call come from a per-thread bump arena (tml_internal.h) that is
     rewound when the outermost entry point returns: calls racing on different threads (ctypes
-    drops the GIL) must not see each other's memory."""
+    drops the GIL) over the results of several builds must not see each other's memory."""
     import ctypes as C
     import threading
 
     from fake_engine import FakeEngine
     import replay
     from traceml_b200 import _abi, sections
-    from traceml_b200.reduce import WindowReducer
 
     outs = {}
     for R in (1, 3, 8):
@@ -137,7 +136,7 @@ def test_sections_json_from_several_threads():
                                     ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=R)
         se.reducer.device = torch.device("cpu")
         red = se.build(W, W).pop("reduce")
-        outs[R] = (WindowReducer.run_out(red), R, W)
+        outs[R] = (red.out, R, W)
     lib = _abi.lib()
     want = {}
     for R, (o, _, W) in outs.items():
@@ -182,3 +181,31 @@ def test_sections_pickle_as_their_text():
         assert back.raw == res.raw and back["system"] == {"nodes": {}}
         assert plain(back) == plain(res)
         assert ("process" in back) is not parse_first
+
+
+def test_reduce_result_pickles_with_its_series():
+    """The Python driver's reduce result travels with its sections: the result struct and the
+    series it kept, so ``n_common``, ``exchange``, the series and every band field survive."""
+    import pickle
+
+    from fake_engine import FakeEngine
+    import replay
+    from traceml_b200 import sections
+
+    recs = replay.make_step_replay("input_straggler", 3, 120, seed=2)
+    procs = replay.make_proc_replay("normal", 3, 60, seed=2)
+    se = sections.SummaryEngine([FakeEngine(recs[r], procs[r]) for r in range(3)],
+                                ram_total=replay.PROC_RAM_TOTAL_BYTES, gpu_count=3)
+    se.reducer.device = torch.device("cpu")
+    res = se.build(100, 100)
+    red = res["reduce"]
+    back = pickle.loads(pickle.dumps(res))
+    assert back.raw == res.raw
+    got = back["reduce"]
+    assert got.exchange == red.exchange == "local" and got.ranks == red.ranks == [0, 1, 2]
+    assert got.proc_aggs == red.proc_aggs
+    for kind in ("time", "mem"):
+        a, b = getattr(red, kind), getattr(got, kind)
+        assert b.n_common == a.n_common == 100 and b.shard == a.shard
+        assert torch.equal(b.series, a.series)
+        assert bytes(b.band_sum) == bytes(a.band_sum) and bytes(b.tail_last) == bytes(a.tail_last)

@@ -1,7 +1,7 @@
 // tml_sections_json: Step-Time / Step-Memory / Process sections of one reduce, as JSON.
 //
 // The one builder of these three sections, for both reduce drivers: it consumes tml_reduce_run's
-// output (the Python staging converts its result to the same struct, reduce.py run_out), fills
+// output (the Python staging in reduce.py fills the same struct), fills
 // the three rule engines' inputs (tml_diag_*), computes the O(R) public rollups and emits the
 // section objects, so the host does one JSON parse per final_summary().
 // Reference arithmetic followed (file:line under src/traceml/):

@@ -18,15 +18,15 @@ Two drivers sequence the same C-ABI stages:
     the native driver; the two are held bit-identical by the tests.
 
 All per-step arithmetic is in ``csrc/tml_engine.cu``, all rank-level rules in
-``csrc/tml_diag.cpp``; the results of both drivers become sections in
-``csrc/tml_sections.cpp`` (``WindowReducer.run_out`` hands it this module's).
+``csrc/tml_diag.cpp``.  Both drivers fill the same ``_abi.ReduceRunOut`` as they go, which
+``csrc/tml_sections.cpp`` turns into sections, and both return it in one view, ``ReduceResult``.
 """
 
 from __future__ import annotations
 
+import functools
 import math
-from dataclasses import dataclass, field
-from typing import Any, Dict, List, Optional, Sequence
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -55,17 +55,16 @@ def _proc_pack(a) -> List[float]:
     return v
 
 
-def _proc_unpack(v) -> Dict[str, Any]:
-    pa: Dict[str, Any] = {}
+def _proc_unpack(v, a) -> None:
+    """The inverse of ``_proc_pack``, into the ``ProcAgg`` ``a``."""
     k = 0
     for f in _PROC_FIELDS:
         if f in _PROC_U64_FIELDS:
-            pa[f] = int(v[k]) | (int(v[k + 1]) << 32)
+            setattr(a, f, int(v[k]) | (int(v[k + 1]) << 32))
             k += 2
         else:
-            pa[f] = int(round(v[k])) if f in _PROC_INT_FIELDS else v[k]
+            setattr(a, f, int(round(v[k])) if f in _PROC_INT_FIELDS else v[k])
             k += 1
-    return pa
 
 # analytics/trends/schema.py:27-62
 _BANDS = ((0.15, 0.25), (0.45, 0.55), (0.90, 1.00))
@@ -208,78 +207,90 @@ def _stream_of(device: torch.device) -> int:
     return int(torch.cuda.current_stream(device).cuda_stream) if device.type == "cuda" else 0
 
 
-@dataclass
-class RankWindow:
-    """What one global rank contributed to one aligned window."""
+class ReduceKind:
+    """One section of a ``ReduceResult``: ``series`` is this process's [16, n_common] (its
+    ``shard`` of the columns valid), None without a reduce pass.  Every other field (alignment,
+    bands) is read from the section's ``KindResultC`` in ``ReduceResult.out``."""
 
-    rank: int
-    n_rows: int = 0
-    t_sums: Sequence[float] = ()
-    m_sums: Sequence[float] = ()
-    info: Dict[str, Any] = field(default_factory=dict)
+    def __init__(self, k, series: Optional[torch.Tensor]):
+        self._k = k
+        self.n_common = int(k.n_common)
+        self.shard = (int(k.shard_lo), int(k.shard_hi))
+        self.series = series
 
-
-@dataclass
-class KindResult:
-    observed: int = 0            # ranks that had candidates
-    used: List[int] = field(default_factory=list)
-    n_common: int = 0
-    start_step: Optional[int] = None
-    end_step: Optional[int] = None
-    windows: Dict[int, RankWindow] = field(default_factory=dict)
-    band_sum: Optional[List[List[float]]] = None   # [16][3]
-    band_cnt: Optional[List[List[int]]] = None
-    tail_first: Optional[List[float]] = None
-    tail_last: Optional[List[float]] = None
-    series: Optional[torch.Tensor] = None          # this process's [16, n_common] (own shard valid)
-    shard: tuple = (0, 0)
+    def __getattr__(self, name: str):
+        return getattr(self.__dict__["_k"], name)
 
 
-@dataclass
-class ReduceOutput:
-    window: int
-    ranks: List[int]
-    infos: Dict[int, Dict[str, Any]]
-    time: KindResult
-    mem: KindResult
-    exchange: str
-    fused_pass: bool
-    timings_ms: Dict[str, float] = field(default_factory=dict)
-    proc_aggs: Dict[int, Dict[str, Any]] = field(default_factory=dict)
+class ReduceResult:
+    """One reduce's result, whichever driver sequenced it: ``out``, the ``_abi.ReduceRunOut`` the
+    section emitter reads (per-rank infos and process aggregates, the alignment and bands of
+    ``out.time`` / ``out.mem``), and the facts callers read from it.
 
+    ``exchange`` names the row exchange used; ``timings_ms`` holds the driver's stage times.
+    ``series``: the series tensors the Python driver wrote, by kind; without them (native
+    driver) ``time.series`` / ``mem.series`` are zero-copy, read-only views of the engine's own
+    workspace: valid until the engine's next reduce or its ``close()``; ``clone()`` them to keep
+    them.  Their row stride may exceed ``n_common``, and when ``series_paired`` is set (the
+    single-rank bulk path) rows 2m and 2m+1 are the same memory mapped twice, so a write into one
+    row would change its partner."""
 
-class NativeReduceOutput:
-    """What ``SummaryEngine.build`` returns as ``"reduce"`` on the native path: the cheap
-    facts eagerly, the full ``ReduceOutput`` (per-rank windows, band sums, series view) only
-    if somebody asks -- the sections no longer need it.  ``time.series`` / ``mem.series`` are
-    zero-copy, read-only views of the engine's own workspace: valid until the engine's next reduce
-    or its ``close()``; ``clone()`` them to keep them.  Their row stride may exceed ``n_common``,
-    and when ``series_paired`` is set (the single-rank bulk path) rows 2m and 2m+1 are the same
-    memory mapped twice, so a write into one row would change its partner."""
-
-    def __init__(self, reducer: "WindowReducer", o, window: int, proc_rows: Optional[int]):
+    def __init__(self, out: _abi.ReduceRunOut, window: int, exchange: str, timings_ms: Dict[str, float],
+                 series: Optional[Dict[str, Optional[torch.Tensor]]] = None,
+                 device: Optional[torch.device] = None):
+        self.out = out
         self.window = window
-        self.exchange = _abi.XCHG_NAME[int(o.exchange_used)]
-        self.fused_pass = bool(o.fused_pass)
-        self.fused_rows = int(o.fused_pass) == 2  # single-rank bulk path: ring -> series in one kernel
-        self.series_paired = bool(o.time.series_paired)
-        self.timings_ms = reducer.native_timings(o)
-        self.n_exchanges = int(o.n_exchanges)
-        self.ranks = list(range(int(o.n_ranks)))
-        self._snap = type(o).from_buffer_copy(o)  # the engine reuses its result struct
-        self._args = (reducer, window, proc_rows)
-        self._full: Optional[ReduceOutput] = None
+        self.exchange = exchange
+        self.timings_ms = timings_ms
+        self._series = series
+        self._device = device
 
-    def _get(self) -> ReduceOutput:
-        if self._full is None:
-            reducer, window, proc_rows = self._args
-            self._full = reducer.convert_native(self._snap, window, proc_rows)
-        return self._full
+    ranks = property(lambda self: list(range(int(self.out.n_ranks))))
+    fused_pass = property(lambda self: bool(self.out.fused_pass))
+    fused_rows = property(lambda self: int(self.out.fused_pass) == 2)  # single-rank bulk: ring -> series in one kernel
+    series_paired = property(lambda self: bool(self.out.time.series_paired))
+    n_exchanges = property(lambda self: int(self.out.n_exchanges))
 
-    time = property(lambda self: self._get().time)
-    mem = property(lambda self: self._get().mem)
-    infos = property(lambda self: self._get().infos)
-    proc_aggs = property(lambda self: self._get().proc_aggs)
+    @functools.cached_property
+    def time(self) -> ReduceKind:
+        return self._kind("time")
+
+    @functools.cached_property
+    def mem(self) -> ReduceKind:
+        return self._kind("mem")
+
+    @property
+    def proc_aggs(self) -> Dict[int, Dict[str, Any]]:
+        """Every rank's process aggregates (``out.procs``) as dicts of their fields; zeros when the
+        reduce had no process rows."""
+        return {r: {f: getattr(self.out.procs[r], f) for f in _PROC_FIELDS} for r in self.ranks}
+
+    def _kind(self, name: str) -> ReduceKind:
+        k = getattr(self.out, name)
+        n = int(k.n_common)
+        if self._series is not None:
+            series = self._series.get(name)
+        elif k.series and n:
+            from .engine import _DevView
+
+            ld = int(k.series_ld)
+            series = torch.as_tensor(_DevView(int(k.series), _abi.TML_SERIES_PER_STEP * ld),
+                                     device=self._device).view(_abi.TML_SERIES_PER_STEP, ld)[:, :n]
+        else:
+            series = None
+        return ReduceKind(k, series)
+
+    def __reduce__(self):
+        """Pickles as the bytes of ``out`` and what the Python driver kept.  ctypes cannot pickle
+        ``out`` itself (it has pointer fields), and the series pointers mean nothing in another
+        process: they travel zeroed, so the native driver's series views do not travel."""
+        o = type(self.out).from_buffer_copy(self.out)
+        o.time.series = o.mem.series = None
+        return (_result_restore, (bytes(o), self.window, self.exchange, self.timings_ms, self._series))
+
+
+def _result_restore(raw, window, exchange, timings_ms, series) -> ReduceResult:
+    return ReduceResult(_abi.ReduceRunOut.from_buffer_copy(raw), window, exchange, timings_ms, series)
 
 
 # ----------------------------------------------------------------------------- reducer
@@ -290,7 +301,6 @@ class WindowReducer:
                  exchange: str = "auto", speculate: bool = True, native: bool = True):
         self.speculate = speculate
         self.native = native        # False: sequence the stages from Python (reference driver)
-        self.last_exchanges = 0
         self.engines = list(engines)
         self.comm = comm or LocalComm()
         self.device = device or torch.device("cuda", self.engines[0].device)
@@ -308,44 +318,44 @@ class WindowReducer:
     def _grank(self, l: int) -> int:
         return self.comm.index * self.L + l
 
-    def _info_dict(self, w) -> Dict[str, Any]:
-        return {
-            "n_retained": int(w.n_retained), "latest_step": int(w.latest_step),
-            "monotone": int(w.monotone), "dup_rows": int(w.dup_rows),
-            "n_rows": [int(w.n_rows[0]), int(w.n_rows[1])],
-            "n_cand": [int(w.n_cand[0]), int(w.n_cand[1])],
-            "lo": [int(w.lo[0]), int(w.lo[1])], "hi": [int(w.hi[0]), int(w.hi[1])],
-            "t_sums": [float(x) for x in w.t_sums], "t_count": int(w.t_count),
-            "n_both": int(getattr(w, "n_both", 0)),
-            "dense": [int(x) for x in getattr(w, "dense", (0, 0))],
-            "kernel_ms": float(getattr(w, "kernel_ms", 0.0)),
-        }
+    @staticmethod
+    def _info_pack(w, mem: Tuple[int, int]) -> List[float]:
+        """A rank's ``WinInfo`` as doubles for the exchange (csrc/tml_summary.cpp pack_info: same
+        layout), advertising ``mem`` = (lo, n_cand) for its memory candidates."""
+        lo, n_cand = list(w.lo), list(w.n_cand)
+        lo[KIND_MEM], n_cand[KIND_MEM] = mem
+        return ([w.n_retained, w.latest_step, w.monotone, w.dup_rows] + list(w.n_rows) + n_cand + lo
+                + list(w.hi) + list(w.t_sums) + [w.t_count, w.n_both] + list(w.dense))
 
     @staticmethod
-    def _info_pack(d: Dict[str, Any]) -> List[float]:
-        return ([d["n_retained"], d["latest_step"], d["monotone"], d["dup_rows"]]
-                + d["n_rows"] + d["n_cand"] + d["lo"] + d["hi"] + d["t_sums"] + [d["t_count"], d["n_both"]] + d["dense"])
+    def _info_unpack(v: Sequence[float], i) -> None:
+        """The inverse of ``_info_pack``, into the ``WinInfo`` ``i``."""
+        n = lambda x: int(round(x))  # noqa: E731  (step ids < 2^53)
+        i.n_retained, i.latest_step, i.monotone, i.dup_rows = (n(x) for x in v[0:4])
+        for q in range(2):
+            i.n_rows[q], i.n_cand[q], i.lo[q], i.hi[q] = n(v[4 + q]), n(v[6 + q]), n(v[8 + q]), n(v[10 + q])
+            i.dense[q] = n(v[21 + q])
+        i.t_sums[:] = [float(x) for x in v[12:19]]
+        i.t_count, i.n_both = n(v[19]), n(v[20])
 
-    @staticmethod
-    def _info_unpack(v: Sequence[float]) -> Dict[str, Any]:
-        i = lambda x: int(round(x))  # noqa: E731  (step ids < 2^53)
-        return {"n_retained": i(v[0]), "latest_step": i(v[1]), "monotone": i(v[2]),
-                "dup_rows": i(v[3]), "n_rows": [i(v[4]), i(v[5])], "n_cand": [i(v[6]), i(v[7])],
-                "lo": [i(v[8]), i(v[9])], "hi": [i(v[10]), i(v[11])],
-                "t_sums": [float(x) for x in v[12:19]], "t_count": i(v[19]), "n_both": i(v[20]), "dense": [i(v[21]), i(v[22])]}
-
-    def reduce(self, window: int, *, proc_rows: Optional[int] = None, stage_timings: bool = False) -> ReduceOutput:
+    def reduce(self, window: int, *, proc_rows: Optional[int] = None, stage_timings: bool = False) -> ReduceResult:
         """``stage_timings``: per-stage CUDA-event / host-clock breakdown (a diagnostic: a dozen torch
         events per call).  Without it ``timings_ms`` still carries ``k3a`` / ``k4``, the
-        two kernels' device times from the library's own events."""
+        two kernels' device times from the library's own events.
+
+        The Python staging fills its ``ReduceRunOut`` the way ``reduce_run`` in
+        csrc/tml_summary.cpp fills ``out``, except for the exchange code and the native driver's
+        counters and times, which stay zero."""
         window = max(1, int(window))
         dev = self.device
         stream = _stream_of(dev)
         if self._native_ok() and not stage_timings:
-            return self._reduce_native(window, proc_rows, stream)
+            return self.native_result(self.run_native(window, proc_rows, stream), window)
         self._k4_events = []
         self._timed = bool(stage_timings)
         R = self.comm.world * self.L
+        o = _abi.ReduceRunOut()
+        o.n_ranks = R
         ev = None
         timings: Dict[str, float] = {}
         import time as _time
@@ -364,12 +374,11 @@ class WindowReducer:
         if ev:
             k3a_ev0 = torch.cuda.Event(enable_timing=True)
             k3a_ev0.record()
-        local_infos = [self._info_dict(e.win_prepare(window, stream)) for e in self.engines]
+        local = [e.win_prepare(window, stream) for e in self.engines]
         if ev:
             k3a_ev = torch.cuda.Event(enable_timing=True)
             k3a_ev.record()
-        for l, e in enumerate(self.engines):
-            self._limit_memory_candidates(e, local_infos[l], window, stream)
+        mems = [self._memory_candidates(e, w, window, stream) for e, w in zip(self.engines, local)]
         # Lock-step speculation: a rank whose own time window is dense assumes the common
         # window IS its window (true whenever the ranks run in lock step) and sends that
         # alignment -- sums and rows handle, nothing to launch -- with its bounds.  If the
@@ -378,33 +387,29 @@ class WindowReducer:
         slen = self._spec_len()
         per = _INFO_LEN + plen + slen
         flat: List[float] = []
-        for l, d in enumerate(local_infos):
-            flat.extend(self._info_pack(d))
-            eng = self.engines[l]
+        for eng, w, mem in zip(self.engines, local, mems):
+            flat.extend(self._info_pack(w, mem))
             if proc_rows:  # process aggregates (K6) ride in the same exchange
                 a = (eng.proc_reduce_collect() if hasattr(eng, "proc_reduce_collect")
                      else eng.proc_reduce(max(1, int(proc_rows)), stream))
                 flat.extend(_proc_pack(a))
             if slen:
                 sp = [0.0] * slen
-                if d["dense"][KIND_TIME] and d["n_cand"][KIND_TIME] > 0:
-                    a = eng.win_select_dense(KIND_TIME, d["lo"][KIND_TIME], d["n_cand"][KIND_TIME], stream)
+                if w.dense[KIND_TIME] and w.n_cand[KIND_TIME] > 0:
+                    a = eng.win_select_dense(KIND_TIME, w.lo[KIND_TIME], w.n_cand[KIND_TIME], stream)
                     sp = self._align_pack(eng, KIND_TIME, a, slen)
                 flat.extend(sp)
-        infos: Dict[int, Dict[str, Any]] = {}
-        proc_aggs: Dict[int, Dict[str, Any]] = {}
         spec: Optional[List[List[float]]] = [] if slen else None
         for p, row in enumerate(self.comm.all_gather_vec(flat, dev)):
             srow: List[float] = []
             for l in range(self.L):
                 v = row[l * per:(l + 1) * per]
-                infos[p * self.L + l] = self._info_unpack(v[:_INFO_LEN])
+                self._info_unpack(v[:_INFO_LEN], o.infos[p * self.L + l])
                 if proc_rows:
-                    proc_aggs[p * self.L + l] = _proc_unpack(v[_INFO_LEN:_INFO_LEN + plen])
+                    _proc_unpack(v[_INFO_LEN:_INFO_LEN + plen], o.procs[p * self.L + l])
                 srow.extend(v[_INFO_LEN + plen:])
             if spec is not None:
                 spec.append(srow)
-        ranks = sorted(infos)
         hw.append(_time.perf_counter())
         if ev:
             ev[1].record()
@@ -412,33 +417,35 @@ class WindowReducer:
         # If on every rank the time and the memory candidates are the very same rows (the
         # common case: ring not longer than the window, every step has memory), one
         # alignment serves both sections.
-        merged = all(d["n_cand"][0] == d["n_cand"][1] == d["n_both"] for d in infos.values())
-        t_res = self._align(KIND_TIME, window, infos, ranks, stream, spec=spec)
+        t, m = o.time, o.mem
+        merged = all(i.n_cand[0] == i.n_cand[1] == i.n_both for i in o.infos[:R])
+        t_handles = self._align(KIND_TIME, window, o.infos, R, t, stream, spec=spec)
         if merged:
-            m_res = KindResult(observed=t_res.observed, used=list(t_res.used), n_common=t_res.n_common,
-                               start_step=t_res.start_step, end_step=t_res.end_step,
-                               windows=dict(t_res.windows))
+            o.mem = o.time  # a copy, of the alignment: nothing else is set yet
+            m_handles = t_handles
         else:
-            m_res = self._align(KIND_MEM, window, infos, ranks, stream)
+            m_handles = self._align(KIND_MEM, window, o.infos, R, m, stream)
         hw.append(_time.perf_counter())
         if ev:
             ev[2].record()
 
         # ---- stage 4: exchange + per-step reduce
-        same = (t_res.n_common > 0 and t_res.n_common == m_res.n_common
-                and t_res.start_step == m_res.start_step and t_res.end_step == m_res.end_step
-                and t_res.used == m_res.used)
-        mode = self._exchange_mode(t_res.n_common or m_res.n_common)
+        same = (t.n_common > 0 and t.n_common == m.n_common and t.start_step == m.start_step
+                and t.end_step == m.end_step and t.used[:t.n_used] == m.used[:m.n_used])
+        mode = self._exchange_mode(t.n_common or m.n_common)
+        series: Dict[str, Optional[torch.Tensor]] = {"time": None, "mem": None}
         if same:
-            self._reduce_pass(KIND_TIME, _abi.MASK_TIME | _abi.MASK_MEM, t_res, stream, mode)
-            m_res.series, m_res.shard = t_res.series, t_res.shard
+            series["time"] = series["mem"] = self._reduce_pass(
+                KIND_TIME, _abi.MASK_TIME | _abi.MASK_MEM, t, t_handles, stream, mode)
+            m.series, m.series_ld, m.shard_lo, m.shard_hi = t.series, t.series_ld, t.shard_lo, t.shard_hi
         else:
-            if t_res.n_common:
-                self._reduce_pass(KIND_TIME, _abi.MASK_TIME, t_res, stream,
-                                  self._exchange_mode(t_res.n_common))
-            if m_res.n_common:
-                self._reduce_pass(KIND_MEM, _abi.MASK_MEM, m_res, stream,
-                                  self._exchange_mode(m_res.n_common))
+            if t.n_common:
+                series["time"] = self._reduce_pass(KIND_TIME, _abi.MASK_TIME, t, t_handles, stream,
+                                                   self._exchange_mode(t.n_common))
+            if m.n_common:
+                series["mem"] = self._reduce_pass(KIND_MEM, _abi.MASK_MEM, m, m_handles, stream,
+                                                  self._exchange_mode(m.n_common))
+        o.fused_pass = 1 if same else 0
         if mode == "p2p":
             self._p2p_warm = True
         hw.append(_time.perf_counter())
@@ -446,10 +453,16 @@ class WindowReducer:
             ev[3].record()
 
         # ---- stage 5: trend bands
-        self._bands(t_res, m_res, same, stream)
+        self._bands(t, series["time"], stream)
+        if same:  # the memory section's series is the time section's: so are its bands
+            m.has_bands, m.band_sum, m.band_cnt = t.has_bands, t.band_sum, t.band_cnt
+            m.tail_first, m.tail_last = t.tail_first, t.tail_last
+        else:
+            self._bands(m, series["mem"], stream)
         hw.append(_time.perf_counter())
         for i, nm in enumerate(("prepare", "align", "reduce", "bands")):
             timings["host_" + nm] = (hw[i + 1] - hw[i]) * 1e3
+        k3a = max((float(getattr(w, "kernel_ms", 0.0)) for w in local), default=0.0)
         if ev:
             ev[4].record()
             torch.cuda.synchronize(dev)
@@ -458,37 +471,35 @@ class WindowReducer:
                 timings[nm] = float(ev[i].elapsed_time(ev[i + 1]))
             timings["total"] = float(ev[0].elapsed_time(ev[4]))
             timings["k3a_stage"] = float(k3a_ev0.elapsed_time(k3a_ev))
-            timings["k3a"] = max((d.get("kernel_ms", 0.0) for d in local_infos), default=0.0) \
-                or timings["k3a_stage"]
+            timings["k3a"] = k3a or timings["k3a_stage"]
             timings["k4"] = float(sum(a.elapsed_time(b) for a, b in self._k4_events))
         elif dev.type == "cuda":  # the bands stage synchronised: both kernels have finished
-            timings["k3a"] = max((d.get("kernel_ms", 0.0) for d in local_infos), default=0.0)
-            if t_res.n_common or m_res.n_common:
+            timings["k3a"] = k3a
+            if t.n_common or m.n_common:
                 timings["k4"] = float(sum(max(0.0, e.kernel_ms(1)) for e in self.engines
                                           if hasattr(e, "kernel_ms")))
-        return ReduceOutput(window=window, ranks=ranks, infos=infos, time=t_res, mem=m_res,
-                            exchange=mode, fused_pass=same, timings_ms=timings, proc_aggs=proc_aggs)
+        return ReduceResult(o, window, mode, timings, series)
 
     # ------------------------------------------------------------------ memory candidate limit
-    def _limit_memory_candidates(self, engine, info: Dict[str, Any], window: int, stream) -> None:
-        """Only the newest ``max(20 W, W + 1)`` distinct step ids of a rank enter the memory
-        alignment (step_memory/loader.py:215, oracle candidate_rows).  The ring normally holds
-        1.5 W rows, so this binds only for a small window over a long ring; then the rank
-        advertises the step id of its limit-th newest candidate as its lower bound -- every
-        later stage works on [max lo, min hi] and never sees the older candidates."""
+    def _memory_candidates(self, engine, info, window: int, stream) -> Tuple[int, int]:
+        """(lo, n_cand) of the memory candidates a rank advertises.  Only the newest
+        ``max(20 W, W + 1)`` distinct step ids of a rank enter the memory alignment
+        (step_memory/loader.py:215, oracle candidate_rows).  The ring normally holds 1.5 W rows,
+        so this binds only for a small window over a long ring; then the rank advertises the step
+        id of its limit-th newest candidate as its lower bound -- every later stage works on
+        [max lo, min hi] and never sees the older candidates."""
         limit = max(20 * window, window + 1)
-        if info["n_cand"][KIND_MEM] <= limit:
-            return
-        lo, hi = info["lo"][KIND_MEM], info["hi"][KIND_MEM]
-        if info["dense"][KIND_MEM]:  # consecutive ids
-            thr = hi - limit + 1
-        else:                        # holes / re-flushed ids: select the newest `limit` of its own
-            span = hi - lo + 1
-            own = torch.empty(span, dtype=torch.uint8, device=self.device)
-            engine.win_presence(KIND_MEM, lo, span, own, stream)
-            thr = int(engine.win_select(KIND_MEM, lo, span, own, limit, stream).start_step)
-        info["lo"][KIND_MEM] = int(thr)
-        info["n_cand"][KIND_MEM] = int(limit)
+        lo, n_cand = int(info.lo[KIND_MEM]), int(info.n_cand[KIND_MEM])
+        if n_cand <= limit:
+            return lo, n_cand
+        hi = int(info.hi[KIND_MEM])
+        if info.dense[KIND_MEM]:  # consecutive ids
+            return hi - limit + 1, limit
+        # holes / re-flushed ids: select the newest `limit` of its own
+        span = hi - lo + 1
+        own = torch.empty(span, dtype=torch.uint8, device=self.device)
+        engine.win_presence(KIND_MEM, lo, span, own, stream)
+        return int(engine.win_select(KIND_MEM, lo, span, own, limit, stream).start_step), limit
 
     # ------------------------------------------------------------------ native sequencing
     def _native_ok(self) -> bool:
@@ -515,9 +526,6 @@ class WindowReducer:
                               self.speculate, ptr or 0, self.comm.index, world,
                               _stream_of(self.device) if stream is None else stream, prev=prev)
 
-    def _reduce_native(self, window: int, proc_rows: Optional[int], stream: int) -> ReduceOutput:
-        return self.convert_native(self.run_native(window, proc_rows, stream), window, proc_rows)
-
     @staticmethod
     def native_timings(o) -> Dict[str, float]:
         names = ("prepare", "align", "reduce", "bands", "total")
@@ -526,78 +534,10 @@ class WindowReducer:
         t["k3a"], t["k4"] = float(o.k3a_ms), max(0.0, float(o.k4_ms))
         return t
 
-    def convert_native(self, o, window: int, proc_rows: Optional[int]) -> ReduceOutput:
-        R = int(o.n_ranks)
-        infos = {r: self._info_dict(o.infos[r]) for r in range(R)}
-        proc_aggs: Dict[int, Dict[str, Any]] = {}
-        if proc_rows:
-            for r in range(R):
-                pa = {f: getattr(o.procs[r], f) for f in _PROC_FIELDS}
-                for f in _PROC_INT_FIELDS:
-                    pa[f] = int(pa[f])
-                proc_aggs[r] = pa
-
-        def kind(k) -> KindResult:
-            res = KindResult(observed=int(k.observed), n_common=int(k.n_common))
-            for i in range(int(k.n_used)):
-                r = int(k.used[i])
-                res.windows[r] = RankWindow(rank=r, n_rows=int(k.n_rows[i]), t_sums=k.t_sums[i][:],
-                                            m_sums=k.m_sums[i][:], info=infos[r])
-            res.used = sorted(res.windows)
-            if res.windows:
-                res.start_step, res.end_step = int(k.start_step), int(k.end_step)
-            n = int(k.n_common)
-            if k.has_bands:
-                res.band_sum = [k.band_sum[s][:] for s in range(16)]
-                res.band_cnt = [k.band_cnt[s][:] for s in range(16)]
-                res.tail_first, res.tail_last = k.tail_first[:], k.tail_last[:]
-            if k.series and n:
-                from .engine import _DevView
-                ld = int(k.series_ld)
-                res.series = torch.as_tensor(_DevView(int(k.series), _abi.TML_SERIES_PER_STEP * ld),
-                                             device=self.device).view(_abi.TML_SERIES_PER_STEP, ld)[:, :n]
-            res.shard = (int(k.shard_lo), int(k.shard_hi))
-            return res
-
-        timings = self.native_timings(o)
-        self.last_exchanges = int(o.n_exchanges)
-        return ReduceOutput(window=window, ranks=list(range(R)), infos=infos, time=kind(o.time), mem=kind(o.mem),
-                            exchange=_abi.XCHG_NAME[int(o.exchange_used)], fused_pass=bool(o.fused_pass),
-                            timings_ms=timings, proc_aggs=proc_aggs)
-
-    @staticmethod
-    def run_out(out: ReduceOutput) -> _abi.ReduceRunOut:
-        """The inverse of ``convert_native``: the result ``tml_reduce_run`` would have produced for
-        ``out``, in every field the section emitter (``tml_sections_json``) reads -- so the Python
-        staging and the native driver share one emitter."""
-        o = _abi.ReduceRunOut()
-        o.n_ranks = len(out.ranks)
-        for r in out.ranks:
-            d, i = out.infos[r], o.infos[r]
-            i.n_retained, i.latest_step, i.monotone, i.dup_rows = d["n_retained"], d["latest_step"], d["monotone"], d["dup_rows"]
-            for q in range(2):
-                i.n_rows[q], i.n_cand[q], i.lo[q], i.hi[q] = d["n_rows"][q], d["n_cand"][q], d["lo"][q], d["hi"][q]
-                i.dense[q] = d["dense"][q]
-            i.t_sums[:] = d["t_sums"]
-            i.t_count, i.n_both = d["t_count"], d["n_both"]
-            if r in out.proc_aggs:
-                for f in _PROC_FIELDS:
-                    setattr(o.procs[r], f, out.proc_aggs[r][f])
-        for k, res in ((o.time, out.time), (o.mem, out.mem)):
-            k.observed, k.n_common = res.observed, res.n_common
-            k.n_used = len(res.used)
-            k.start_step, k.end_step = res.start_step or 0, res.end_step or 0
-            for idx, r in enumerate(res.used):
-                w = res.windows[r]
-                k.used[idx], k.n_rows[idx] = r, w.n_rows
-                k.t_sums[idx][:] = w.t_sums
-                k.m_sums[idx][:] = w.m_sums
-            if res.band_sum is not None:
-                k.has_bands = 1
-                for s in range(16):
-                    k.band_sum[s][:], k.band_cnt[s][:] = res.band_sum[s], res.band_cnt[s]
-                k.tail_first[:], k.tail_last[:] = res.tail_first, res.tail_last
-        return o
+    def native_result(self, o, window: int) -> ReduceResult:
+        """The view of a ``run_native`` result, over its own copy: the engine reuses its struct."""
+        return ReduceResult(type(o).from_buffer_copy(o), window, _abi.XCHG_NAME[int(o.exchange_used)],
+                            self.native_timings(o), device=self.device)
 
     # ------------------------------------------------------------------ alignment
     def _spec_len(self) -> int:
@@ -608,23 +548,24 @@ class WindowReducer:
             self.exchange == "p2p" or (self.exchange == "auto" and self._peers_on_this_host()))
         return _ALIGN_LEN if handles else 15
 
-    def _align(self, kind: int, window: int, infos, ranks, stream, spec=None) -> KindResult:
-        res = KindResult()
-        part = [r for r in ranks if infos[r]["n_cand"][kind] > 0]
+    def _align(self, kind: int, window: int, infos, R: int, res, stream, spec=None) -> Dict[int, bytes]:
+        """The alignment of ``kind`` over the ``R`` ranks' ``infos``, into ``res`` (a
+        ``KindResultC``); the CUDA-IPC rows handle of every used rank (see ``_parse_aligns``)."""
+        part = [r for r in range(R) if infos[r].n_cand[kind] > 0]
         res.observed = len(part)
         if not part:
-            return res
-        glo = max(infos[r]["lo"][kind] for r in part)
-        ghi = min(infos[r]["hi"][kind] for r in part)
+            return {}
+        glo = max(infos[r].lo[kind] for r in part)
+        ghi = min(infos[r].hi[kind] for r in part)
         if ghi < glo:
-            return res
+            return {}
         span = ghi - glo + 1
         dev = self.device
-        if all(infos[r]["dense"][kind] for r in part):
+        if all(infos[r].dense[kind] for r in part):
             if (spec is not None and span <= window
-                    and all(infos[r]["lo"][kind] == glo and infos[r]["hi"][kind] == ghi for r in part)):
+                    and all(infos[r].lo[kind] == glo and infos[r].hi[kind] == ghi for r in part)):
                 # every participant speculated on exactly [glo, ghi]: its block is the alignment
-                return self._parse_aligns(res, spec, self._spec_len(), part, infos)
+                return self._parse_aligns(res, spec, self._spec_len(), part)
             # lock-step fast path: every participant holds every step id of [glo, ghi]
             n_common = min(span, window)
             first = ghi - n_common + 1
@@ -632,7 +573,7 @@ class WindowReducer:
             for l, e in enumerate(self.engines):
                 a = e.win_select_dense(kind, first, n_common, stream)
                 flat.extend(self._align_pack(e, kind, a))
-            return self._collect_aligns(kind, res, flat, part, infos)
+            return self._collect_aligns(res, flat, part)
         presence = None
         for l, e in enumerate(self.engines):
             p = torch.empty(span, dtype=torch.uint8, device=dev)
@@ -643,7 +584,7 @@ class WindowReducer:
         for l, e in enumerate(self.engines):
             a = e.win_select(kind, glo, span, presence, window, stream)
             flat.extend(self._align_pack(e, kind, a))
-        return self._collect_aligns(kind, res, flat, part, infos)
+        return self._collect_aligns(res, flat, part)
 
     def _align_pack(self, engine, kind, a, length: Optional[int] = None) -> List[float]:
         """15 numbers + (p2p only) the rows' CUDA-IPC handle, so the peer mapping
@@ -659,38 +600,30 @@ class WindowReducer:
             out += [0.0] * (length - len(out))
         return out
 
-    def _collect_aligns(self, kind, res, flat, part, infos) -> KindResult:
+    def _collect_aligns(self, res, flat, part) -> Dict[int, bytes]:
         # n_common is identical on every rank, so every rank packed the same layout
         alen = _ALIGN_LEN if len(flat) == _ALIGN_LEN * self.L else 15
-        return self._parse_aligns(res, self.comm.all_gather_vec(flat, self.device), alen, part, infos)
+        return self._parse_aligns(res, self.comm.all_gather_vec(flat, self.device), alen, part)
 
-    def _parse_aligns(self, res, rows, alen, part, infos) -> KindResult:
-        res.handles = {}
-        gathered = []
-        p2p = alen == _ALIGN_LEN
-        for row in rows:
-            lst = []
-            for l in range(self.L):
-                v = row[l * alen:(l + 1) * alen]
-                lst.append({"n_common": int(round(v[0])), "start": int(round(v[1])),
-                            "end": int(round(v[2])), "n_rows": int(round(v[3])),
-                            "t_sums": list(v[4:11]), "m_sums": list(v[11:15]),
-                            "handle": bytes(int(round(b)) for b in v[15:87]) if p2p else b""})
-            gathered.append(lst)
-        n_common = max(a["n_common"] for lst in gathered for a in lst)
-        res.n_common = n_common
-        if n_common == 0:
-            return res
-        for p, lst in enumerate(gathered):
-            for l, a in enumerate(lst):
-                r = p * self.L + l
-                if r in part and a["n_rows"] > 0:
-                    res.windows[r] = RankWindow(rank=r, n_rows=a["n_rows"], t_sums=a["t_sums"],
-                                                m_sums=a["m_sums"], info=infos[r])
-                    res.handles[r] = a["handle"]
-                    res.start_step, res.end_step = a["start"], a["end"]
-        res.used = sorted(res.windows)
-        return res
+    def _parse_aligns(self, res, rows, alen, part) -> Dict[int, bytes]:
+        """``res``'s alignment from the gathered blocks, ``alen`` numbers per rank: the ranks of
+        ``part`` with aligned rows, in ascending order.  Returns their rows handles (empty unless
+        the blocks carry them: p2p)."""
+        i = lambda x: int(round(x))  # noqa: E731
+        blocks = [row[l * alen:(l + 1) * alen] for row in rows for l in range(self.L)]  # by global rank
+        res.n_common = max(i(v[0]) for v in blocks)
+        handles: Dict[int, bytes] = {}
+        if res.n_common == 0:
+            return handles
+        for r, v in enumerate(blocks):
+            if r in part and i(v[3]) > 0:
+                u = res.n_used
+                res.used[u], res.n_rows[u] = r, i(v[3])
+                res.t_sums[u][:], res.m_sums[u][:] = list(v[4:11]), list(v[11:15])
+                res.start_step, res.end_step = i(v[1]), i(v[2])
+                res.n_used = u + 1
+                handles[r] = bytes(i(b) for b in v[15:87]) if alen == _ALIGN_LEN else b""
+        return handles
 
     # ------------------------------------------------------------------ exchange
     # One-shot cost of the fused peer-load exchange is the CUDA-IPC mapping of R-1 peer
@@ -714,17 +647,18 @@ class WindowReducer:
             return "a2a" if self.L == 1 else "nccl"
         return "p2p"
 
-    def _reduce_pass(self, kind: int, mask: int, res: KindResult, stream, mode: str) -> None:
+    def _reduce_pass(self, kind: int, mask: int, res, handles: Dict[int, bytes], stream,
+                     mode: str) -> torch.Tensor:
+        """The per-step series of ``res``'s aligned window, over the row exchange ``mode``: fills
+        ``res``'s series fields and returns the [16, n_common] tensor they point into."""
         n = res.n_common
-        used = res.used
-        R = len(used)
+        used = res.used[:res.n_used]
         dev = self.device
         # series buffer of this process: [16, n]; only this process's shard is written
         series = torch.empty(_abi.TML_SERIES_PER_STEP * n, dtype=torch.float64, device=dev)
         my = [self._grank(l) for l in range(self.L)]
         # rows handle per used rank
         rows: Dict[int, Any] = {}
-        local_used = [r for r in used if r in my]
         if mode == "local":
             for r in used:
                 rows[r] = self.engines[r - self.comm.index * self.L].win_rows_tensor(kind, n)
@@ -769,7 +703,7 @@ class WindowReducer:
                 if r in my:
                     rows[r] = self.engines[r - self.comm.index * self.L].win_rows_tensor(kind, n)
                 else:
-                    rows[r] = e0.peer_open(res.handles[r])
+                    rows[r] = e0.peer_open(handles[r])
         # step-sharded: shard s of W_total shards -> engine with global rank s
         W = self.comm.world * self.L
         lo_first, hi_last = None, None
@@ -789,57 +723,41 @@ class WindowReducer:
         if timed:
             k1.record()
             self._k4_events.append((k0, k1))
-        res.series = series.view(_abi.TML_SERIES_PER_STEP, n)
-        res.shard = (lo_first or 0, hi_last or 0)
+        res.series, res.series_ld = series.data_ptr(), n
+        res.shard_lo, res.shard_hi = lo_first or 0, hi_last or 0
+        return series.view(_abi.TML_SERIES_PER_STEP, n)
 
     # ------------------------------------------------------------------ bands
-    def _bands(self, t_res: KindResult, m_res: KindResult, same: bool, stream) -> None:
-        def run(res: KindResult, kinds):
-            n = res.n_common
-            if n == 0 or res.series is None:
-                return
-            a = _abi.BandArgs()
-            a.n_common = n
-            a.shard_lo, a.shard_hi = res.shard
-            lay_t = trend_layout(n, min_points=200, warmup_frac=0.10)
-            lay_m = trend_layout(n, min_points=50, warmup_frac=0.0)
-            for k, lay in ((0, lay_t), (1, lay_m)):
-                for b in range(3):
-                    a.band_lo[k][b] = lay[b][0] if lay else 0
-                    a.band_hi[k][b] = lay[b][1] if lay else 0
-            a.tail_first[0] = 0
-            a.tail_first[1] = n - min(n, 1000)
-            out = self.engines[0].win_bands(res.series, a, stream)
-            vec = ([float(out.sum[s][b]) for s in range(16) for b in range(3)]
-                   + [float(out.cnt[s][b]) for s in range(16) for b in range(3)]
-                   + [float(out.tail_first[s]) for s in range(16)]
-                   + [float(out.tail_last[s]) for s in range(16)])
-            parts = []
-            for row in self.comm.all_gather_vec(vec, self.device):
-                parts.append({
-                    "sum": [[row[s * 3 + b] for b in range(3)] for s in range(16)],
-                    "cnt": [[int(round(row[48 + s * 3 + b])) for b in range(3)] for s in range(16)],
-                    "tf": row[96:112], "tl": row[112:128]})
-            res.band_sum = [[sum(p["sum"][s][b] for p in parts) for b in range(3)] for s in range(16)]
-            res.band_cnt = [[sum(p["cnt"][s][b] for p in parts) for b in range(3)] for s in range(16)]
-
-            def pick(key, s):
-                for p in parts:
-                    v = p[key][s]
-                    if not math.isnan(v):
-                        return v
-                return float("nan")
-
-            res.tail_first = [pick("tf", s) for s in range(16)]
-            res.tail_last = [pick("tl", s) for s in range(16)]
-
-        run(t_res, (0,))
-        if same:
-            m_res.band_sum, m_res.band_cnt = t_res.band_sum, t_res.band_cnt
-            m_res.tail_first, m_res.tail_last = t_res.tail_first, t_res.tail_last
-        else:
-            run(m_res, (1,))
+    def _bands(self, res, series: Optional[torch.Tensor], stream) -> None:
+        """``res``'s trend bands from this process's shard of ``series``, summed over the ranks."""
+        n = res.n_common
+        if n == 0 or series is None:
+            return
+        a = _abi.BandArgs()
+        a.n_common = n
+        a.shard_lo, a.shard_hi = res.shard_lo, res.shard_hi
+        lay_t = trend_layout(n, min_points=200, warmup_frac=0.10)
+        lay_m = trend_layout(n, min_points=50, warmup_frac=0.0)
+        for k, lay in ((0, lay_t), (1, lay_m)):
+            for b in range(3):
+                a.band_lo[k][b] = lay[b][0] if lay else 0
+                a.band_hi[k][b] = lay[b][1] if lay else 0
+        a.tail_first[0] = 0
+        a.tail_first[1] = n - min(n, 1000)
+        out = self.engines[0].win_bands(series, a, stream)
+        vec = ([float(out.sum[s][b]) for s in range(16) for b in range(3)]
+               + [float(out.cnt[s][b]) for s in range(16) for b in range(3)]
+               + [float(out.tail_first[s]) for s in range(16)]
+               + [float(out.tail_last[s]) for s in range(16)])
+        rows = self.comm.all_gather_vec(vec, self.device)
+        for s in range(16):
+            for b in range(3):  # sums in rank order
+                res.band_sum[s][b] = sum(row[s * 3 + b] for row in rows)
+                res.band_cnt[s][b] = sum(int(round(row[48 + s * 3 + b])) for row in rows)
+            # the tails come from the one rank whose shard holds their step
+            res.tail_first[s] = next((row[96 + s] for row in rows if not math.isnan(row[96 + s])), math.nan)
+            res.tail_last[s] = next((row[112 + s] for row in rows if not math.isnan(row[112 + s])), math.nan)
+        res.has_bands = 1
 
 
-__all__ = ["WindowReducer", "LocalComm", "TorchDistComm", "ReduceOutput", "KindResult",
-           "RankWindow", "trend_layout"]
+__all__ = ["WindowReducer", "LocalComm", "TorchDistComm", "ReduceResult", "ReduceKind", "trend_layout"]

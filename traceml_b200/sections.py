@@ -18,7 +18,7 @@ import os
 from typing import Any, Dict, Optional, Sequence
 
 from . import _abi
-from .reduce import NativeReduceOutput, WindowReducer, _stream_of
+from .reduce import WindowReducer, _stream_of
 
 
 # ----------------------------------------------------------------------------- process
@@ -252,14 +252,12 @@ class SummaryEngine:
             # JSON emitter out of the time the GPU waits for the host.
             prev = self._unemitted
             o = self.reducer.run_native(w, rows, prev=prev if prev is not None and prev._raw is None else None)
-            red = NativeReduceOutput(self.reducer, o, w, rows)
-            src = red._snap
+            red = self.reducer.native_result(o, w)
         else:
             red = self.reducer.reduce(w, proc_rows=rows, stage_timings=timings)
-            src = WindowReducer.run_out(red)
         # ram_total / gpu_count are per-host constants (psutil.virtual_memory().total,
         # torch.cuda.device_count()); single-node scope: identical on every rank
-        res = _abi.Sections(src=src, args=_abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0))
+        res = _abi.Sections(src=red.out, args=_abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0))
         res["reduce"] = red
         res["system"] = self._system_section(seng)
         if native:

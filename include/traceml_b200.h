@@ -144,7 +144,8 @@ int tml_phase_host(tml_ctx* ctx, uint32_t phase, uint64_t dur_ns);
 /* Close the step: commit kernel stages the in-flight record through shared
  * memory, merges the host-clock phases and the allocator peaks (c10 allocator
  * counters are host state: they travel as launch arguments), writes one
- * coalesced 128-B line into the HBM ring, updates the running statistics and
+ * record into the HBM ring (kept there as a 64-B hot half, a 64-B cold half
+ * and a memory byte), updates the running statistics and
  * bumps the head.  It writes NOTHING to host memory and issues no system-scope
  * fence: the training stream pays for the record, not for the sampler.
  * Replaces StepMemoryTracker.record + flush_step_events:
@@ -197,7 +198,10 @@ uint64_t tml_launch_count(tml_ctx* ctx); /* kernels launched by this context */
 uint64_t tml_proc_count(tml_ctx* ctx);
 
 /* Bulk append of already-formed records from HOST memory (replay, resume,
- * or a rank that spooled to disk): one async H2D copy per contiguous span. */
+ * or a rank that spooled to disk), asynchronous on `stream`: the records go
+ * through bounded device staging chunks and are split into the ring's layout;
+ * keep host_records alive until `stream` is synchronised.  If n > ring_slots
+ * only the last ring_slots records are kept. */
 int tml_ring_load(tml_ctx* ctx, const tml_step_record* host_records, uint64_t n,
                   void* stream);
 int tml_proc_load(tml_ctx* ctx, const tml_proc_record* host_records, uint64_t n,

@@ -15,8 +15,9 @@ line:
   * ``kernel_ms``: device time per build of each kernel (torch.profiler, a run of its own), and
     ``device_idle_ms``: ``build_ms`` minus the pass and the band kernel;
   * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved), CUDA events,
-    median of 25 after warm-up; the fused pass against it, counting the bytes it moves: W * 192 when
-    each median / worst series pair is stored once (``series_paired``), W * 256 otherwise;
+    median of 25 after warm-up; the fused pass against it, counting the bytes it moves: the 64-B hot
+    half of each ring record and its memory byte, plus W * 64 of series when each median / worst
+    series pair is stored once (``series_paired``, W * 129 in all), W * 128 otherwise (W * 193);
   * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
 """
 from __future__ import annotations
@@ -188,9 +189,9 @@ def measure(steps: int, window: int, warmup: int) -> dict:
     med = {k: statistics.median(v) for k, v in stage.items() if not k.startswith("host_")}
     wall_ms, sj_ms = statistics.median(wall), statistics.median(sj)
     ceil = copy_ceiling(torch)
-    # 128 B record read per step, plus 8 series x 8 B written when the pairs are mapped twice
-    # (series_paired), 16 x 8 B otherwise
-    fused_bytes = W * (192.0 if paired else 256.0)
+    # 65 B read per step (the ring's hot half and memory byte), plus 8 series x 8 B written when the
+    # pairs are mapped twice (series_paired), 16 x 8 B otherwise
+    fused_bytes = W * (129.0 if paired else 193.0)
     k3a = med.get("k3a") or 0.0
     fused_gbps = fused_bytes / (k3a * 1e-3) / 1e9 if k3a else None
     return {

@@ -314,6 +314,9 @@ SIGNATURES = {
                                    C.POINTER(C.c_int)]),
     # private: K6s on the native driver's side stream, behind the caller's stream
     "tml_sys_reduce_beside_": (C.c_int, [vp, u32, vp]),
+    # private: the step ring's records rebuilt from its device layout; tml_ring_load's staging chunk
+    "tml_ring_read_": (C.c_int, [vp, u64, u64, vp, vp]),
+    "tml_ring_load_chunk_": (u64, []),
 }
 
 _LIB: Optional[C.CDLL] = None

@@ -26,25 +26,26 @@ __global__ void k_comb_head(const DevState* __restrict__ st, CombAcc* acc) { acc
 
 // K7a: last `lookback` ring records -> rows / step ids / candidate flags.
 __global__ void __launch_bounds__(CB_THREADS) k_comb_rows(
-    const tml_step_record* __restrict__ ring, u32 ring_slots,
-    u32 lookback, u32 kind, tml_window_row* __restrict__ rows, u64* __restrict__ steps,
+    StepRing ring, u32 lookback, u32 kind, tml_window_row* __restrict__ rows, u64* __restrict__ steps,
     u8* __restrict__ cand, CombAcc* acc) {
   const u64 head = acc->head;
+  const u32 ring_slots = ring.slots;
   u64 n = head < (u64)ring_slots ? head : (u64)ring_slots;
   if (n > lookback) n = lookback;
   const u64 first_k = head - n;
   u64 lo = ~0ull, hi = 0, latest = 0;
   u32 nc = 0, viol = 0;
   for (u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (u64)gridDim.x * blockDim.x) {
-    const tml_step_record* r = &ring[(first_k + i) % ring_slots];
+    const u64 slot = (first_k + i) % ring_slots;
+    const RingHot* r = &ring.hot[slot];
     const u64 step = r->step;
     tml_window_row o;
-    o.dataloader = ns_to_ms(r->dur_ns[0]);
-    o.h2d = ns_to_ms(r->dur_ns[1]);
-    o.forward = ns_to_ms(r->dur_ns[2]);
-    o.backward = ns_to_ms(r->dur_ns[3]);
-    o.optimizer = ns_to_ms(r->dur_ns[4]);
-    o.step_wall = ns_to_ms(r->dur_ns[5]);
+    o.dataloader = ns_to_ms(r->dl);
+    o.h2d = ns_to_ms(ring.cold[slot].h2d);
+    o.forward = ns_to_ms(r->fwd);
+    o.backward = ns_to_ms(r->bwd);
+    o.optimizer = ns_to_ms(r->opt);
+    o.step_wall = ns_to_ms(r->wall);
     o.peak_alloc = (double)r->peak_alloc;
     o.peak_resv = (double)r->peak_resv;
     rows[i] = o;
@@ -53,11 +54,11 @@ __global__ void __launch_bounds__(CB_THREADS) k_comb_rows(
     // view only sees rows whose peaks are not NULL (common.py:143-150): newest such row
     bool last_of_step = true;
     if (i + 1 < n) {
-      const tml_step_record* nx = &ring[(first_k + i + 1) % ring_slots];
-      last_of_step = nx->step != step || (kind == TML_KIND_MEM && (nx->flags & TML_REC_HAS_MEM) == 0u);
+      const u64 nx = (first_k + i + 1) % ring_slots;
+      last_of_step = ring.hot[nx].step != step || (kind == TML_KIND_MEM && ring.mem[nx] == 0);
     }
-    if (kind == TML_KIND_MEM && (r->flags & TML_REC_HAS_MEM) == 0u) last_of_step = false;
-    if (i > 0 && ring[(first_k + i - 1) % ring_slots].step > step) ++viol;
+    if (kind == TML_KIND_MEM && ring.mem[slot] == 0) last_of_step = false;
+    if (i > 0 && ring.hot[(first_k + i - 1) % ring_slots].step > step) ++viol;
     if (i == 0) acc->first_step = step;
     cand[i] = last_of_step ? 1 : 0;
     if (last_of_step) { lo = step < lo ? step : lo; hi = step > hi ? step : hi; ++nc; }
@@ -287,7 +288,7 @@ int tml_combined_prepare(tml_ctx* c, uint32_t kind, uint32_t lookback, void* str
   if (grid > c->n_sms) grid = c->n_sms;
   k_comb_head<<<1, 1, 0, s>>>(c->d_state, w->d_acc);
   CK(cudaPeekAtLastError());
-  k_comb_rows<<<grid, CB_THREADS, 0, s>>>(c->d_ring, c->ring_slots, (u32)lb, kind, w->d_rows, w->d_steps,
+  k_comb_rows<<<grid, CB_THREADS, 0, s>>>(c->ring, (u32)lb, kind, w->d_rows, w->d_steps,
                                           w->d_cand, w->d_acc);
   CK(cudaPeekAtLastError());
   c->launches += 2;

@@ -2,8 +2,8 @@
 //
 // Kernel map (DESIGN.md section 4):
 //   K1  k_stamp_begin / k_stamp_end   %globaltimer phase stamps on the training stream
-//   K2  k_commit                      in-flight record -> smem -> one 128-B line in the
-//                                     HBM ring (+ host-mapped mirror), running stats
+//   K2  k_commit                      in-flight record -> smem -> the HBM ring's hot and cold
+//                                     halves + memory byte, running stats
 //   K5  k_proc_commit                 64-B process sample into the proc ring
 //   K3a k_window_rows                 ring -> WindowRow[] (ns->ms), step ids, flags, bounds
 //   K3b k_presence                    presence bytes over [glo, glo+span)
@@ -19,7 +19,7 @@
 //
 // Nothing here is a dense contraction: no tensor-core path.  Every bulk kernel
 // is HBM-bound; accesses are 16-byte vectorised and warp-coalesced, tiles are
-// staged through swizzled shared memory where the record layout (AoS, 128 B)
+// staged through swizzled shared memory where the record layout (64-B hot halves)
 // would otherwise make a warp touch 32 lines per load.
 
 #include <cuda_runtime.h>
@@ -48,6 +48,70 @@ static_assert(sizeof(tml_step_record) == 128, "StepRecord must be 128 B");
 static_assert(sizeof(tml_window_row) == 64, "WindowRow must be 64 B");
 static_assert(sizeof(tml_proc_record) == 64, "ProcRecord must be 64 B");
 static_assert(sizeof(tml_sys_gpu) == 32 && sizeof(tml_sys_record) == 576, "SysRecord must be 64 + 16 x 32 B");
+
+// ------------------------------------------------------------------ step ring layout (device only)
+// Slot k of the step ring is the public 128-B tml_step_record split in two 64-B halves plus a byte.
+// The window pass reads only the hot half and the memory byte (65 B per step, not 128); the cold
+// half holds what only the drain, the staged rows (h2d) and the live tick read.
+struct RingHot {
+  u64 step;
+  u64 dl, fwd, bwd, opt, wall;  // dur_ns[0], dur_ns[2..5]
+  u64 peak_alloc, peak_resv;
+};
+struct RingCold {
+  u64 h2d;  // dur_ns[1]: first, so a reader of h2d alone touches one 32-B sector
+  u32 n_calls[TML_N_PHASES];
+  double host_ts;
+  u32 gpu_mask;
+  u32 flags;
+  u64 seq;
+  u64 pad;
+};
+struct StepRing {
+  RingHot* hot;
+  RingCold* cold;
+  u8* mem;  // 1 when the slot's flags have TML_REC_HAS_MEM (a copy of the bit in the cold half)
+  u32 slots;
+};
+static_assert(sizeof(RingHot) == 64 && sizeof(RingCold) == 64, "ring halves must be 64 B");
+// The mem array is read in 16-B pieces from the 16-B boundary at or below a tile's first slot:
+// it is allocated with this many bytes past the last slot.
+#define RING_MEM_PAD 32u
+
+// 8-B word w of tml_step_record is ring word ring_word(w): 0..7 in the hot half, 8..15 in the cold
+// half (nibble w of the constant).
+#define RING_WORD_MAP 0xFEDC76BA95432810ull
+__host__ __device__ constexpr int ring_word(int w) { return (int)((RING_WORD_MAP >> (4 * w)) & 15ull); }
+#define TML_RW(pub, half, off) \
+  static_assert(ring_word(offsetof(tml_step_record, pub) / 8) == (half) * 8 + (int)(off) / 8, #pub)
+TML_RW(step, 0, offsetof(RingHot, step));
+TML_RW(dur_ns[0], 0, offsetof(RingHot, dl));
+TML_RW(dur_ns[1], 1, offsetof(RingCold, h2d));
+TML_RW(dur_ns[2], 0, offsetof(RingHot, fwd));
+TML_RW(dur_ns[3], 0, offsetof(RingHot, bwd));
+TML_RW(dur_ns[4], 0, offsetof(RingHot, opt));
+TML_RW(dur_ns[5], 0, offsetof(RingHot, wall));
+TML_RW(n_calls[0], 1, offsetof(RingCold, n_calls[0]));
+TML_RW(n_calls[2], 1, offsetof(RingCold, n_calls[2]));
+TML_RW(n_calls[4], 1, offsetof(RingCold, n_calls[4]));
+TML_RW(peak_alloc, 0, offsetof(RingHot, peak_alloc));
+TML_RW(peak_resv, 0, offsetof(RingHot, peak_resv));
+TML_RW(host_ts, 1, offsetof(RingCold, host_ts));
+TML_RW(gpu_mask, 1, offsetof(RingCold, gpu_mask));
+TML_RW(seq, 1, offsetof(RingCold, seq));
+TML_RW(_pad, 1, offsetof(RingCold, pad));
+#undef TML_RW
+static_assert(offsetof(tml_step_record, flags) - offsetof(tml_step_record, gpu_mask) ==
+              offsetof(RingCold, flags) - offsetof(RingCold, gpu_mask), "gpu_mask | flags share a word");
+#define RING_FLAGS_WORD 13  // public word holding gpu_mask (low) | flags (high)
+static_assert(offsetof(tml_step_record, gpu_mask) == RING_FLAGS_WORD * 8, "flags word");
+
+// public word w of slot `slot` (the drain mirror and the test readback rebuild records with it)
+__device__ __forceinline__ u64 ring_word_at(const StepRing& ring, u64 slot, int w) {
+  const int d = ring_word(w);
+  return d < 8 ? reinterpret_cast<const u64*>(&ring.hot[slot])[d]
+               : reinterpret_cast<const u64*>(&ring.cold[slot])[d - 8];
+}
 
 #define TML_N_SLOTS 64u      // begin-timestamp slots (regions in flight)
 #define TML_N_GSLOTS 64u     // begin slots of graph-captured regions, after the host-launched ones
@@ -187,13 +251,12 @@ __global__ void __maxnreg__(24) k_stamp_end(DevState* st, u32 slot, u32 phase, u
 
 // ------------------------------------------------------------------ K2: commit
 // 6 warps: warp p owns phase p's running statistics; warp 0 also assembles the
-// 128-B record in shared memory and writes it as 8 x 16-B coalesced stores.
+// record in shared memory and writes its two 64-B ring halves (8 x 16-B stores) and the memory byte.
 
 // Nothing in here leaves the GPU: writing the record and the live statistics into host-mapped
 // memory and closing with __threadfence_system would cost the TRAINING stream time every step for
 // the benefit of a sampler that looks twice a second.  The sampler instead fetches what it needs itself (k_mirror, on its own stream, tml_drain / tml_live).
-__global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* ring, u32 ring_slots,
-                                                 CommitArgs a) {
+__global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, CommitArgs a) {
   __shared__ __align__(16) u64 rec[16];
   __shared__ u64 s_dur[TML_MAX_PHASES];
   __shared__ u32 s_calls[TML_MAX_PHASES];
@@ -279,15 +342,18 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* r
 
   if (warp == 0) {
     const u64 seq = a.seq;  // the host counts commits: no read of the head on the critical path
-    if (lane == 0) {
+    const u64 slot = seq % ring.slots;
+    if (lane == 0) {  // rec[0..8): the hot half, rec[8..16): the cold half
       rec[0] = a.step;
+      rec[1] = s_dur[0];
 #pragma unroll
-      for (int p = 0; p < 6; ++p) rec[1 + p] = s_dur[p];
-      rec[7] = (u64)s_calls[0] | ((u64)s_calls[1] << 32);
-      rec[8] = (u64)s_calls[2] | ((u64)s_calls[3] << 32);
-      rec[9] = (u64)s_calls[4] | ((u64)s_calls[5] << 32);
-      rec[10] = a.peak_alloc;
-      rec[11] = a.peak_resv;
+      for (int p = 2; p < 6; ++p) rec[p] = s_dur[p];
+      rec[6] = a.peak_alloc;
+      rec[7] = a.peak_resv;
+      rec[8] = s_dur[1];
+      rec[9] = (u64)s_calls[0] | ((u64)s_calls[1] << 32);
+      rec[10] = (u64)s_calls[2] | ((u64)s_calls[3] << 32);
+      rec[11] = (u64)s_calls[4] | ((u64)s_calls[5] << 32);
       rec[12] = (u64)__double_as_longlong(a.host_ts);
       rec[13] = (u64)s_mask | ((u64)a.flags << 32);
       rec[14] = seq;
@@ -296,7 +362,10 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* r
     __syncwarp();
     if (lane < 8) {
       uint4 v = reinterpret_cast<const uint4*>(rec)[lane];
-      reinterpret_cast<uint4*>(&ring[seq % ring_slots])[lane] = v;
+      uint4* half = lane < 4 ? reinterpret_cast<uint4*>(&ring.hot[slot]) : reinterpret_cast<uint4*>(&ring.cold[slot]);
+      half[lane & 3] = v;
+    } else if (lane == 8) {
+      ring.mem[slot] = (a.flags & TML_REC_HAS_MEM) ? 1 : 0;
     }
     __syncwarp();
     if (lane == 0) {
@@ -310,20 +379,18 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, tml_step_record* r
 // Sampler side: copy the records committed since `from` (at most the newest mirror_slots) and the
 // live statistics into host-mapped memory.  One CTA, on the sampler's own stream; the caller
 // synchronises that stream, so no system-scope fence is needed here either.
-__global__ void __launch_bounds__(1024) k_mirror(const DevState* st, const tml_step_record* __restrict__ ring,
-                                                  u32 ring_slots, tml_step_record* mirror, u32 mirror_slots,
-                                                  HostPage* page, u64 from) {
+__global__ void __launch_bounds__(1024) k_mirror(const DevState* st, StepRing ring, tml_step_record* mirror,
+                                                  u32 mirror_slots, HostPage* page, u64 from) {
   __shared__ u64 s_head;
   if (threadIdx.x == 0) s_head = *reinterpret_cast<const volatile u64*>(&st->head);
   __syncthreads();
   const u64 head = s_head;
   if (head - from > (u64)mirror_slots) from = head - mirror_slots;
-  const u64 n16 = (head - from) * 8ull;  // 16-B pieces
-  for (u64 k = threadIdx.x; k < n16; k += blockDim.x) {
-    const u64 seq = from + (k >> 3);
-    const int q = (int)(k & 7);
-    reinterpret_cast<uint4*>(&mirror[seq % mirror_slots])[q] =
-        reinterpret_cast<const uint4*>(&ring[seq % ring_slots])[q];
+  const u64 n8 = (head - from) * 16ull;  // 8-B words of the public records
+  for (u64 k = threadIdx.x; k < n8; k += blockDim.x) {
+    const u64 seq = from + (k >> 4);
+    const int w = (int)(k & 15);
+    reinterpret_cast<u64*>(&mirror[seq % mirror_slots])[w] = ring_word_at(ring, seq % ring.slots, w);
   }
   const int nl = (int)(sizeof(tml_live_stats) / 8);
   for (int k = threadIdx.x; k < nl; k += blockDim.x)
@@ -470,12 +537,13 @@ __global__ void k_finalize(const double* __restrict__ partials, int nblk, int nc
 }
 
 // ------------------------------------------------------------------ K3a: window rows
-// Ring (128-B AoS records) -> WindowRow[] (64 B), step ids, row flags, bounds, sums.
+// Ring (64-B hot halves, h2d from the cold halves, memory bytes) -> WindowRow[] (64 B), step ids,
+// row flags, bounds, sums.
 //   * tiles are fetched with cp.async (LDGSTS, 16 B per lane per copy, fully coalesced)
-//     into XOR-swizzled shared buffers, two per warp, so tile i+1 is in flight while
-//     tile i is converted -- without it the kernel is HBM-latency-bound (long-scoreboard
+//     into XOR-swizzled shared buffers, WR_STAGES per warp, so the next tiles are in flight
+//     while tile i is converted -- without it the kernel is HBM-latency-bound (long-scoreboard
 //     stalls);
-//   * the swizzle makes the per-lane 128-B record read bank-conflict-free;
+//   * the swizzle makes the per-lane 64-B hot record read bank-conflict-free;
 //   * rows leave through a swizzled staging buffer as coalesced 16-B stores;
 //   * integer side results live in registers for the whole persistent loop.
 
@@ -493,57 +561,99 @@ __device__ __forceinline__ double ns_to_ms(u64 ns) {
 
 #define WR_THREADS 256
 #define WR_WARPS (WR_THREADS / 32)
-// per warp: two 32-record input buffers (2 x 4 KB) + one 32-row output buffer (2 KB)
-#define WR_WARP_U4 (2 * 32 * 8 + 32 * 4)
+// Tiles in a warp's load pipeline: WR_STAGES - 1 are in flight while one is converted.  A tile's
+// hot halves are 2 KB, so 4 stages keep 6 KB per warp (96 KB per SM at 2 CTAs) in flight.
+#define WR_STAGES 4
+// one stage: 32 hot halves (2 KB), the memory bytes of the tile (3 x 16 B from the 16-B boundary at
+// or below its first slot) and, for K3a, 32 h2d words (256 B)
+#define TILE_HOT_U4 (32 * 4)
+#define TILE_MEM_U4 3
+#define TILE_H2D_U4 16
+#define WF_STAGE_U4 (TILE_HOT_U4 + TILE_MEM_U4)
+#define WR_STAGE_U4 (TILE_HOT_U4 + TILE_MEM_U4 + TILE_H2D_U4)
+// per warp: the stages + one 32-row output buffer (2 KB)
+#define WR_WARP_U4 (WR_STAGES * WR_STAGE_U4 + 32 * 4)
 #define WR_SMEM_BYTES (WR_WARPS * WR_WARP_U4 * 16)
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gsrc) : "memory");
 }
+__device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
+  unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(gsrc) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// one warp fetches its 32-record tile: 8 x cp.async per lane, each instruction = 512 B contiguous.
+// A whole tile with no ring wrap is fetched at linear addresses; any other tile slot by slot.
+__device__ __forceinline__ bool tile_linear(const StepRing& ring, u64 slot0, u64 n, u64 base) {
+  return base + 32 <= n && slot0 + 32 <= (u64)ring.slots;
+}
+
+// one warp fetches its 32-record tile into one stage: 4 x cp.async per lane for the hot halves, each
+// instruction = 512 B contiguous, stored XOR-swizzled (16-B chunk q of record r at r*4 + (q ^ (r>>1 & 3)));
+// the memory bytes; with H2D the h2d word of each record (one 32-B sector of its cold half).
 // slot0 = ring slot of the tile's first record (maintained incrementally by the caller).
-__device__ __forceinline__ void wr_issue_warp(uint4* buf, const uint4* __restrict__ ring4, u32 ring_slots,
-                                              u64 slot0, u64 n, u64 base, int lane) {
-  if (base + 32 <= n && slot0 + 32 <= (u64)ring_slots) {  // whole tile, no ring wrap: linear addresses
-    const uint4* src = ring4 + slot0 * 8;
+template <bool H2D>
+__device__ __forceinline__ void ring_issue_tile(uint4* stage, const StepRing& ring, u64 slot0, u64 n, u64 base,
+                                                int lane) {
+  const uint4* __restrict__ hot4 = reinterpret_cast<const uint4*>(ring.hot);
+  uint4* mem = stage + TILE_HOT_U4;
+  u64* h2d = reinterpret_cast<u64*>(mem + TILE_MEM_U4);
+  if (tile_linear(ring, slot0, n, base)) {
+    const uint4* src = hot4 + slot0 * 4;
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
+    for (int c = 0; c < 4; ++c) {
       const int idx = c * 32 + lane;
-      cp_async16(&buf[(idx & ~7) | ((idx ^ (idx >> 3)) & 7)], src + idx);
+      cp_async16(&stage[(idx & ~3) | ((idx ^ (idx >> 3)) & 3)], src + idx);
     }
+    if (lane < TILE_MEM_U4) cp_async16(&mem[lane], ring.mem + (slot0 & ~15ull) + 16 * lane);
+    if (H2D) cp_async8(&h2d[lane], &ring.cold[slot0 + lane].h2d);
     return;
   }
 #pragma unroll
-  for (int c = 0; c < 8; ++c) {
+  for (int c = 0; c < 4; ++c) {
     const int idx = c * 32 + lane;
-    const int r = idx >> 3, q = idx & 7;
+    const int r = idx >> 2, q = idx & 3;
     if (base + (u64)r < n) {
       u64 slot = slot0 + (u64)r;
-      while (slot >= ring_slots) slot -= ring_slots;
-      cp_async16(&buf[r * 8 + (q ^ (r & 7))], &ring4[slot * 8 + q]);
+      while (slot >= ring.slots) slot -= ring.slots;
+      cp_async16(&stage[r * 4 + (q ^ ((r >> 1) & 3))], &hot4[slot * 4 + q]);
     }
+  }
+  if (base + (u64)lane < n) {
+    u64 slot = slot0 + (u64)lane;
+    while (slot >= ring.slots) slot -= ring.slots;
+    reinterpret_cast<u8*>(mem)[lane] = ring.mem[slot];  // byte-wise: only a ring wrap or the last tile
+    if (H2D) cp_async8(&h2d[lane], &ring.cold[slot].h2d);
   }
 }
 
+// the memory byte of record `lane` of a landed tile (ring_issue_tile's two layouts)
+__device__ __forceinline__ u32 tile_mem(const uint4* stage, bool linear, u64 slot0, int lane) {
+  return reinterpret_cast<const u8*>(stage + TILE_HOT_U4)[linear ? (int)(slot0 & 15ull) + lane : lane];
+}
+
+// slot s advanced by adv (both < slots) around the ring, without leaving 32 bits
+__device__ __forceinline__ u32 slot_next(u32 s, u32 adv, u32 slots) {
+  return s >= slots - adv ? s - (slots - adv) : s + adv;
+}
+
 // K3a.  Persistent grid, WARP-PRIVATE software pipelines: every warp streams its own
-// 32-record tiles (cp.async double buffer -> XOR-swizzled smem -> registers -> swizzled
+// 32-record tiles (cp.async, WR_STAGES buffers -> XOR-swizzled smem -> registers -> swizzled
 // smem -> coalesced 16-B stores) and synchronises only with __syncwarp; neighbour step
-// ids come from warp shuffles (tile edges: two 8-B global reads).  No block barrier in
+// ids come from warp shuffles (tile edges: three small global reads).  No block barrier in
 // the loop (block barriers and waits dominate once the loads are asynchronous).
 __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
-    const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
+    StepRing ring, u64 first_k, u64 n, u64 t_start,
     tml_window_row* __restrict__ rows, u64* __restrict__ steps, u8* __restrict__ flags,
     WinAcc* acc, double* partials, double* __restrict__ csum, u64 csum_top) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint4* w_in0 = reinterpret_cast<uint4*>(wr_smem) + warp * WR_WARP_U4;
-  uint4* w_in1 = w_in0 + 32 * 8;
-  uint4* w_out = w_in1 + 32 * 8;
+  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WR_WARP_U4;
+  uint4* w_out = w_in + WR_STAGES * WR_STAGE_U4;
 
   u64 a_lo0 = ~0ull, a_lo1 = ~0ull, a_hi0 = 0, a_hi1 = 0, a_latest = 0;
   u32 a_nc0 = 0, a_nc1 = 0, a_nr0 = 0, a_nr1 = 0, a_viol = 0, a_dups = 0, a_tc = 0, a_both = 0;
@@ -552,54 +662,57 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
   double mx_a = -INFINITY, mx_r = -INFINITY;      // rank peaks over the window rows
   const u64 nwt = (n + 31) / 32;
   const u64 wstride = (u64)gridDim.x * WR_WARPS;
-  const uint4* ring4 = reinterpret_cast<const uint4*>(ring);
+  const u32 ring_slots = ring.slots;
   uint4* rows4 = reinterpret_cast<uint4*>(rows);
 
   u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-  // ring slot of this warp's current tile and the per-trip advance, both kept < ring_slots:
-  // two 64-bit modulos per warp for the whole kernel instead of one per lane per tile
-  u64 slot_cur = (first_k + wt * 32) % ring_slots;
-  const u64 slot_adv = (wstride * 32) % ring_slots;
-  if (wt < nwt) wr_issue_warp(w_in0, ring4, ring_slots, slot_cur, n, wt * 32, lane);
-  cp_async_commit();
+  // ring slots of this warp's current tile and of the next tile to issue, and the per-trip advance,
+  // all kept < ring_slots: two 64-bit modulos per warp for the whole kernel instead of one per lane per tile
+  u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
+  const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
+  u32 slot_iss = slot_cur;
+#pragma unroll
+  for (int s = 0; s < WR_STAGES - 1; ++s) {
+    const u64 t = wt + (u64)s * wstride;
+    if (t < nwt) ring_issue_tile<true>(w_in + s * WR_STAGE_U4, ring, slot_iss, n, t * 32, lane);
+    cp_async_commit();
+    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+  }
 
   for (int it = 0; wt < nwt; wt += wstride, ++it) {
-    uint4* cur = (it & 1) ? w_in1 : w_in0;
-    uint4* nxt = (it & 1) ? w_in0 : w_in1;
+    uint4* cur = w_in + (it % WR_STAGES) * WR_STAGE_U4;
     const u64 base = wt * 32;
-    const u64 next = wt + wstride;
-    u64 slot_next = slot_cur + slot_adv;
-    if (slot_next >= ring_slots) slot_next -= ring_slots;
-    if (next < nwt) wr_issue_warp(nxt, ring4, ring_slots, slot_next, n, next * 32, lane);
+    const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
+    if (ahead < nwt)
+      ring_issue_tile<true>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WR_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
     cp_async_commit();
-    const u64 slot_tile = slot_cur;  // ring slot of this tile's first record
+    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+    const u32 slot_tile = slot_cur;  // ring slot of this tile's first record
     // tile-edge neighbours (first/last-of-step tests) straight from the ring
     u64 halo_step = 0;
-    u32 halo_flags = 0;
-    if (lane == 0 && base > 0) halo_step = ring[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
+    u32 halo_mem = 0;
+    if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
     if (lane == 31 && base + 32 < n) {
-      u64 hs = slot_cur + 32;
+      u64 hs = (u64)slot_cur + 32;
       while (hs >= ring_slots) hs -= ring_slots;
-      const tml_step_record* p = &ring[hs];
-      halo_step = p->step; halo_flags = p->flags;
+      halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
     }
-    slot_cur = slot_next;
-    cp_async_wait<1>();  // this tile has landed; the next one stays in flight
+    slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
+    cp_async_wait<WR_STAGES - 1>();  // this tile has landed; the next ones stay in flight
     __syncwarp();
 
     const u64 i = base + (u64)lane;
     const bool live = i < n;
-    const int sw = lane & 7;
-    const uint4 c0 = cur[lane * 8 + (0 ^ sw)], c1 = cur[lane * 8 + (1 ^ sw)];
-    const uint4 c2 = cur[lane * 8 + (2 ^ sw)], c3 = cur[lane * 8 + (3 ^ sw)];
-    const uint4 c5 = cur[lane * 8 + (5 ^ sw)], c6 = cur[lane * 8 + (6 ^ sw)];
+    const int sw = (lane >> 1) & 3;
+    const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
+    const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
+    const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
     const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-    const u32 rflags = c6.w;
     u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
     u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
-    u32 next_flags = __shfl_down_sync(0xffffffffu, rflags, 1);
+    u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
     if (lane == 0) prev_step = halo_step;
-    if (lane == 31) { next_step = halo_step; next_flags = halo_flags; }
+    if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
     double t_dl = 0.0, t_fwd = 0.0, t_bwd = 0.0, t_opt = 0.0, t_wall = 0.0, t_tr = 0.0;  // K3e chunk sums
 
     // Time candidate: the OLDEST USABLE row of its step id inside the window.  The reference reads the
@@ -607,9 +720,9 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     // step (model.py:226-248), so a step whose oldest row is unusable is kept through a newer row.
     // A run of one step id is contiguous in a monotone ring; runs are cut at t_start.
     const bool uit_row = live && i >= t_start &&
-                         ((((u64)c0.z | ((u64)c0.w << 32)) | ((u64)c1.z | ((u64)c1.w << 32)) |
-                           ((u64)c2.x | ((u64)c2.y << 32)) | ((u64)c2.z | ((u64)c2.w << 32)) |
-                           ((u64)c3.x | ((u64)c3.y << 32))) != 0ull);  // usable: a summarised phase > 0 ns
+                         ((((u64)c0.z | ((u64)c0.w << 32)) | ((u64)c1.x | ((u64)c1.y << 32)) |
+                           ((u64)c1.z | ((u64)c1.w << 32)) | ((u64)c2.x | ((u64)c2.y << 32)) |
+                           ((u64)c2.z | ((u64)c2.w << 32))) != 0ull);  // usable: a summarised phase > 0 ns
     const u32 heads = __ballot_sync(0xffffffffu, lane == 0 || i == t_start || prev_step != step);
     const u32 uits = __ballot_sync(0xffffffffu, uit_row);
     const int head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));  // lane where this row's run starts
@@ -621,9 +734,9 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
         while (j > t_start) {
           --j;
           sl = sl == 0 ? ring_slots - 1 : sl - 1;
-          const tml_step_record* p = &ring[sl];
+          const RingHot* p = &ring.hot[sl];
           if (p->step != step) break;
-          if ((p->dur_ns[0] | p->dur_ns[2] | p->dur_ns[3] | p->dur_ns[4] | p->dur_ns[5]) != 0ull) { carry = true; break; }
+          if ((p->dl | p->fwd | p->bwd | p->opt | p->wall) != 0ull) { carry = true; break; }
         }
       }
       carry = __shfl_sync(0xffffffffu, carry, 0);
@@ -632,21 +745,21 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 
     if (live) {
       const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
-      const u64 d1 = (u64)c1.x | ((u64)c1.y << 32);
-      const u64 d2 = (u64)c1.z | ((u64)c1.w << 32);
-      const u64 d3 = (u64)c2.x | ((u64)c2.y << 32);
-      const u64 d4 = (u64)c2.z | ((u64)c2.w << 32);
-      const u64 d5 = (u64)c3.x | ((u64)c3.y << 32);
-      const u64 pa = (u64)c5.x | ((u64)c5.y << 32);
-      const u64 pr = (u64)c5.z | ((u64)c5.w << 32);
+      const u64 d1 = reinterpret_cast<const u64*>(cur + TILE_HOT_U4 + TILE_MEM_U4)[lane];
+      const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
+      const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
+      const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
+      const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
+      const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
+      const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
       const double dl = ns_to_ms(d0), h2d = ns_to_ms(d1), fwd = ns_to_ms(d2);
       const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
-      const bool has_mem = (rflags & TML_REC_HAS_MEM) != 0u;
+      const bool has_mem = rmem != 0u;
       const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
       const bool in_time = i >= t_start;
       const bool uit = usable && in_time;
       const bool has_prev = i > 0, has_next = (i + 1) < n;
-      const bool last_m = !has_next || (next_step != step) || ((next_flags & TML_REC_HAS_MEM) == 0u);
+      const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
       u8 f = 0;
       if (usable) f |= RF_USABLE;
       if (has_mem) f |= RF_HAS_MEM;
@@ -799,7 +912,8 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 
 // ------------------------------------------------------------------ K3a+K4 fused (single rank)
 // With ONE rank the cross-rank median and worst of a step are the rank's own value, so the
-// per-step series can be written straight from the ring records: 128 B in, 128 B out per step, and
+// per-step series can be written straight from the ring records: 65 B in (the hot half and the memory
+// byte), 128 B out per step, and
 // the 64-B WindowRows -- written by K3a only to be re-read by K4 (256 MB each way at
 // W = 4e6) -- never exist.  Same warp-private
 // cp.async pipeline as k_window_rows; lane = record, so each of the 16 series receives 32
@@ -812,17 +926,18 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // the partials and hand the accumulator over (k_bands).
 // Series row s starts at series + s * ld.  PAIRED: rows 2m and 2m+1 are one physical row mapped
 // twice (tml_summary.cpp), so only the even rows are stored: 64 B out per step instead of 128.
-#define WF_WARP_U4 (2 * 32 * 8)
+#define WF_WARP_U4 (WR_STAGES * WF_STAGE_U4)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
 
+// 2 CTAs of WR_THREADS per SM need <= 128 registers; left to itself ptxas takes 96 for the plain
+// instance, with the cap it keeps 94 with no spills.
 template <bool PAIRED>
-__global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
-    const tml_step_record* __restrict__ ring, u32 ring_slots, u64 first_k, u64 n, u64 t_start,
+__global__ void __maxnreg__(94) k_window_fused(
+    StepRing ring, u64 first_k, u64 n, u64 t_start,
     double* __restrict__ series, u64 ld, WinAcc* acc, double* partials) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint4* w_in0 = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
-  uint4* w_in1 = w_in0 + 32 * 8;
+  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
 
   u64 a_lo0 = ~0ull, a_lo1 = ~0ull, a_hi0 = 0, a_hi1 = 0, a_latest = 0;
   u32 a_nc0 = 0, a_nc1 = 0, a_nr0 = 0, a_nr1 = 0, a_viol = 0, a_dups = 0, a_tc = 0, a_both = 0;
@@ -831,66 +946,70 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_fused(
   double mx_a = -INFINITY, mx_r = -INFINITY;
   const u64 nwt = (n + 31) / 32;
   const u64 wstride = (u64)gridDim.x * WR_WARPS;
-  const uint4* ring4 = reinterpret_cast<const uint4*>(ring);
+  const u32 ring_slots = ring.slots;
 
   u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-  u64 slot_cur = (first_k + wt * 32) % ring_slots;
-  const u64 slot_adv = (wstride * 32) % ring_slots;
-  if (wt < nwt) wr_issue_warp(w_in0, ring4, ring_slots, slot_cur, n, wt * 32, lane);
-  cp_async_commit();
+  u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
+  const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
+  u32 slot_iss = slot_cur;
+#pragma unroll
+  for (int s = 0; s < WR_STAGES - 1; ++s) {
+    const u64 t = wt + (u64)s * wstride;
+    if (t < nwt) ring_issue_tile<false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
+    cp_async_commit();
+    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+  }
 
   for (int it = 0; wt < nwt; wt += wstride, ++it) {
-    uint4* cur = (it & 1) ? w_in1 : w_in0;
-    uint4* nxt = (it & 1) ? w_in0 : w_in1;
+    uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
     const u64 base = wt * 32;
-    const u64 next = wt + wstride;
-    u64 slot_next = slot_cur + slot_adv;
-    if (slot_next >= ring_slots) slot_next -= ring_slots;
-    if (next < nwt) wr_issue_warp(nxt, ring4, ring_slots, slot_next, n, next * 32, lane);
+    const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
+    if (ahead < nwt)
+      ring_issue_tile<false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
     cp_async_commit();
+    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+    const u32 slot_tile = slot_cur;
     u64 halo_step = 0;
-    u32 halo_flags = 0;
-    if (lane == 0 && base > 0) halo_step = ring[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
+    u32 halo_mem = 0;
+    if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
     if (lane == 31 && base + 32 < n) {
-      u64 hs = slot_cur + 32;
+      u64 hs = (u64)slot_cur + 32;
       while (hs >= ring_slots) hs -= ring_slots;
-      const tml_step_record* p = &ring[hs];
-      halo_step = p->step; halo_flags = p->flags;
+      halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
     }
-    slot_cur = slot_next;
-    cp_async_wait<1>();
+    slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
+    cp_async_wait<WR_STAGES - 1>();
     __syncwarp();
 
     const u64 i = base + (u64)lane;
     const bool live = i < n;
-    const int sw = lane & 7;
-    const uint4 c0 = cur[lane * 8 + (0 ^ sw)], c1 = cur[lane * 8 + (1 ^ sw)];
-    const uint4 c2 = cur[lane * 8 + (2 ^ sw)], c3 = cur[lane * 8 + (3 ^ sw)];
-    const uint4 c5 = cur[lane * 8 + (5 ^ sw)], c6 = cur[lane * 8 + (6 ^ sw)];
+    const int sw = (lane >> 1) & 3;
+    const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
+    const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
+    const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
     const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-    const u32 rflags = c6.w;
     u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
     u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
-    u32 next_flags = __shfl_down_sync(0xffffffffu, rflags, 1);
+    u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
     if (lane == 0) prev_step = halo_step;
-    if (lane == 31) { next_step = halo_step; next_flags = halo_flags; }
+    if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
 
     if (live) {
       const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
-      const u64 d2 = (u64)c1.z | ((u64)c1.w << 32);
-      const u64 d3 = (u64)c2.x | ((u64)c2.y << 32);
-      const u64 d4 = (u64)c2.z | ((u64)c2.w << 32);
-      const u64 d5 = (u64)c3.x | ((u64)c3.y << 32);
-      const u64 pa = (u64)c5.x | ((u64)c5.y << 32);
-      const u64 pr = (u64)c5.z | ((u64)c5.w << 32);
+      const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
+      const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
+      const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
+      const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
+      const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
+      const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
       const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
       const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
-      const bool has_mem = (rflags & TML_REC_HAS_MEM) != 0u;
+      const bool has_mem = rmem != 0u;
       const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
       const bool in_time = i >= t_start;
       const bool has_prev = i > 0, has_next = (i + 1) < n;
       const bool first_in_win = (i == t_start) || !has_prev || (prev_step != step);
-      const bool last_m = !has_next || (next_step != step) || ((next_flags & TML_REC_HAS_MEM) == 0u);
+      const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
       const bool cand_t = usable && in_time && first_in_win;
       const bool cand_m = has_mem && last_m;
       a_latest = step > a_latest ? step : a_latest;
@@ -1878,7 +1997,12 @@ struct tml_ctx {
   int n_sms = 132;
   u32 ring_slots = 0, proc_slots = 0, mirror_slots = 0, pmirror_slots = 0;
   DevState* d_state = nullptr;
-  tml_step_record* d_ring = nullptr;
+  StepRing ring = {nullptr, nullptr, nullptr, 0};  // one allocation: hot | cold | mem
+  // tml_ring_load: two staging chunks (allocated on first use), the stream that fills them and
+  // events for "chunk b copied" / "chunk b split, its buffer free"
+  void* d_load_stage = nullptr;
+  cudaStream_t load_stream = nullptr;
+  cudaEvent_t load_copied[2] = {nullptr, nullptr}, load_free[2] = {nullptr, nullptr}, load_start = nullptr;
   tml_proc_record* d_pring = nullptr;
   HostPage* h_page = nullptr;        HostPage* d_page = nullptr;
   tml_step_record* h_mirror = nullptr; tml_step_record* d_mirror = nullptr;
@@ -2119,7 +2243,15 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   if (!c->graph_refs) { delete c; return set_err(TML_ERR_NOMEM, "tml_init: host allocation failed"); }
   CK(cudaMalloc(&c->d_state, sizeof(DevState)));
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
-  CK(cudaMalloc(&c->d_ring, (size_t)ring_slots * sizeof(tml_step_record)));
+  {
+    char* p = nullptr;
+    CK(cudaMalloc(&p, (size_t)ring_slots * (sizeof(RingHot) + sizeof(RingCold) + 1) + RING_MEM_PAD));
+    c->ring.hot = reinterpret_cast<RingHot*>(p);
+    c->ring.cold = reinterpret_cast<RingCold*>(p + (size_t)ring_slots * sizeof(RingHot));
+    c->ring.mem = reinterpret_cast<u8*>(p + (size_t)ring_slots * (sizeof(RingHot) + sizeof(RingCold)));
+    c->ring.slots = ring_slots;
+    CK(cudaMemset(c->ring.mem, 0, (size_t)ring_slots + RING_MEM_PAD));  // the pad is read, never used
+  }
   CK(cudaMalloc(&c->d_pring, (size_t)proc_slots * sizeof(tml_proc_record)));
   CK(cudaHostAlloc(&c->h_page, sizeof(HostPage), cudaHostAllocMapped));
   memset(c->h_page, 0, sizeof(HostPage));
@@ -2159,7 +2291,14 @@ int tml_shutdown(tml_ctx* c) {
   const u64 graphs_live = c->graph_refs->graphs.load();
   if (!graphs_live) { cudaFree(c->d_state); cudaFree(c->d_layer_acc); }
   if (c->graph_refs->owners.fetch_sub(1) == 1) delete c->graph_refs;
-  cudaFree(c->d_ring); cudaFree(c->d_pring);
+  cudaFree(c->ring.hot); cudaFree(c->d_pring);
+  cudaFree(c->d_load_stage);
+  if (c->load_stream) cudaStreamDestroy(c->load_stream);
+  for (int b = 0; b < 2; ++b) {
+    if (c->load_copied[b]) cudaEventDestroy(c->load_copied[b]);
+    if (c->load_free[b]) cudaEventDestroy(c->load_free[b]);
+  }
+  if (c->load_start) cudaEventDestroy(c->load_start);
   cudaFreeHost(c->h_page); cudaFreeHost(c->h_mirror); cudaFreeHost(c->h_pmirror);
   cudaFree(c->d_rows); cudaFree(c->d_steps); cudaFree(c->d_flags);
   for (int k = 0; k < 2; ++k) { cudaFree(c->d_rowof[k]); cudaFree(c->d_xrows[k]); }
@@ -2468,7 +2607,7 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
   a.peak_alloc = peak_alloc;
   a.peak_resv = peak_resv;
   a.seq = c->commits;
-  k_commit<<<1, 192, 0, s>>>(c->d_state, c->d_ring, c->ring_slots, a);
+  k_commit<<<1, 192, 0, s>>>(c->d_state, c->ring, a);
   memset(c->host_dur, 0, sizeof(c->host_dur));
   memset(c->host_calls, 0, sizeof(c->host_calls));
   if (cudaPeekAtLastError() != cudaSuccess)
@@ -2495,8 +2634,8 @@ static int refresh_mirror(tml_ctx* c) {
   DeviceGuard dg(c);
   std::lock_guard<std::mutex> g(c->mirror_mu);
   if (!c->drain_stream) CK(cudaStreamCreateWithFlags(&c->drain_stream, cudaStreamNonBlocking));
-  k_mirror<<<1, 1024, 0, c->drain_stream>>>(c->d_state, c->d_ring, c->ring_slots, c->d_mirror, c->mirror_slots,
-                                            c->d_page, c->mirror_copied);
+  k_mirror<<<1, 1024, 0, c->drain_stream>>>(c->d_state, c->ring, c->d_mirror, c->mirror_slots, c->d_page,
+                                            c->mirror_copied);
   CK(cudaPeekAtLastError());
   CK(cudaStreamSynchronize(c->drain_stream));
   c->mirror_copied = c->h_page->mirror_head;
@@ -2586,11 +2725,84 @@ __global__ void k_set_heads(DevState* st, u64 head, u64 proc_head, int which) {
   if (which == 0) st->head = head; else st->proc_head = proc_head;
 }
 
+}  // extern "C"
+
+// Public records -> the ring's halves and memory bytes: m records from `src` (device staging) into
+// the slots from pos0 on, ring wrap included (pos0 < slots, m <= slots).  One thread per 8-B word.
+__global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, u64 pos0) {
+  for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < m * 16; k += (u64)gridDim.x * blockDim.x) {
+    u64 slot = pos0 + (k >> 4);
+    if (slot >= ring.slots) slot -= ring.slots;
+    const int w = (int)(k & 15), d = ring_word(w);
+    const u64 v = src[k];
+    if (d < 8) reinterpret_cast<u64*>(&ring.hot[slot])[d] = v;
+    else reinterpret_cast<u64*>(&ring.cold[slot])[d - 8] = v;
+    if (w == RING_FLAGS_WORD) ring.mem[slot] = ((u32)(v >> 32) & TML_REC_HAS_MEM) ? 1 : 0;
+  }
+}
+
+// The ring's slots from first_k on (n of them) -> public records at `out` (device).
+__global__ void k_ring_join(StepRing ring, u64 first_k, u64 n, u64* __restrict__ out) {
+  for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < n * 16; k += (u64)gridDim.x * blockDim.x)
+    out[k] = ring_word_at(ring, (first_k + (k >> 4)) % ring.slots, (int)(k & 15));
+}
+
+// records per staging chunk of tml_ring_load (32 MB)
+#define RING_LOAD_CHUNK (1u << 18)
+
+extern "C" {
+
+uint64_t tml_ring_load_chunk_(void) { return RING_LOAD_CHUNK; }
+
+int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stream) {
+  if (!c || (!out && n) || first + n > c->commits || c->commits - first > c->ring.slots)
+    return set_err(TML_ERR_ARG, "tml_ring_read_: records outside the retained ring");
+  if (n == 0) return TML_OK;
+  DeviceGuard dg(c);
+  k_ring_join<<<grid_for(c, n * 16, 256), 256, 0, (cudaStream_t)stream>>>(c->ring, first, n, (u64*)out);
+  CK(cudaPeekAtLastError());
+  return TML_OK;
+}
+
+// The records arrive in the public AoS layout: each bounded chunk is copied into device staging on
+// the context's load stream while the previous chunk is split into the ring on the caller's stream.
 int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* stream) {
   if (!c || (!host && n)) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
-  int rc = load_span(c->d_ring, c->ring_slots, sizeof(tml_step_record), c->commits, host, n, s);
-  if (rc != TML_OK) return rc;
+  DeviceGuard dg(c);
+  {  // if n > slots only the last `slots` survive
+    const u32 slots = c->ring.slots;
+    const u64 keep = n > slots ? (u64)slots : n;
+    const char* src = (const char*)host + (size_t)(n - keep) * sizeof(tml_step_record);
+    if (keep && !c->d_load_stage) {
+      CK(cudaMalloc(&c->d_load_stage, 2 * (size_t)RING_LOAD_CHUNK * sizeof(tml_step_record)));
+      CK(cudaStreamCreateWithFlags(&c->load_stream, cudaStreamNonBlocking));
+      CK(cudaEventCreateWithFlags(&c->load_start, cudaEventDisableTiming));
+      for (int b = 0; b < 2; ++b) {
+        CK(cudaEventCreateWithFlags(&c->load_copied[b], cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&c->load_free[b], cudaEventDisableTiming));
+      }
+    }
+    if (keep) {  // the copies follow what the caller's stream holds (it may still be writing `host`)
+      CK(cudaEventRecord(c->load_start, s));
+      CK(cudaStreamWaitEvent(c->load_stream, c->load_start, 0));
+    }
+    const u64 start = c->commits + (n - keep);
+    for (u64 off = 0, k = 0; off < keep; off += RING_LOAD_CHUNK, ++k) {
+      const int b = (int)(k & 1);
+      const u64 m = keep - off < RING_LOAD_CHUNK ? keep - off : RING_LOAD_CHUNK;
+      char* stage = (char*)c->d_load_stage + (size_t)b * RING_LOAD_CHUNK * sizeof(tml_step_record);
+      CK(cudaStreamWaitEvent(c->load_stream, c->load_free[b], 0));  // its last split has read it
+      CK(cudaMemcpyAsync(stage, src + (size_t)off * sizeof(tml_step_record), (size_t)m * sizeof(tml_step_record),
+                         cudaMemcpyHostToDevice, c->load_stream));
+      CK(cudaEventRecord(c->load_copied[b], c->load_stream));
+      CK(cudaStreamWaitEvent(s, c->load_copied[b], 0));
+      k_ring_split<<<grid_for(c, m * 16, 256), 256, 0, s>>>(c->ring, (const u64*)stage, m,
+                                                             (start + off) % c->ring.slots);
+      CK(cudaPeekAtLastError());
+      CK(cudaEventRecord(c->load_free[b], s));
+    }
+  }
   c->commits += n;
   k_set_heads<<<1, 1, 0, s>>>(c->d_state, c->commits, 0, 0);
   CK(cudaPeekAtLastError());
@@ -2825,7 +3037,7 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
     wr_attr = true;
   }
   int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
-  if (grid > c->n_sms * 2) grid = c->n_sms * 2;  // 2 resident CTAs per SM (83 KB smem each)
+  if (grid > c->n_sms * 2) grid = c->n_sms * 2;  // 2 resident CTAs per SM (90 KB smem each)
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   // K3e (reference-order sums) needs approximate 256-row chunk sums for its plan: K3a has every row
   // in registers anyway and adds them up on the way (tml_exact_sum.cuh: X1 without a pass of its own)
@@ -2844,7 +3056,7 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
     CK(cudaMemsetAsync(d_csum, 0, (size_t)nchunks * 8 * sizeof(double), s));
   }
   CK(cudaEventRecord(c->ev0, s));
-  k_window_rows<<<grid, WR_THREADS, WR_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, c->win_tstart,
+  k_window_rows<<<grid, WR_THREADS, WR_SMEM_BYTES, s>>>(c->ring, first_k, n, c->win_tstart,
                                             c->d_rows, c->d_steps, c->d_flags, &c->d_final->win.acc,
                                             c->d_partials, d_csum, (u64)(n - 1 + wsrc.pad));
   CK(cudaPeekAtLastError());
@@ -2923,7 +3135,7 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, u64 ld, bool 
   if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
   CK(cudaEventRecord(c->ev0, s));
   auto* kern = paired ? k_window_fused<true> : k_window_fused<false>;
-  kern<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->d_ring, c->ring_slots, first_k, n, t_start, series, ld,
+  kern<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->ring, first_k, n, t_start, series, ld,
                                                &c->d_final->chain_acc, c->d_partials);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));

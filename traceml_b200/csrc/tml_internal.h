@@ -36,6 +36,13 @@ int tml_summary_run_(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args
 // ordered behind what `stream` holds at the call: SummaryEngine.build runs K6s beside the window pass.
 int tml_sys_reduce_beside_(tml_ctx* c, uint32_t max_rows, void* stream);
 
+// The device keeps the step ring as hot and cold halves plus a memory byte per slot.  read: records
+// [first, first + n) of the retained ring rebuilt in the public 128-B layout into `out` (device),
+// on `stream`.  load_chunk: records per staging chunk of tml_ring_load.  (Tests check the layout
+// round trip with them.)
+int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stream);
+uint64_t tml_ring_load_chunk_(void);
+
 #ifdef __cplusplus
 }
 #endif

@@ -200,7 +200,8 @@ uint64_t tml_proc_count(tml_ctx* ctx);
 /* Bulk append of already-formed records from HOST memory (replay, resume,
  * or a rank that spooled to disk), asynchronous on `stream`: the records go
  * through bounded device staging chunks and are split into the ring's layout;
- * keep host_records alive until `stream` is synchronised.  If n > ring_slots
+ * keep host_records alive until `stream` is synchronised.  The records must be
+ * in place at the call: their step ids are read then.  If n > ring_slots
  * only the last ring_slots records are kept. */
 int tml_ring_load(tml_ctx* ctx, const tml_step_record* host_records, uint64_t n,
                   void* stream);

@@ -9,8 +9,8 @@ whether the ``--dump-outputs`` files of the first round are byte-identical betwe
 ``profiles/single_rank_build.py``'s pass-vs-copy-ceiling figures of each tree (one run each, after
 the rounds) and the card's name, power limit and max SM clock (read-only ``nvidia-smi`` query).
 
-Both trees must already be built (``__graft_entry__.build()``).  Used to compare the step ring's
-hot/cold layout with the single 128-B record layout of the commit before it.
+Both trees must already be built (``__graft_entry__.build()``).  Tree A is usually the parent commit
+and tree B the change under test: any two trees whose bench and profile take these arguments.
 """
 from __future__ import annotations
 

@@ -317,6 +317,8 @@ SIGNATURES = {
     # private: the step ring's records rebuilt from its device layout; tml_ring_load's staging chunk
     "tml_ring_read_": (C.c_int, [vp, u64, u64, vp, vp]),
     "tml_ring_load_chunk_": (u64, []),
+    # private: the dense-window certificate the ring's writers keep, for the last `window` rows
+    "tml_ring_certified_": (C.c_int, [vp, u32]),
 }
 
 _LIB: Optional[C.CDLL] = None

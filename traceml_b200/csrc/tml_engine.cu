@@ -150,7 +150,35 @@ struct DevState {
   u64 layer_begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // deep profile: its own begin slots (hundreds of layer
                                                    // regions open and close while ONE phase region stays
                                                    // open), same two banks as begin_ts
+  // Dense-window certificate (window_certified): each mark is one past the newest commit number that
+  // breaks its condition, 0 = none.  Raised with atomicMax only, by k_commit and k_ring_split.
+  u64 gap_mark;       // step id != the previous commit's step id + 1
+  u64 nomem_mark;     // flags without TML_REC_HAS_MEM
+  u64 unusable_mark;  // dl, fwd, bwd, opt and wall all 0 ns
 };
+
+// Is the window over the retained commits [first_k, first_k + n), time window from row t_start on,
+// dense in the sense of fused_result?  fused_result accepts exactly the windows where
+//   (a) step[c] == step[c-1] + 1 for every c in (first_k, first_k + n),
+//   (b) every retained record has TML_REC_HAS_MEM,
+//   (c) every record from first_k + t_start on is usable (a summarised phase > 0 ns):
+// dense[1] with violations == 0 needs all n rows to be memory candidates -- each has memory (b) and
+// differs from its successor's step id -- over n consecutive ids between lo and hi, so the
+// non-decreasing ids rise by exactly 1 per row (a); dense[0] with ncand[0] == n_win needs every
+// window row usable (c).  Conversely under (a)-(c) every row is a candidate of both kinds with
+// consecutive ids, hi[0] == hi[1] is the newest id, and there are no violations or duplicates.
+// A decreasing or repeated id breaks (a).  A break at first_k itself is allowed (its predecessor is
+// no longer retained), hence gap_mark <= first_k + 1.  Marks only grow and first_k only grows, so a
+// verdict can be lost to later commits but never gained.  The marks are read by the pass that
+// reads the ring, so they cover the same commits as its ring reads: the build must be ordered
+// after the commits it summarises, as for the records themselves.
+__host__ __device__ __forceinline__ bool step_follows(u64 prev, u64 step) {
+  return prev != ~0ull && step == prev + 1;
+}
+__host__ __device__ __forceinline__ bool window_certified(u64 gap_mark, u64 nomem_mark, u64 unusable_mark,
+                                                          u64 first_k, u64 t_start) {
+  return gap_mark <= first_k + 1 && nomem_mark <= first_k && unusable_mark <= first_k + t_start;
+}
 
 // host-mapped page: written by kernels, read by the sampler thread with no CUDA call
 struct HostPage {
@@ -169,6 +197,8 @@ struct CommitArgs {
   u64 peak_alloc;  // c10 allocator peaks of the step (host state: they travel as launch arguments)
   u64 peak_resv;
   u64 seq;         // commit number = ring position (the host counts them)
+  u32 gap;         // the host's verdicts for the certificate: step != the previous step id + 1,
+  u32 nomem;       // no TML_REC_HAS_MEM (k_commit decides "unusable" itself)
 };
 
 struct WinAcc {  // integer side results of k_window_rows (atomics; order-independent)
@@ -369,6 +399,10 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, Com
     }
     __syncwarp();
     if (lane == 0) {
+      // the certificate's marks: rare, and not waited for (nothing reads them back here)
+      if (a.gap) atomicMax(&st->gap_mark, seq + 1);
+      if (a.nomem) atomicMax(&st->nomem_mark, seq + 1);
+      if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
       __threadfence();  // the record is visible to every later reader of `head` on this GPU
       st->live.steps_committed = seq + 1;
       st->head = seq + 1;
@@ -594,9 +628,9 @@ __device__ __forceinline__ bool tile_linear(const StepRing& ring, u64 slot0, u64
 
 // one warp fetches its 32-record tile into one stage: 4 x cp.async per lane for the hot halves, each
 // instruction = 512 B contiguous, stored XOR-swizzled (16-B chunk q of record r at r*4 + (q ^ (r>>1 & 3)));
-// the memory bytes; with H2D the h2d word of each record (one 32-B sector of its cold half).
+// with MEM the memory bytes; with H2D the h2d word of each record (one 32-B sector of its cold half).
 // slot0 = ring slot of the tile's first record (maintained incrementally by the caller).
-template <bool H2D>
+template <bool H2D, bool MEM = true>
 __device__ __forceinline__ void ring_issue_tile(uint4* stage, const StepRing& ring, u64 slot0, u64 n, u64 base,
                                                 int lane) {
   const uint4* __restrict__ hot4 = reinterpret_cast<const uint4*>(ring.hot);
@@ -609,7 +643,7 @@ __device__ __forceinline__ void ring_issue_tile(uint4* stage, const StepRing& ri
       const int idx = c * 32 + lane;
       cp_async16(&stage[(idx & ~3) | ((idx ^ (idx >> 3)) & 3)], src + idx);
     }
-    if (lane < TILE_MEM_U4) cp_async16(&mem[lane], ring.mem + (slot0 & ~15ull) + 16 * lane);
+    if (MEM && lane < TILE_MEM_U4) cp_async16(&mem[lane], ring.mem + (slot0 & ~15ull) + 16 * lane);
     if (H2D) cp_async8(&h2d[lane], &ring.cold[slot0 + lane].h2d);
     return;
   }
@@ -623,10 +657,10 @@ __device__ __forceinline__ void ring_issue_tile(uint4* stage, const StepRing& ri
       cp_async16(&stage[r * 4 + (q ^ ((r >> 1) & 3))], &hot4[slot * 4 + q]);
     }
   }
-  if (base + (u64)lane < n) {
+  if ((MEM || H2D) && base + (u64)lane < n) {
     u64 slot = slot0 + (u64)lane;
     while (slot >= ring.slots) slot -= ring.slots;
-    reinterpret_cast<u8*>(mem)[lane] = ring.mem[slot];  // byte-wise: only a ring wrap or the last tile
+    if (MEM) reinterpret_cast<u8*>(mem)[lane] = ring.mem[slot];  // byte-wise: only a ring wrap or the last tile
     if (H2D) cp_async8(&h2d[lane], &ring.cold[slot].h2d);
   }
 }
@@ -931,11 +965,19 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 
 // 2 CTAs of WR_THREADS per SM need <= 128 registers; left to itself ptxas takes 96 for the plain
 // instance, with the cap it keeps 94 with no spills.
+//
+// A window the ring's writers certified dense (window_certified, read once per CTA) takes a pure
+// stream of hot halves: every row is the first of its step id, has memory and a successor with a
+// new id, and every window row is usable, so the halo loads, memory bytes and neighbour shuffles
+// that decide this in general are not needed.  The tile -> warp -> CTA mapping and each lane's
+// order of additions are those of the general loop, so sums, maxima and counters are bit-identical.
+// Any other window takes the general loop.
 template <bool PAIRED>
 __global__ void __maxnreg__(94) k_window_fused(
     StepRing ring, u64 first_k, u64 n, u64 t_start,
-    double* __restrict__ series, u64 ld, WinAcc* acc, double* partials) {
+    double* __restrict__ series, u64 ld, WinAcc* acc, double* partials, const DevState* st) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
+  __shared__ u32 s_cert;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
 
@@ -948,102 +990,165 @@ __global__ void __maxnreg__(94) k_window_fused(
   const u64 wstride = (u64)gridDim.x * WR_WARPS;
   const u32 ring_slots = ring.slots;
 
-  u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-  u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
-  const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
-  u32 slot_iss = slot_cur;
+  if (tid == 0) s_cert = window_certified(st->gap_mark, st->nomem_mark, st->unusable_mark, first_k, t_start);
+  __syncthreads();
+  if (s_cert) {
+    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
+    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
+    u32 slot_iss = (u32)((first_k + wt * 32) % ring_slots);
 #pragma unroll
-  for (int s = 0; s < WR_STAGES - 1; ++s) {
-    const u64 t = wt + (u64)s * wstride;
-    if (t < nwt) ring_issue_tile<false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
-    cp_async_commit();
-    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-  }
-
-  for (int it = 0; wt < nwt; wt += wstride, ++it) {
-    uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
-    const u64 base = wt * 32;
-    const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
-    if (ahead < nwt)
-      ring_issue_tile<false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
-    cp_async_commit();
-    slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-    const u32 slot_tile = slot_cur;
-    u64 halo_step = 0;
-    u32 halo_mem = 0;
-    if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
-    if (lane == 31 && base + 32 < n) {
-      u64 hs = (u64)slot_cur + 32;
-      while (hs >= ring_slots) hs -= ring_slots;
-      halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
+    for (int s = 0; s < WR_STAGES - 1; ++s) {
+      const u64 t = wt + (u64)s * wstride;
+      if (t < nwt) ring_issue_tile<false, false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
     }
-    slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
-    cp_async_wait<WR_STAGES - 1>();
-    __syncwarp();
-
-    const u64 i = base + (u64)lane;
-    const bool live = i < n;
-    const int sw = (lane >> 1) & 3;
-    const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
-    const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
-    const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
-    const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-    u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
-    u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
-    u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
-    if (lane == 0) prev_step = halo_step;
-    if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
-
-    if (live) {
-      const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
-      const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
-      const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
-      const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
-      const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
-      const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
-      const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
-      const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
-      const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
-      const bool has_mem = rmem != 0u;
-      const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
-      const bool in_time = i >= t_start;
-      const bool has_prev = i > 0, has_next = (i + 1) < n;
-      const bool first_in_win = (i == t_start) || !has_prev || (prev_step != step);
-      const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
-      const bool cand_t = usable && in_time && first_in_win;
-      const bool cand_m = has_mem && last_m;
-      a_latest = step > a_latest ? step : a_latest;
-      a_viol += (has_prev && step < prev_step) ? 1u : 0u;
-      a_dups += (has_prev && step == prev_step) ? 1u : 0u;
-      a_nr0 += in_time ? 1u : 0u;
-      a_nr1 += has_mem ? 1u : 0u;
-      if (cand_t) { a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0; ++a_nc0; }
-      if (cand_m) { a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1; ++a_nc1; }
-      a_both += (cand_t && cand_m) ? 1u : 0u;
-      const double compute = (fwd + bwd) + opt;
-      const double traced = fmax(wall, compute);      // model.py:246
-      if (usable && in_time) {
-        sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
-        sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
-        ++a_tc;
+    for (int it = 0; wt < nwt; wt += wstride, ++it) {
+      const uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
+      const u64 base = wt * 32;
+      const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
+      if (ahead < nwt)
+        ring_issue_tile<false, false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n,
+                                      ahead * 32, lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+      cp_async_wait<WR_STAGES - 1>();
+      __syncwarp();
+      const u64 i = base + (u64)lane;
+      if (i < n) {
+        const int sw = (lane >> 1) & 3;
+        const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
+        const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
+        const u64 step = (u64)c0.x | ((u64)c0.y << 32);
+        a_latest = step > a_latest ? step : a_latest;
+        a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1;
+        ++a_nr1;  // a memory candidate
+        if (i >= t_start) {  // a time candidate, usable
+          const double dl = ns_to_ms((u64)c0.z | ((u64)c0.w << 32)), fwd = ns_to_ms((u64)c1.x | ((u64)c1.y << 32));
+          const double bwd = ns_to_ms((u64)c1.z | ((u64)c1.w << 32)), opt = ns_to_ms((u64)c2.x | ((u64)c2.y << 32));
+          const double wall = ns_to_ms((u64)c2.z | ((u64)c2.w << 32));
+          const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
+          const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
+          a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0;
+          ++a_nr0;
+          const double compute = (fwd + bwd) + opt;
+          const double traced = fmax(wall, compute);
+          sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
+          sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
+          a_sa += pa; a_sr += pr;
+          mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
+          const double wait = fmax(0.0, traced - compute);
+          double* S = series + (i - t_start);
+          auto put = [&](int m, double v) {
+            S[(u64)(2 * m) * ld] = v;
+            if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
+          };
+          put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
+          put(4, traced); put(5, wait); put(6, (double)pa); put(7, (double)pr);
+        }
       }
-      if (in_time) {
-        a_sa += pa; a_sr += pr;
-        mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
-        // one rank: median == worst == the value (adapters.py:92-139 with a single column)
-        const u64 j = i - t_start;
-        const double wait = fmax(0.0, traced - compute);  // model.py:247
-        const double va = (double)pa, vr = (double)pr;
-        double* S = series + j;
-        auto put = [&](int m, double v) {  // metric m: median row 2m, worst row 2m+1
-          S[(u64)(2 * m) * ld] = v;
-          if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
-        };
-        put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
-        put(4, traced); put(5, wait); put(6, va); put(7, vr);
-      }
+      __syncwarp();  // `cur` is free again
     }
-    __syncwarp();  // `cur` is free again
+    a_nc0 = a_tc = a_both = a_nr0;
+    a_nc1 = a_nr1;
+  } else {
+    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
+    u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
+    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
+    u32 slot_iss = slot_cur;
+#pragma unroll
+    for (int s = 0; s < WR_STAGES - 1; ++s) {
+      const u64 t = wt + (u64)s * wstride;
+      if (t < nwt) ring_issue_tile<false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+    }
+
+    for (int it = 0; wt < nwt; wt += wstride, ++it) {
+      uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
+      const u64 base = wt * 32;
+      const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
+      if (ahead < nwt)
+        ring_issue_tile<false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+      const u32 slot_tile = slot_cur;
+      u64 halo_step = 0;
+      u32 halo_mem = 0;
+      if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
+      if (lane == 31 && base + 32 < n) {
+        u64 hs = (u64)slot_cur + 32;
+        while (hs >= ring_slots) hs -= ring_slots;
+        halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
+      }
+      slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
+      cp_async_wait<WR_STAGES - 1>();
+      __syncwarp();
+
+      const u64 i = base + (u64)lane;
+      const bool live = i < n;
+      const int sw = (lane >> 1) & 3;
+      const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
+      const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
+      const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
+      const u64 step = (u64)c0.x | ((u64)c0.y << 32);
+      u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
+      u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
+      u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
+      if (lane == 0) prev_step = halo_step;
+      if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
+
+      if (live) {
+        const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
+        const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
+        const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
+        const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
+        const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
+        const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
+        const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
+        const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
+        const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
+        const bool has_mem = rmem != 0u;
+        const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
+        const bool in_time = i >= t_start;
+        const bool has_prev = i > 0, has_next = (i + 1) < n;
+        const bool first_in_win = (i == t_start) || !has_prev || (prev_step != step);
+        const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
+        const bool cand_t = usable && in_time && first_in_win;
+        const bool cand_m = has_mem && last_m;
+        a_latest = step > a_latest ? step : a_latest;
+        a_viol += (has_prev && step < prev_step) ? 1u : 0u;
+        a_dups += (has_prev && step == prev_step) ? 1u : 0u;
+        a_nr0 += in_time ? 1u : 0u;
+        a_nr1 += has_mem ? 1u : 0u;
+        if (cand_t) { a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0; ++a_nc0; }
+        if (cand_m) { a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1; ++a_nc1; }
+        a_both += (cand_t && cand_m) ? 1u : 0u;
+        const double compute = (fwd + bwd) + opt;
+        const double traced = fmax(wall, compute);      // model.py:246
+        if (usable && in_time) {
+          sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
+          sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
+          ++a_tc;
+        }
+        if (in_time) {
+          a_sa += pa; a_sr += pr;
+          mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
+          // one rank: median == worst == the value (adapters.py:92-139 with a single column)
+          const u64 j = i - t_start;
+          const double wait = fmax(0.0, traced - compute);  // model.py:247
+          const double va = (double)pa, vr = (double)pr;
+          double* S = series + j;
+          auto put = [&](int m, double v) {  // metric m: median row 2m, worst row 2m+1
+            S[(u64)(2 * m) * ld] = v;
+            if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
+          };
+          put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
+          put(4, traced); put(5, wait); put(6, va); put(7, vr);
+        }
+      }
+      __syncwarp();  // `cur` is free again
+    }
   }
   cp_async_wait<0>();
   {
@@ -2013,6 +2118,7 @@ struct tml_ctx {
   unsigned long long* d_ticket = nullptr;    // K4's tile counter
   cudaEvent_t ev_proc = nullptr;             // the process aggregates have reached the staging slot
   u64 commits = 0;
+  u64 last_step = 0;  // step id of commit number commits - 1 (the certificate's gap test)
   u64 launches = 0;  // kernels this context has launched (bench: gpu_launches)
   u32 next_slot = 0;
   // graph-captured regions (tml_graph_*): capture-time host state, behind graph_mu
@@ -2607,12 +2713,15 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
   a.peak_alloc = peak_alloc;
   a.peak_resv = peak_resv;
   a.seq = c->commits;
+  a.gap = c->commits > 0 && !step_follows(c->last_step, step);
+  a.nomem = (flags & TML_REC_HAS_MEM) == 0u;
   k_commit<<<1, 192, 0, s>>>(c->d_state, c->ring, a);
   memset(c->host_dur, 0, sizeof(c->host_dur));
   memset(c->host_calls, 0, sizeof(c->host_calls));
   if (cudaPeekAtLastError() != cudaSuccess)
     return set_err(TML_ERR_CUDA, "commit launch: %s", cudaGetErrorString(cudaGetLastError()));
   c->commits += 1;
+  c->last_step = step;
   c->launches += 1;
   c->win_ready = false;
   return TML_OK;
@@ -2729,15 +2838,34 @@ __global__ void k_set_heads(DevState* st, u64 head, u64 proc_head, int which) {
 
 // Public records -> the ring's halves and memory bytes: m records from `src` (device staging) into
 // the slots from pos0 on, ring wrap included (pos0 < slots, m <= slots).  One thread per 8-B word.
-__global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, u64 pos0) {
+// The thread of a record's step word also raises the certificate's marks for it (commit number
+// seq0 + its index); `pred`: the step id before the chunk's first record, has_pred = 0 if none.
+__global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, u64 pos0, DevState* st, u64 seq0,
+                             u64 pred, u32 has_pred) {
+  u32 gap = 0, nomem = 0, unusable = 0;  // 1 + the chunk index of this thread's newest break, 0 = none
   for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < m * 16; k += (u64)gridDim.x * blockDim.x) {
-    u64 slot = pos0 + (k >> 4);
+    const u64 r = k >> 4;
+    u64 slot = pos0 + r;
     if (slot >= ring.slots) slot -= ring.slots;
     const int w = (int)(k & 15), d = ring_word(w);
     const u64 v = src[k];
     if (d < 8) reinterpret_cast<u64*>(&ring.hot[slot])[d] = v;
     else reinterpret_cast<u64*>(&ring.cold[slot])[d - 8] = v;
     if (w == RING_FLAGS_WORD) ring.mem[slot] = ((u32)(v >> 32) & TML_REC_HAS_MEM) ? 1 : 0;
+    if (w == 0) {  // public words: 1 dl, 3..6 fwd bwd opt wall, RING_FLAGS_WORD flags (high half)
+      const bool has_prev = r > 0 || has_pred != 0u;
+      if (has_prev && !step_follows(r > 0 ? src[k - 16] : pred, v)) gap = (u32)r + 1u;
+      if (!(((u32)(src[k + RING_FLAGS_WORD] >> 32)) & TML_REC_HAS_MEM)) nomem = (u32)r + 1u;
+      if ((src[k + 1] | src[k + 3] | src[k + 4] | src[k + 5] | src[k + 6]) == 0ull) unusable = (u32)r + 1u;
+    }
+  }
+  gap = __reduce_max_sync(0xffffffffu, gap);
+  nomem = __reduce_max_sync(0xffffffffu, nomem);
+  unusable = __reduce_max_sync(0xffffffffu, unusable);
+  if ((threadIdx.x & 31) == 0) {
+    if (gap) atomicMax(&st->gap_mark, seq0 + gap);
+    if (nomem) atomicMax(&st->nomem_mark, seq0 + nomem);
+    if (unusable) atomicMax(&st->unusable_mark, seq0 + unusable);
   }
 }
 
@@ -2764,8 +2892,21 @@ int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stre
   return TML_OK;
 }
 
+int tml_ring_certified_(tml_ctx* c, uint32_t window) {
+  if (!c || window == 0) return TML_ERR_ARG;
+  DeviceGuard dg(c);
+  u64 marks[3];
+  static_assert(offsetof(DevState, nomem_mark) == offsetof(DevState, gap_mark) + 8 &&
+                offsetof(DevState, unusable_mark) == offsetof(DevState, gap_mark) + 16, "marks are adjacent");
+  CK(cudaDeviceSynchronize());
+  CK(cudaMemcpy(marks, &c->d_state->gap_mark, sizeof(marks), cudaMemcpyDeviceToHost));
+  const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
+  return window_certified(marks[0], marks[1], marks[2], c->commits - n, n > window ? n - window : 0) ? 1 : 0;
+}
+
 // The records arrive in the public AoS layout: each bounded chunk is copied into device staging on
 // the context's load stream while the previous chunk is split into the ring on the caller's stream.
+// The step ids before each chunk are read from `host` at the call (the certificate's gap test).
 int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* stream) {
   if (!c || (!host && n)) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
@@ -2783,12 +2924,16 @@ int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* str
         CK(cudaEventCreateWithFlags(&c->load_free[b], cudaEventDisableTiming));
       }
     }
-    if (keep) {  // the copies follow what the caller's stream holds (it may still be writing `host`)
+    if (keep) {  // the copies follow what the caller's stream holds
       CK(cudaEventRecord(c->load_start, s));
       CK(cudaStreamWaitEvent(c->load_stream, c->load_start, 0));
     }
     const u64 start = c->commits + (n - keep);
+    const tml_step_record* kept = reinterpret_cast<const tml_step_record*>(src);
     for (u64 off = 0, k = 0; off < keep; off += RING_LOAD_CHUNK, ++k) {
+      // the step id before the chunk: the caller's previous record, or the last one committed before
+      const bool has_pred = off > 0 || n > keep || c->commits > 0;
+      const u64 pred = off > 0 || n > keep ? kept[(long long)off - 1].step : c->last_step;
       const int b = (int)(k & 1);
       const u64 m = keep - off < RING_LOAD_CHUNK ? keep - off : RING_LOAD_CHUNK;
       char* stage = (char*)c->d_load_stage + (size_t)b * RING_LOAD_CHUNK * sizeof(tml_step_record);
@@ -2798,11 +2943,13 @@ int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* str
       CK(cudaEventRecord(c->load_copied[b], c->load_stream));
       CK(cudaStreamWaitEvent(s, c->load_copied[b], 0));
       k_ring_split<<<grid_for(c, m * 16, 256), 256, 0, s>>>(c->ring, (const u64*)stage, m,
-                                                             (start + off) % c->ring.slots);
+                                                             (start + off) % c->ring.slots, c->d_state,
+                                                             start + off, pred, has_pred ? 1u : 0u);
       CK(cudaPeekAtLastError());
       CK(cudaEventRecord(c->load_free[b], s));
     }
   }
+  if (n) c->last_step = host[n - 1].step;
   c->commits += n;
   k_set_heads<<<1, 1, 0, s>>>(c->d_state, c->commits, 0, 0);
   CK(cudaPeekAtLastError());
@@ -3136,7 +3283,7 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, u64 ld, bool 
   CK(cudaEventRecord(c->ev0, s));
   auto* kern = paired ? k_window_fused<true> : k_window_fused<false>;
   kern<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->ring, first_k, n, t_start, series, ld,
-                                               &c->d_final->chain_acc, c->d_partials);
+                                               &c->d_final->chain_acc, c->d_partials, c->d_state);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));
   c->launches += 1;

@@ -42,6 +42,9 @@ int tml_sys_reduce_beside_(tml_ctx* c, uint32_t max_rows, void* stream);
 // round trip with them.)
 int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stream);
 uint64_t tml_ring_load_chunk_(void);
+// 1 if the ring's writers certify the retained ring's last `window` rows dense, else 0 (waits for
+// the device; tests compare it with the records)
+int tml_ring_certified_(tml_ctx* c, uint32_t window);
 
 #ifdef __cplusplus
 }

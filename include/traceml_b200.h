@@ -176,6 +176,60 @@ int tml_graph_phase_end(tml_ctx* ctx, uint32_t phase, int slot, void* stream);
  * state.  Takes no context: it stays readable after tml_shutdown. */
 uint64_t tml_graph_refs(void);
 
+/* ------------------------------------------------- GRAPH-CAPTURED STEPS
+ * A step whose boundary is captured into the graph `stream` is capturing, so
+ * every replay commits one step record.  Both follow the rules of
+ * tml_graph_phase_begin / _end: a capturing stream (else TML_ERR_STATE), a
+ * graph slot at the capture's nesting depth, closed LIFO, and the graph holds
+ * the context's device state.
+ *
+ * tml_graph_step_begin captures the step's %globaltimer begin stamp and returns
+ * its graph slot.  tml_graph_step_commit closes the innermost open graph region,
+ * which must be a step (else TML_ERR_STATE), and captures the commit kernel.
+ * Each replay of it writes the record with
+ *   - the commit number (ring slot, epoch) taken from the device's head,
+ *   - step id = the device's last committed id + 1 (the last id itself with
+ *     TML_GRAPH_STEP_FAILED: a step whose body raised keeps the old id),
+ *   - step_time = %globaltimer at the commit - the begin stamp,
+ *   - the phases the graph's regions and tml_graph_phase_host added to the
+ *     accumulator set open on the device,
+ *   - peak_alloc / peak_resv = the bytes last published by
+ *     tml_graph_step_publish; `flags` TML_REC_HAS_MEM marks them real,
+ *   - the dense-window certificate's verdicts, decided on the device.
+ *
+ * The first captured commit puts the context in DEVICE-COMMITTED mode for the
+ * rest of its life.  From then on the device counts commits and step ids:
+ *   - tml_step_commit's `step` only says whether the host step advanced the id
+ *     (non-zero) or not (0, a failed step: it flushes under the last id), and
+ *     its ring position comes from the device's head;
+ *   - host-launched stamps take their epoch from the device's head;
+ *   - tml_layer_commit ignores `step` and takes the device's ring position
+ *     and id;
+ *   - tml_step_count and every reader of the retained ring (tml_win_*,
+ *     tml_ring_*) first read the count back from the device (one 16-B copy):
+ *     call them with the step path quiescent.
+ *
+ * tml_graph_step_publish (host-launched, TML_ERR_CAPTURE on a capturing
+ * stream) stores the allocator's current allocated / reserved bytes for the
+ * captured commits that run after it.  Its first call after the mode is
+ * entered also seeds the device's last step id: the last committed id, or
+ * `base_step` when nothing was committed yet.  Call it once the capture has
+ * ended, before the first replay, and after every host commit.
+ * tml_graph_step_id reads the device's last step id (one 8-B copy;
+ * TML_ERR_STATE outside device-committed mode).  tml_graph_phase_host is
+ * tml_phase_host for device-committed mode: a 1-warp kernel on `stream` adds
+ * the duration to the step open on the device when it runs (outside the mode,
+ * or on a capturing stream, it is tml_phase_host).  tml_graph_layer_commit
+ * captures the deep profile's step close (tml_layer_init first, else
+ * TML_ERR_STATE): every replay snapshots the layers under the device's id. */
+#define TML_GRAPH_STEP_FAILED 0x80000000u
+int tml_graph_step_begin(tml_ctx* ctx, void* stream);
+int tml_graph_step_commit(tml_ctx* ctx, uint32_t flags, void* stream);
+int tml_graph_step_publish(tml_ctx* ctx, uint64_t base_step, uint64_t alloc, uint64_t resv, void* stream);
+int tml_graph_step_id(tml_ctx* ctx, uint64_t* step);
+int tml_graph_phase_host(tml_ctx* ctx, uint32_t phase, uint64_t dur_ns, void* stream);
+int tml_graph_layer_commit(tml_ctx* ctx, void* stream);
+
 /* ------------------------------------------------------- SAMPLER-SIDE (host)
  * Called from the sampler thread; never touches the training stream. */
 
@@ -193,7 +247,9 @@ int tml_live(tml_ctx* ctx, tml_live_stats* out);
 int tml_proc_commit(tml_ctx* ctx, const tml_proc_record* sample, void* stream);
 int tml_proc_drain(tml_ctx* ctx, tml_proc_record* out, uint32_t max_records,
                    uint32_t* n_out, uint64_t* n_dropped);
-uint64_t tml_step_count(tml_ctx* ctx); /* records committed so far */
+/* records committed so far (in device-committed mode it reads the count from
+ * the device: one 16-B copy, with the step path quiescent) */
+uint64_t tml_step_count(tml_ctx* ctx);
 uint64_t tml_launch_count(tml_ctx* ctx); /* kernels launched by this context */
 uint64_t tml_proc_count(tml_ctx* ctx);
 

@@ -21,6 +21,7 @@ TML_MAX_RANKS = 64
 TML_SERIES_PER_STEP = 16
 TML_OK = 0
 TML_ERR_CAPTURE = -7
+TML_GRAPH_STEP_FAILED = 0x80000000  # tml_graph_step_commit: the step's body raised, keep the old id
 TML_ERR_NONMONOTONIC = -5
 KIND_TIME, KIND_MEM = 0, 1
 MASK_TIME, MASK_MEM = 1, 2
@@ -248,6 +249,12 @@ SIGNATURES = {
     "tml_graph_layer_begin": (C.c_int, [vp, vp]),
     "tml_graph_layer_end": (C.c_int, [vp, u32, u32, C.c_int, u64, vp]),
     "tml_graph_refs": (u64, []),
+    "tml_graph_step_begin": (C.c_int, [vp, vp]),
+    "tml_graph_step_commit": (C.c_int, [vp, u32, vp]),
+    "tml_graph_step_publish": (C.c_int, [vp, u64, u64, u64, vp]),
+    "tml_graph_step_id": (C.c_int, [vp, C.POINTER(u64)]),
+    "tml_graph_phase_host": (C.c_int, [vp, u32, u64, vp]),
+    "tml_graph_layer_commit": (C.c_int, [vp, vp]),
     "tml_drain": (C.c_int, [vp, vp, u32, C.POINTER(u32), C.POINTER(u64)]),
     "tml_live": (C.c_int, [vp, C.POINTER(LiveStats)]),
     "tml_proc_commit": (C.c_int, [vp, C.POINTER(ProcRecord), vp]),

@@ -155,6 +155,11 @@ struct DevState {
   u64 gap_mark;       // step id != the previous commit's step id + 1
   u64 nomem_mark;     // flags without TML_REC_HAS_MEM
   u64 unusable_mark;  // dl, fwd, bwd, opt and wall all 0 ns
+  // Device-committed mode (a step commit was captured into a CUDA graph): the commit number and the
+  // step id live here, next to each other so that one copy refreshes the host's view of both
+  u64 dc_head;    // == head, written by k_commit_dev and k_set_dc
+  u64 dc_step;    // step id of commit dc_head - 1 (before any commit: the base the host seeded)
+  u64 dc_mem[2];  // allocated / reserved bytes the host last published (captured commits record them)
 };
 
 // Is the window over the retained commits [first_k, first_k + n), time window from row t_start on,
@@ -199,6 +204,20 @@ struct CommitArgs {
   u64 seq;         // commit number = ring position (the host counts them)
   u32 gap;         // the host's verdicts for the certificate: step != the previous step id + 1,
   u32 nomem;       // no TML_REC_HAS_MEM (k_commit decides "unusable" itself)
+};
+
+// k_commit_dev: what is left once the commit number, the epoch, the step id and the certificate's
+// verdicts come from the device.  A captured commit's arguments are frozen at capture.
+#define TML_NO_WALL_SLOT 0xffffffffu
+struct DevCommitArgs {
+  double host_ts;  // host commits (captured ones stamp %globaltimer)
+  u64 host_dur[TML_MAX_PHASES];
+  u32 host_calls[TML_MAX_PHASES];
+  u64 peak_alloc;  // host commits (captured ones record the published dc_mem)
+  u64 peak_resv;
+  u32 flags;
+  u32 advance;     // step id = the last one + advance (0: the step's body raised)
+  u32 wall_slot;   // captured: begin_ts slot of the step's wall; TML_NO_WALL_SLOT: a host commit
 };
 
 struct WinAcc {  // integer side results of k_window_rows (atomics; order-independent)
@@ -282,6 +301,70 @@ __global__ void __maxnreg__(24) k_stamp_end(DevState* st, u32 slot, u32 phase, u
 // ------------------------------------------------------------------ K2: commit
 // 6 warps: warp p owns phase p's running statistics; warp 0 also assembles the
 // record in shared memory and writes its two 64-B ring halves (8 x 16-B stores) and the memory byte.
+
+// k_commit_dev's running statistics and ring store: k_commit's own code, which stays inline in
+// k_commit because calling these changes its SASS.
+// Running statistics of phase `warp` after a step of `dur` ns / `calls` calls: count / sum / worst
+// exactly, median from the log histogram by a warp-shuffle inclusive scan of per-lane bin counts.
+// c[8]: this lane's 8 bins of h, already fetched; run_sum / run_max: lane 0's.
+__device__ __forceinline__ void commit_stats(DevState* st, int warp, int lane, u32* h, u32 (&c)[8], u64 dur,
+                                             u32 calls, u64 run_sum, u64 run_max) {
+  if (calls > 0u) {
+    const u32 bin = hist_bin(dur);
+    if ((int)(bin >> 3) == lane) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) c[k] += ((bin & 7u) == (u32)k) ? 1u : 0u;
+      h[bin] = c[0] * ((bin & 7u) == 0u) + c[1] * ((bin & 7u) == 1u) + c[2] * ((bin & 7u) == 2u) +
+               c[3] * ((bin & 7u) == 3u) + c[4] * ((bin & 7u) == 4u) + c[5] * ((bin & 7u) == 5u) +
+               c[6] * ((bin & 7u) == 6u) + c[7] * ((bin & 7u) == 7u);
+    }
+    u32 local = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) local += c[k];
+    u32 incl = local;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      u32 n = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += n;
+    }
+    u32 total = __shfl_sync(0xffffffffu, incl, 31);
+    u32 target = (total + 1u) >> 1;
+    u32 excl = incl - local;
+    unsigned hit = __ballot_sync(0xffffffffu, (excl < target) && (target <= incl));
+    int src = __ffs(hit) - 1;
+    const u64 sum = __shfl_sync(0xffffffffu, run_sum, 0) + dur;
+    u64 mx = __shfl_sync(0xffffffffu, run_max, 0);
+    mx = dur > mx ? dur : mx;
+    if (lane == src) {
+      u32 run = excl;
+      u32 mbin = lane * 8;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        run += c[k];
+        if (run >= target) { mbin = lane * 8 + k; break; }
+      }
+      st->live_sum[warp] = sum;
+      st->live_max[warp] = mx;
+      tml_live_phase* lp = &st->live.phase[warp];
+      lp->count = total;
+      lp->sum_ns = sum;
+      lp->worst_ns = mx;
+      lp->median_ns = hist_bin_center(mbin);
+    }
+  }
+}
+
+// Warp 0: the record staged in rec[16] (hot half, then cold half) -> ring slot `slot` as 8 x 16-B
+// stores, plus its memory byte.
+__device__ __forceinline__ void commit_store(const StepRing& ring, u64 slot, const u64* rec, int lane, u32 flags) {
+  if (lane < 8) {
+    uint4 v = reinterpret_cast<const uint4*>(rec)[lane];
+    uint4* half = lane < 4 ? reinterpret_cast<uint4*>(&ring.hot[slot]) : reinterpret_cast<uint4*>(&ring.cold[slot]);
+    half[lane & 3] = v;
+  } else if (lane == 8) {
+    ring.mem[slot] = (flags & TML_REC_HAS_MEM) ? 1 : 0;
+  }
+}
 
 // Nothing in here leaves the GPU: writing the record and the live statistics into host-mapped
 // memory and closing with __threadfence_system would cost the TRAINING stream time every step for
@@ -410,6 +493,125 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, Com
   }
 }
 
+// K2 in device-committed mode: launched by the host, or captured into a CUDA graph and run on every
+// replay.  The commit number (ring slot, epoch) is the head, the step id the device's last id +
+// a.advance, and the certificate's gap / no-memory verdicts are decided here with the host path's
+// definitions.  The epoch is only known once the head has arrived, so lanes 0..7 fetch phase `warp`'s
+// word of all 8 accumulator sets alongside the head and the histogram: the critical path keeps ONE
+// global round trip, and the epoch's words are picked by shuffle.  A captured commit's wall
+// (phase 5) is %globaltimer minus the begin stamp its tml_graph_step_begin captured.
+__global__ void __launch_bounds__(192) k_commit_dev(DevState* st, StepRing ring, DevCommitArgs a) {
+  __shared__ __align__(16) u64 rec[16];
+  __shared__ u64 s_dur[TML_MAX_PHASES];
+  __shared__ u32 s_calls[TML_MAX_PHASES];
+  __shared__ u32 s_mask;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool captured = a.wall_slot != TML_NO_WALL_SLOT;
+  const u64 t1 = globaltimer_ns();
+
+  u32* h = st->hist[warp];
+  u32 c[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) c[k] = h[lane * 8 + k];
+  u64 e_dur = 0, x = 0;
+  u32 e_calls = 0, e_mask = 0;
+  if (lane < (int)TML_N_EPOCHS) {
+    e_dur = st->acc[lane].dur_ns[warp];
+    e_calls = st->acc[lane].n_calls[warp];
+    if (warp == 0) e_mask = st->acc[lane].gpu_mask;
+  } else if (lane == 8) {
+    x = st->head;
+  } else if (lane == 9) {
+    x = st->live_sum[warp];
+  } else if (lane == 10) {
+    x = st->live_max[warp];
+  } else if (lane == 11) {
+    if (warp == 0) x = st->dc_step;
+    else if (warp == 5 && captured) x = st->begin_ts[a.wall_slot];
+  } else if (lane == 12 && warp == 0) {
+    x = st->dc_mem[0];
+  } else if (lane == 13 && warp == 0) {
+    x = st->dc_mem[1];
+  }
+  const u64 seq = __shfl_sync(0xffffffffu, x, 8);
+  const u32 epoch = (u32)(seq % TML_N_EPOCHS);
+  u64 dur = __shfl_sync(0xffffffffu, e_dur, epoch) + a.host_dur[warp];
+  u32 calls = __shfl_sync(0xffffffffu, e_calls, epoch) + a.host_calls[warp];
+  const u32 mask = __shfl_sync(0xffffffffu, e_mask, epoch);
+  const u64 run_sum = __shfl_sync(0xffffffffu, x, 9), run_max = __shfl_sync(0xffffffffu, x, 10);
+  const u64 x11 = __shfl_sync(0xffffffffu, x, 11);
+  if (warp == 5 && captured) {
+    dur += t1 > x11 ? t1 - x11 : 0ull;
+    calls += 1u;
+  }
+  if (lane == 0) {
+    DevAcc* acc = &st->acc[epoch];
+    s_dur[warp] = dur;
+    s_calls[warp] = calls;
+    acc->dur_ns[warp] = 0;
+    acc->n_calls[warp] = 0;
+    if (warp == 0) {
+      s_mask = mask;
+      acc->gpu_mask = 0;
+      acc->dur_ns[6] = 0; acc->dur_ns[7] = 0; acc->n_calls[6] = 0; acc->n_calls[7] = 0;
+    }
+  }
+  commit_stats(st, warp, lane, h, c, dur, calls, run_sum, run_max);
+  __syncthreads();
+
+  if (warp == 0) {
+    const u64 last = x11;
+    const u64 m_alloc = __shfl_sync(0xffffffffu, x, 12), m_resv = __shfl_sync(0xffffffffu, x, 13);
+    const u64 step = last + a.advance;
+    const u64 slot = seq % ring.slots;
+    if (lane == 0) {
+      rec[0] = step;
+      rec[1] = s_dur[0];
+#pragma unroll
+      for (int p = 2; p < 6; ++p) rec[p] = s_dur[p];
+      rec[6] = captured ? m_alloc : a.peak_alloc;
+      rec[7] = captured ? m_resv : a.peak_resv;
+      rec[8] = s_dur[1];
+      rec[9] = (u64)s_calls[0] | ((u64)s_calls[1] << 32);
+      rec[10] = (u64)s_calls[2] | ((u64)s_calls[3] << 32);
+      rec[11] = (u64)s_calls[4] | ((u64)s_calls[5] << 32);
+      rec[12] = (u64)__double_as_longlong(captured ? (double)t1 * 1.0e-9 : a.host_ts);
+      rec[13] = (u64)s_mask | ((u64)a.flags << 32);
+      rec[14] = seq;
+      rec[15] = 0;
+    }
+    __syncwarp();
+    commit_store(ring, slot, rec, lane, a.flags);
+    __syncwarp();
+    if (lane == 0) {
+      if (seq > 0 && !step_follows(last, step)) atomicMax(&st->gap_mark, seq + 1);
+      if ((a.flags & TML_REC_HAS_MEM) == 0u) atomicMax(&st->nomem_mark, seq + 1);
+      if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
+      st->dc_step = step;
+      st->dc_head = seq + 1;
+      __threadfence();
+      st->live.steps_committed = seq + 1;
+      st->head = seq + 1;
+    }
+  }
+}
+
+// The device words of device-committed mode: the commit count and the last step id (the host's
+// seed, ring loads and resets), and the published allocator bytes unless `mem` is 0.
+__global__ void k_set_dc(DevState* st, u64 head, u64 step, int seed, u64 alloc, u64 resv, int mem) {
+  if (seed) { st->dc_head = head; st->dc_step = step; }
+  if (mem) { st->dc_mem[0] = alloc; st->dc_mem[1] = resv; }
+}
+
+// tml_graph_phase_host: a host-clock duration added to the accumulator set open on the device
+__global__ void k_host_phase(DevState* st, u32 phase, u64 d) {
+  if (threadIdx.x == 0) {
+    DevAcc* a = &st->acc[st->head % TML_N_EPOCHS];
+    atomicAdd(&a->dur_ns[phase], d);
+    atomicAdd(&a->n_calls[phase], 1u);
+  }
+}
+
 // Sampler side: copy the records committed since `from` (at most the newest mirror_slots) and the
 // live statistics into host-mapped memory.  One CTA, on the sampler's own stream; the caller
 // synchronises that stream, so no system-scope fence is needed here either.
@@ -476,6 +678,30 @@ __global__ void k_layer_commit(LayerAcc* acc, tml_layer_record* ring, u32 n_laye
   }
 }
 __global__ void k_layer_head(u64* head, u64 v) { *head = v; }
+
+// Device-committed mode: the ring position is the layer head and the step id the device's last one
+// (k_commit_dev ran just before on the same stream).  With several CTAs every CTA must have read the
+// head before it moves, so k_layer_head_inc moves it afterwards.
+__global__ void k_layer_commit_dev(LayerAcc* acc, tml_layer_record* ring, u32 n_layers, u32 ring_steps,
+                                   const DevState* st, u64* head) {
+  const u64 seq = *head, step = st->dc_step;
+  const u32 l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l < n_layers) {
+    LayerAcc a = acc[l];
+    tml_layer_record r;
+    r.step = step; r.fwd_ns = a.fwd_ns; r.bwd_ns = a.bwd_ns; r.fwd_calls = a.fwd_calls; r.bwd_calls = a.bwd_calls;
+    r.fwd_bytes = a.fwd_bytes; r.bwd_bytes = a.bwd_bytes;
+    ring[(size_t)(seq % ring_steps) * n_layers + l] = r;
+    LayerAcc z;
+    memset(&z, 0, sizeof(z));
+    acc[l] = z;
+  }
+  __syncthreads();
+  if (gridDim.x == 1) {
+    if (threadIdx.x == 0) { __threadfence(); *head = seq + 1; }
+  }
+}
+__global__ void k_layer_head_inc(u64* head) { *head += 1; }
 
 // ------------------------------------------------------------------ K5: proc commit
 
@@ -2127,6 +2353,13 @@ struct tml_ctx {
   unsigned long long graph_capture = 0;        // capture sequence that holds graph_cur
   GraphCapture* graph_cur = nullptr;
   GraphRefs* graph_refs = nullptr;
+  u64 graph_step_slots = 0;  // graph slots (bit per depth) opened by tml_graph_step_begin
+  // Device-committed mode, entered by the first captured step commit: from then on the commit number
+  // and the step id are counted on the device (DevState::dc_*), and `commits` / `last_step` are
+  // refreshed from there by their readers.
+  bool dc_on = false;
+  bool dc_seeded = false;  // k_set_dc has given the device words their base
+  u64 dc_base = 0;         // the step id before any commit (tml_graph_step_publish)
   u64 host_dur[TML_MAX_PHASES] = {0};
   u32 host_calls[TML_MAX_PHASES] = {0};
   // sampler-thread state
@@ -2393,11 +2626,14 @@ int tml_shutdown(tml_ctx* c) {
   cudaDeviceSynchronize();
   for (auto& kv : c->peers) cudaIpcCloseMemHandle(kv.second);
   // a live graph's stamps still write into the DevState and the layer accumulators: those few KB
-  // stay allocated for the rest of the process
+  // stay allocated for the rest of the process, and so do the step and layer rings once a step
+  // commit has been captured
   const u64 graphs_live = c->graph_refs->graphs.load();
+  const bool rings_live = graphs_live && c->dc_on;
   if (!graphs_live) { cudaFree(c->d_state); cudaFree(c->d_layer_acc); }
   if (c->graph_refs->owners.fetch_sub(1) == 1) delete c->graph_refs;
-  cudaFree(c->ring.hot); cudaFree(c->d_pring);
+  if (!rings_live) { cudaFree(c->ring.hot); cudaFree(c->d_layer_ring); cudaFree(c->d_layer_head); }
+  cudaFree(c->d_pring);
   cudaFree(c->d_load_stage);
   if (c->load_stream) cudaStreamDestroy(c->load_stream);
   for (int b = 0; b < 2; ++b) {
@@ -2411,7 +2647,6 @@ int tml_shutdown(tml_ctx* c) {
   cudaFree(c->d_selrow); cudaFree(c->d_selstep); cudaFree(c->d_blockcnt); cudaFree(c->d_total);
   cudaFree(c->d_noncontig); cudaFree(c->d_gacc);
   cudaFree(c->d_xs_buf); cudaFree(c->d_xs_out); cudaFree(c->d_xs_stats);
-  cudaFree(c->d_layer_ring); cudaFree(c->d_layer_head);
   if (c->h_layer_stage) cudaFreeHost(c->h_layer_stage);
   if (c->drain_stream) cudaStreamDestroy(c->drain_stream);
   if (c->xs_stream) cudaStreamDestroy(c->xs_stream);
@@ -2470,7 +2705,8 @@ int tml_phase_end(tml_ctx* c, uint32_t phase, int slot, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard dg(c);
   if (check_capture(s)) return TML_ERR_CAPTURE;
-  k_stamp_end<<<1, 32, 0, s>>>(c->d_state, (u32)slot, phase, (u32)(c->commits % TML_N_EPOCHS));
+  k_stamp_end<<<1, 32, 0, s>>>(c->d_state, (u32)slot, phase,
+                               c->dc_on ? TML_EPOCH_FROM_HEAD : (u32)(c->commits % TML_N_EPOCHS));
   c->launches += 1;
   if (cudaPeekAtLastError() != cudaSuccess)
     return set_err(TML_ERR_CUDA, "stamp_end launch: %s", cudaGetErrorString(cudaGetLastError()));
@@ -2522,6 +2758,35 @@ static int graph_hold(tml_ctx* c, cudaStream_t s, bool layers, const char* what)
   return TML_OK;
 }
 
+// Device-committed mode: the first host launch after the mode is entered gives the device words
+// their base (the host's count, and its last step id or the published base), in stream order.
+static int dc_seed(tml_ctx* c, cudaStream_t s) {
+  if (c->dc_seeded) return TML_OK;
+  k_set_dc<<<1, 1, 0, s>>>(c->d_state, c->commits, c->commits > 0 ? c->last_step : c->dc_base, 1, 0, 0, 0);
+  c->launches += 1;
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "seed launch: %s", cudaGetErrorString(cudaGetLastError()));
+  c->dc_seeded = true;
+  return TML_OK;
+}
+
+// Readers of `commits` / `last_step` in device-committed mode fetch them from the device first: one
+// 16-B copy.  They run with the step path quiescent (summary builds, tests), never on it.
+static int dc_refresh(tml_ctx* c) {
+  if (!c->dc_on || !c->dc_seeded) return TML_OK;
+  static_assert(offsetof(DevState, dc_step) == offsetof(DevState, dc_head) + 8, "dc words are adjacent");
+  u64 w[2];
+  CK(cudaMemcpy(w, &c->d_state->dc_head, sizeof(w), cudaMemcpyDeviceToHost));
+  c->commits = w[0];
+  c->last_step = w[1];
+  return TML_OK;
+}
+#define DC_REFRESH(c)                        \
+  do {                                       \
+    const int rc_ = dc_refresh(c);           \
+    if (rc_ != TML_OK) return rc_;           \
+  } while (0)
+
 extern "C" {
 
 int tml_graph_phase_begin(tml_ctx* c, uint32_t phase, void* stream) {
@@ -2546,7 +2811,7 @@ int tml_graph_phase_end(tml_ctx* c, uint32_t phase, int slot, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard dg(c);
   std::lock_guard<std::mutex> g(c->graph_mu);
-  if ((u32)slot + 1u != c->graph_depth)
+  if ((u32)slot + 1u != c->graph_depth || ((c->graph_step_slots >> slot) & 1ull))
     return set_err(TML_ERR_ARG, "tml_graph_phase_end: slot %d is not the innermost open graph region", slot);
   c->graph_depth = (u32)slot;  // the region is closed on the host whatever the capture does below
   int rc = graph_hold(c, s, false, "tml_graph_phase_end");
@@ -2558,6 +2823,92 @@ int tml_graph_phase_end(tml_ctx* c, uint32_t phase, int slot, void* stream) {
 }
 
 uint64_t tml_graph_refs(void) { return g_graph_refs.load(); }
+
+// ---------------------------------------------------------------- graph-captured steps
+// A step whose begin and commit are captured: the begin stamps its wall into a graph slot (the
+// rules of tml_graph_phase_begin), the commit closes that slot and captures k_commit_dev.  The first
+// captured commit puts the context in device-committed mode.
+int tml_graph_step_begin(tml_ctx* c, void* stream) {
+  if (!c) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  if (c->graph_depth >= TML_N_GSLOTS)
+    return set_err(TML_ERR_STATE, "tml_graph_step_begin: %u graph regions already open", TML_N_GSLOTS);
+  int rc = graph_hold(c, s, false, "tml_graph_step_begin");
+  if (rc != TML_OK) return rc;
+  const u32 slot = c->graph_depth;
+  k_stamp_begin<<<1, 32, 0, s>>>(c->d_state, TML_N_SLOTS + slot);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph step_begin capture: %s", cudaGetErrorString(cudaGetLastError()));
+  c->graph_depth = slot + 1u;
+  c->graph_step_slots |= 1ull << slot;
+  return (int)slot;
+}
+
+int tml_graph_step_commit(tml_ctx* c, uint32_t flags, void* stream) {
+  if (!c || (flags & ~(TML_REC_HAS_MEM | TML_GRAPH_STEP_FAILED))) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  const u32 slot = c->graph_depth - 1u;
+  if (c->graph_depth == 0 || !((c->graph_step_slots >> slot) & 1ull))
+    return set_err(TML_ERR_STATE, "tml_graph_step_commit: the innermost open graph region is not a step");
+  c->graph_depth = slot;  // closed on the host whatever the capture does below
+  c->graph_step_slots &= ~(1ull << slot);
+  int rc = graph_hold(c, s, false, "tml_graph_step_commit");
+  if (rc != TML_OK) return rc;
+  DevCommitArgs a;
+  memset(&a, 0, sizeof(a));
+  a.flags = flags & TML_REC_HAS_MEM;
+  a.advance = (flags & TML_GRAPH_STEP_FAILED) ? 0u : 1u;
+  a.wall_slot = TML_N_SLOTS + slot;
+  k_commit_dev<<<1, 192, 0, s>>>(c->d_state, c->ring, a);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "graph step_commit capture: %s", cudaGetErrorString(cudaGetLastError()));
+  c->dc_on = true;
+  return TML_OK;
+}
+
+int tml_graph_step_publish(tml_ctx* c, uint64_t base_step, uint64_t alloc, uint64_t resv, void* stream) {
+  if (!c) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  if (check_capture(s)) return TML_ERR_CAPTURE;
+  if (!c->dc_seeded) c->dc_base = base_step;
+  if (c->dc_on) {
+    int rc = dc_seed(c, s);
+    if (rc != TML_OK) return rc;
+  }
+  k_set_dc<<<1, 1, 0, s>>>(c->d_state, 0, 0, 0, alloc, resv, 1);
+  c->launches += 1;
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "publish launch: %s", cudaGetErrorString(cudaGetLastError()));
+  return TML_OK;
+}
+
+int tml_graph_step_id(tml_ctx* c, uint64_t* step) {
+  if (!c || !step) return TML_ERR_ARG;
+  if (!c->dc_on) return TML_ERR_STATE;
+  DeviceGuard dg(c);
+  if (!c->dc_seeded) { *step = c->commits > 0 ? c->last_step : c->dc_base; return TML_OK; }
+  CK(cudaMemcpy(step, &c->d_state->dc_step, sizeof(u64), cudaMemcpyDeviceToHost));
+  return TML_OK;
+}
+
+int tml_graph_phase_host(tml_ctx* c, uint32_t phase, uint64_t dur_ns, void* stream) {
+  if (!c || phase >= TML_MAX_PHASES) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (!c->dc_on || check_capture(s)) return tml_phase_host(c, phase, dur_ns);
+  DeviceGuard dg(c);
+  int rc = dc_seed(c, s);
+  if (rc != TML_OK) return rc;
+  k_host_phase<<<1, 32, 0, s>>>(c->d_state, phase, dur_ns);
+  c->launches += 1;
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "host phase launch: %s", cudaGetErrorString(cudaGetLastError()));
+  return TML_OK;
+}
 
 // ---------------------------------------------------------------- deep profile
 int tml_layer_init(tml_ctx* c, uint32_t n_layers, uint32_t steps) {
@@ -2640,12 +2991,41 @@ int tml_graph_layer_end(tml_ctx* c, uint32_t layer, uint32_t direction, int slot
   return TML_OK;
 }
 
+}  // extern "C"
+
+// The layer step close of device-committed mode: ring position from d_layer_head, step id from the
+// device's last one.  Launched by the host or captured into a graph (`captured`: not a launch).
+static int layer_commit_dev(tml_ctx* c, cudaStream_t s, bool captured) {
+  const int blocks = (int)((c->n_layers + 255) / 256);
+  k_layer_commit_dev<<<blocks, 256, 0, s>>>(c->d_layer_acc, c->d_layer_ring, c->n_layers, c->layer_steps,
+                                            c->d_state, c->d_layer_head);
+  if (blocks > 1) k_layer_head_inc<<<1, 1, 0, s>>>(c->d_layer_head);
+  if (cudaPeekAtLastError() != cudaSuccess)
+    return set_err(TML_ERR_CUDA, "layer commit: %s", cudaGetErrorString(cudaGetLastError()));
+  if (!captured) c->launches += blocks > 1 ? 2 : 1;
+  return TML_OK;
+}
+
+extern "C" {
+
+int tml_graph_layer_commit(tml_ctx* c, void* stream) {
+  if (!c) return TML_ERR_ARG;
+  if (!c->n_layers) return TML_ERR_STATE;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  std::lock_guard<std::mutex> g(c->graph_mu);
+  int rc = graph_hold(c, s, true, "tml_graph_layer_commit");
+  if (rc != TML_OK) return rc;
+  return layer_commit_dev(c, s, true);
+}
+
 int tml_layer_commit(tml_ctx* c, uint64_t step, void* stream) {
   if (!c || !c->n_layers) return TML_ERR_STATE;
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard dg(c);
   if (check_capture(s)) return TML_ERR_CAPTURE;
   const int blocks = (int)((c->n_layers + 255) / 256);
+  if (c->dc_on) return layer_commit_dev(c, s, false);  // `step` is the device's
   k_layer_commit<<<blocks, 256, 0, s>>>(c->d_layer_acc, c->d_layer_ring, c->n_layers, c->layer_steps,
                                         c->layer_commits, step, c->d_layer_head);
   if (blocks > 1) k_layer_head<<<1, 1, 0, s>>>(c->d_layer_head, c->layer_commits + 1);
@@ -2704,6 +3084,27 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard dg(c);
   if (check_capture(s)) return TML_ERR_CAPTURE;
+  if (c->dc_on) {  // the device counts: `step` only says whether the step advanced the id
+    int rc = dc_seed(c, s);
+    if (rc != TML_OK) return rc;
+    DevCommitArgs d;
+    d.host_ts = host_ts;
+    memcpy(d.host_dur, c->host_dur, sizeof(d.host_dur));
+    memcpy(d.host_calls, c->host_calls, sizeof(d.host_calls));
+    d.peak_alloc = peak_alloc;
+    d.peak_resv = peak_resv;
+    d.flags = flags;
+    d.advance = step != 0 ? 1u : 0u;
+    d.wall_slot = TML_NO_WALL_SLOT;
+    k_commit_dev<<<1, 192, 0, s>>>(c->d_state, c->ring, d);
+    memset(c->host_dur, 0, sizeof(c->host_dur));
+    memset(c->host_calls, 0, sizeof(c->host_calls));
+    if (cudaPeekAtLastError() != cudaSuccess)
+      return set_err(TML_ERR_CUDA, "commit launch: %s", cudaGetErrorString(cudaGetLastError()));
+    c->launches += 1;
+    c->win_ready = false;
+    return TML_OK;
+  }
   CommitArgs a;
   a.step = step; a.host_ts = host_ts;
   memcpy(a.host_dur, c->host_dur, sizeof(a.host_dur));
@@ -2727,7 +3128,14 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
   return TML_OK;
 }
 
-uint64_t tml_step_count(tml_ctx* c) { return c ? c->commits : 0; }
+uint64_t tml_step_count(tml_ctx* c) {
+  if (!c) return 0;
+  if (c->dc_on) {
+    DeviceGuard dg(c);
+    dc_refresh(c);
+  }
+  return c->commits;
+}
 uint64_t tml_launch_count(tml_ctx* c) { return c ? c->launches : 0; }
 uint64_t tml_proc_count(tml_ctx* c) { return c ? c->proc_commits.load() : 0; }
 uint64_t tml_sys_count(tml_ctx* c) {
@@ -2883,10 +3291,12 @@ extern "C" {
 uint64_t tml_ring_load_chunk_(void) { return RING_LOAD_CHUNK; }
 
 int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stream) {
-  if (!c || (!out && n) || first + n > c->commits || c->commits - first > c->ring.slots)
+  if (!c) return TML_ERR_ARG;
+  DeviceGuard dg(c);
+  DC_REFRESH(c);
+  if ((!out && n) || first + n > c->commits || c->commits - first > c->ring.slots)
     return set_err(TML_ERR_ARG, "tml_ring_read_: records outside the retained ring");
   if (n == 0) return TML_OK;
-  DeviceGuard dg(c);
   k_ring_join<<<grid_for(c, n * 16, 256), 256, 0, (cudaStream_t)stream>>>(c->ring, first, n, (u64*)out);
   CK(cudaPeekAtLastError());
   return TML_OK;
@@ -2900,6 +3310,7 @@ int tml_ring_certified_(tml_ctx* c, uint32_t window) {
                 offsetof(DevState, unusable_mark) == offsetof(DevState, gap_mark) + 16, "marks are adjacent");
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(marks, &c->d_state->gap_mark, sizeof(marks), cudaMemcpyDeviceToHost));
+  DC_REFRESH(c);
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   return window_certified(marks[0], marks[1], marks[2], c->commits - n, n > window ? n - window : 0) ? 1 : 0;
 }
@@ -2911,6 +3322,7 @@ int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* str
   if (!c || (!host && n)) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   DeviceGuard dg(c);
+  DC_REFRESH(c);
   {  // if n > slots only the last `slots` survive
     const u32 slots = c->ring.slots;
     const u64 keep = n > slots ? (u64)slots : n;
@@ -2953,6 +3365,10 @@ int tml_ring_load(tml_ctx* c, const tml_step_record* host, uint64_t n, void* str
   c->commits += n;
   k_set_heads<<<1, 1, 0, s>>>(c->d_state, c->commits, 0, 0);
   CK(cudaPeekAtLastError());
+  if (c->dc_on && c->dc_seeded) {
+    k_set_dc<<<1, 1, 0, s>>>(c->d_state, c->commits, c->last_step, 1, 0, 0, 0);
+    CK(cudaPeekAtLastError());
+  }
   c->win_ready = false;
   // bulk-loaded history is not new telemetry: the sampler's cursor starts behind it
   c->mirror_copied = c->drain_tail = c->commits;
@@ -3051,6 +3467,7 @@ int tml_ring_reset(tml_ctx* c) {
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   memset(c->h_page, 0, sizeof(HostPage));
   c->commits = 0; c->proc_commits.store(0); c->next_slot = 0;
+  if (c->dc_on) c->dc_seeded = true;  // the cleared device words: no commit, last id 0
   c->sys_commits = 0; c->sys_last_n = 0;
   c->drain_tail = 0; c->pdrain_tail = 0; c->mirror_copied = 0;
   memset(c->host_dur, 0, sizeof(c->host_dur));
@@ -3144,6 +3561,7 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
   if (!c || !out || window == 0) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
+  DC_REFRESH(c);
   memset(out, 0, sizeof(*out));
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
@@ -3252,6 +3670,10 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
 
 int tml_win_peek(tml_ctx* c, uint32_t window, uint64_t* n_retained, uint64_t* n_window) {
   if (!c || window == 0) return TML_ERR_ARG;
+  if (c->dc_on) {
+    DeviceGuard dg(c);
+    DC_REFRESH(c);
+  }
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   if (n_retained) *n_retained = n;
   if (n_window) *n_window = n > window ? window : n;
@@ -3319,6 +3741,7 @@ int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uin
   if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
+  DC_REFRESH(c);
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   if (n == 0) return set_err(TML_ERR_STATE, "chained window pass over an empty ring");
   c->win_ready = false;
@@ -3386,6 +3809,7 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
   memset(out, 0, sizeof(*out));
   memset(aligned, 0, sizeof(*aligned));
   *ok = 0;
+  DC_REFRESH(c);
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   c->win_ready = false;
   out->n_retained = n;

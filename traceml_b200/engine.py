@@ -48,6 +48,10 @@ class Engine:
         self._commit = self._lib.tml_step_commit
         self._gbegin = self._lib.tml_graph_phase_begin  # regions captured into a CUDA graph
         self._gend = self._lib.tml_graph_phase_end
+        self._gsbegin = self._lib.tml_graph_step_begin  # steps captured into a CUDA graph
+        self._gscommit = self._lib.tml_graph_step_commit
+        self._gpublish = self._lib.tml_graph_step_publish
+        self._ghost = self._lib.tml_graph_phase_host
         self._drain_buf = np.zeros(4096, dtype=STEP_RECORD_DTYPE)
         self._pdrain_buf = np.zeros(8192, dtype=PROC_RECORD_DTYPE)
         self._run_out = _abi.ReduceRunOut()
@@ -97,6 +101,12 @@ class Engine:
 
     def step_discard(self) -> None:
         self._lib.tml_step_discard(self._h)
+
+    def graph_step_id(self) -> int:
+        """The device's last step id once a step commit has been captured (one 8-B read)."""
+        out = C.c_uint64(0)
+        _abi.check(self._lib.tml_graph_step_id(self._h, C.byref(out)), "tml_graph_step_id")
+        return int(out.value)
 
     @property
     def step_count(self) -> int:

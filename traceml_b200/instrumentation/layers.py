@@ -20,6 +20,7 @@ only under ``TRACEML_PROFILE=deep`` (``sdk/instrumentation.py:222``).
 from __future__ import annotations
 
 import ctypes as C
+import sys
 import time
 from typing import Any, Dict, Iterable, List, Optional, Tuple
 
@@ -139,6 +140,15 @@ class LayerProfile:
             self._lib.tml_layer_commit(self.engine._h, int(step),
                                        torch._C._cuda_getCurrentRawStream(self.engine.device))
 
+    def commit_graph(self) -> None:
+        """The step boundary of a step captured into a CUDA graph: every replay closes the layers'
+        step under the step id the device assigned."""
+        if self.names:
+            rc = self._lib.tml_graph_layer_commit(self.engine._h,
+                                                  torch._C._cuda_getCurrentRawStream(self.engine.device))
+            if rc < 0:
+                print(f"[TraceML] layer step close not captured (status {rc})", file=sys.stderr)
+
     def drain(self) -> np.ndarray:
         """Finished steps as a ``[steps, layers]`` record array (sampler thread)."""
         if not self.names:
@@ -204,10 +214,15 @@ def commit_all(step: int) -> None:
         p.commit(step)
 
 
+def commit_all_graph() -> None:
+    for p in _PROFILES.values():
+        p.commit_graph()
+
+
 def reset() -> None:
     for p in _PROFILES.values():
         p.detach()
     _PROFILES.clear()
 
 
-__all__ = ["LayerProfile", "attach", "profile_of", "commit_all", "reset", "get_hookable_modules", "LAYER_RECORD_DTYPE"]
+__all__ = ["LayerProfile", "attach", "profile_of", "commit_all", "commit_all_graph", "reset", "get_hookable_modules", "LAYER_RECORD_DTYPE"]

@@ -10,11 +10,12 @@ from threading import RLock
 
 
 class TraceSessionState:
-    __slots__ = ("_step", "_lock")
+    __slots__ = ("_step", "_lock", "_device_step")
 
     def __init__(self, initial_step: int = 0) -> None:
         self._lock = RLock()
         self._step = self._check(initial_step)
+        self._device_step = None
 
     @staticmethod
     def _check(value: int) -> int:
@@ -26,8 +27,17 @@ class TraceSessionState:
 
     @property
     def step(self) -> int:
+        """The last step id.  Once a step commit has been captured into a CUDA graph the replays
+        create the steps on the device, and this reads the device's last id (one 8-B copy)."""
+        read = self._device_step
+        if read is not None:
+            return read()
         with self._lock:
             return self._step
+
+    def bind_device_step(self, read) -> None:
+        """``read()`` returns the device's last step id from now on (None: the host counter again)."""
+        self._device_step = read
 
     def set_step(self, value: int) -> int:
         v = self._check(value)

@@ -17,6 +17,11 @@ Under CUDA-graph capture the stamp entry points return ``TML_ERR_CAPTURE`` and t
 region takes the host clock, unless a ``trace_graph`` scope is open on this thread:
 then the stamps are captured into the graph (``tml_graph_phase_begin`` / ``_end``)
 and time the region on every replay.
+
+Once a step commit has been captured (``DEVICE_STEPS``), replays commit steps on the
+device, and host-clock regions are added there too (``tml_graph_phase_host``): to
+the step the device has open when they run, so input waits between replays land in
+the step the next replay commits.
 """
 from __future__ import annotations
 
@@ -51,11 +56,13 @@ GRAPH_SLOT0 = -(1 << 16)
 
 class _GraphScope(threading.local):
     depth = 0   # open trace_graph scopes on this thread
+    steps = 0   # step commits this thread captured (trace_graph publishes memory when it grew)
 
 
 GRAPH_SCOPE = _GraphScope()
 GRAPH_SCOPES_OPEN = [0]  # open trace_graph scopes in the process (layer backward hooks run on
                          # autograd's device thread, not on the thread that opened the scope)
+DEVICE_STEPS = False     # the engine is in device-committed mode (a step commit was captured)
 
 
 def _resolve():
@@ -89,8 +96,13 @@ class _Quiet(RuntimeError):
 
 
 def _reset() -> None:
-    global _ENG, _FAST, _RESOLVE_FAILED
+    global _ENG, _FAST, _RESOLVE_FAILED, DEVICE_STEPS
     _RESOLVE_FAILED = None
+    if DEVICE_STEPS:
+        from ..runtime import get_trace_session_state
+
+        get_trace_session_state().bind_device_step(None)
+        DEVICE_STEPS = False
     if _FAST is not None:
         try:
             _FAST.unbind()
@@ -215,7 +227,10 @@ class timed_region:
                 if self.slot >= 0:
                     fast.end(self.phase, self.slot)
                 elif self.slot > GRAPH_SLOT0:
-                    fast.host(self.phase, _perf_ns() - self.t0)
+                    if DEVICE_STEPS:
+                        _device_host(self.eng, self.phase, _perf_ns() - self.t0)
+                    else:
+                        fast.host(self.phase, _perf_ns() - self.t0)
                 else:
                     self._graph_end()
             else:
@@ -223,7 +238,10 @@ class timed_region:
                 if self.slot >= 0:
                     eng._end(eng._h, self.phase, self.slot, _raw_stream(_cur_dev()))
                 elif self.slot > GRAPH_SLOT0:
-                    eng._host(eng._h, self.phase, _perf_ns() - self.t0)
+                    if DEVICE_STEPS:
+                        _device_host(eng, self.phase, _perf_ns() - self.t0)
+                    else:
+                        eng._host(eng._h, self.phase, _perf_ns() - self.t0)
                 else:
                     self._graph_end()
         except Exception as e:  # nothing here may break training
@@ -237,6 +255,11 @@ class timed_region:
             print(f"[TraceML] graph region not closed (status {rc})", file=sys.stderr)
 
 
+def _device_host(eng, phase: int, dur_ns: int) -> None:
+    """A host-clock duration in device-committed mode: added on the device, in stream order."""
+    eng._ghost(eng._h, phase, max(0, int(dur_ns)), _raw_stream(_cur_dev()))
+
+
 def record_event(evt: TimeEvent) -> None:
     """Record an already-measured event (host duration) into the open step."""
     if disabled():
@@ -247,7 +270,11 @@ def record_event(evt: TimeEvent) -> None:
     try:
         ms = evt.gpu_time_ms if evt.gpu_time_ms is not None else (evt.cpu_end - evt.cpu_start) * 1000.0
         eng = _ENG or _resolve()
-        eng._host(eng._h, phase_of(evt.name), max(0, int(round(float(ms) * 1.0e6))))
+        dur = max(0, int(round(float(ms) * 1.0e6)))
+        if DEVICE_STEPS:
+            _device_host(eng, phase_of(evt.name), dur)
+        else:
+            eng._host(eng._h, phase_of(evt.name), dur)
     except _Quiet:
         pass
     except Exception as exc:

@@ -144,8 +144,9 @@ int tml_phase_host(tml_ctx* ctx, uint32_t phase, uint64_t dur_ns);
 /* Close the step: commit kernel stages the in-flight record through shared
  * memory, merges the host-clock phases and the allocator peaks (c10 allocator
  * counters are host state: they travel as launch arguments), writes one
- * record into the HBM ring (kept there as a 64-B hot half, a 64-B cold half
- * and a memory byte), updates the running statistics and
+ * record into the HBM ring (kept there as a 64-B hot half, a 64-B cold half,
+ * a 32-B packed copy of the hot half and a memory byte), updates the running
+ * statistics and
  * bumps the head.  It writes NOTHING to host memory and issues no system-scope
  * fence: the training stream pays for the record, not for the sampler.
  * Replaces StepMemoryTracker.record + flush_step_events:

@@ -4,7 +4,10 @@ Runs ``bench.py --gpus 1 --steps K --warmup W --no-cpu-baseline`` from tree A, t
 ``--rounds`` rounds, each in a process of its own, and prints one JSON line with, per tree, the median
 and min-max of: ``ms_per_step``, ``sustained.ms_per_step``, the fused pass
 (``roofline.kernels.k_window_fused.ms``), ``e2e.ms_per_step``, ``default_window.ms`` and
-``step_overhead.micro_mlp.b200_overhead_us``; plus ``parity.ok`` / ``series.bit_equal`` of every run,
+``step_overhead.micro_mlp.b200_overhead_us``, the step path's ``step_overhead.telemetry_rate.step_records_per_s``
+and ``step_overhead.api_cost_us.step_commit``, and the device time of one ring load of the bench's
+records (``profiles/ring_load.py`` of this tree run against each tree, once per round, median of its
+loads); plus ``parity.ok`` / ``series.bit_equal`` of every run,
 whether the ``--dump-outputs`` files of the first round are byte-identical between the trees,
 ``profiles/single_rank_build.py``'s pass-vs-copy-ceiling figures of each tree (one run each, after
 the rounds) and the card's name, power limit and max SM clock (read-only ``nvidia-smi`` query).
@@ -33,6 +36,9 @@ METRICS = {
     "e2e_ms_per_step": ("e2e", "ms_per_step"),
     "default_window_ms": ("default_window", "ms"),
     "micro_mlp_overhead_us": ("step_overhead", "micro_mlp", "b200_overhead_us"),
+    "step_records_per_s": ("step_overhead", "telemetry_rate", "step_records_per_s"),
+    "step_commit_us": ("step_overhead", "api_cost_us", "step_commit"),
+    "ring_load_ms": ("ring_load", "load_ms", "median"),
 }
 
 
@@ -89,6 +95,7 @@ def main() -> None:
             if r == 0:
                 cmd += ["--dump-outputs", os.path.join(os.path.abspath(args.out), f"dump_{name}")]
             res = run(tree, cmd)
+            res["ring_load"] = run(tree, [os.path.join(ROOT, "profiles", "ring_load.py"), "--tree", tree])
             runs[name].append(res)
             print(json.dumps({"round": r, "tree": name, **{k: dig(res, p) for k, p in METRICS.items()},
                               "error": res.get("error")}), file=sys.stderr, flush=True)

@@ -15,9 +15,11 @@ line:
   * ``kernel_ms``: device time per build of each kernel (torch.profiler, a run of its own), and
     ``device_idle_ms``: ``build_ms`` minus the pass and the band kernel;
   * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved), CUDA events,
-    median of 25 after warm-up; the fused pass against it, counting the bytes it moves: the 64-B hot
-    half of each ring record and its memory byte, plus W * 64 of series when each median / worst
-    series pair is stored once (``series_paired``, W * 129 in all), W * 128 otherwise (W * 193);
+    median of 25 after warm-up; the fused pass against it, counting the bytes it moves by the stream
+    that ran (``stream``): 32 B per step for a packed-streamable window (the ring's packed records),
+    64 B for another certified one (the hot halves), 65 B otherwise (the hot halves and the memory
+    bytes), plus W * 64 of series when each median / worst series pair is stored once
+    (``series_paired``), W * 128 otherwise;
   * ``gpu``: card name, power limit and max SM clock (read-only ``nvidia-smi`` query).
 """
 from __future__ import annotations
@@ -184,18 +186,22 @@ def measure(steps: int, window: int, warmup: int) -> dict:
         sj.append((time.perf_counter() - t0) * 1e3)
     seg = segments(summ, W, steps)
     kern = kernel_times(torch, summ, W)
+    from traceml_b200 import _abi
+
+    stream = ("packed" if _abi.lib().tml_ring_packed_(eng.handle, W) == 1 else
+              "certified" if _abi.lib().tml_ring_certified_(eng.handle, W) == 1 else "general")
     eng.close()
     del host, recs
     med = {k: statistics.median(v) for k, v in stage.items() if not k.startswith("host_")}
     wall_ms, sj_ms = statistics.median(wall), statistics.median(sj)
     ceil = copy_ceiling(torch)
-    # 65 B read per step (the ring's hot half and memory byte), plus 8 series x 8 B written when the
-    # pairs are mapped twice (series_paired), 16 x 8 B otherwise
-    fused_bytes = W * (129.0 if paired else 193.0)
+    # bytes read per step by the stream that ran, plus 8 series x 8 B written when the pairs are
+    # mapped twice (series_paired), 16 x 8 B otherwise
+    fused_bytes = W * ({"packed": 32.0, "certified": 64.0, "general": 65.0}[stream] + (64.0 if paired else 128.0))
     k3a = med.get("k3a") or 0.0
     fused_gbps = fused_bytes / (k3a * 1e-3) / 1e9 if k3a else None
     return {
-        "window": W, "steps": steps, "fused_rows": fused, "series_paired": paired,
+        "window": W, "steps": steps, "fused_rows": fused, "series_paired": paired, "stream": stream,
         "build_ms": build_ms, "build_wall_ms": wall_ms, "launches_per_build": launches,
         "stage_ms": med, "sections_json_ms": sj_ms,
         "python_rest_ms": wall_ms - med.get("total", 0.0) - sj_ms,

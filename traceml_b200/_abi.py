@@ -326,6 +326,8 @@ SIGNATURES = {
     "tml_ring_load_chunk_": (u64, []),
     # private: the dense-window certificate the ring's writers keep, for the last `window` rows
     "tml_ring_certified_": (C.c_int, [vp, u32]),
+    # private: that certificate and every retained record within the ring's packed copy
+    "tml_ring_packed_": (C.c_int, [vp, u32]),
 }
 
 _LIB: Optional[C.CDLL] = None

@@ -3,7 +3,7 @@
 // Kernel map (DESIGN.md section 4):
 //   K1  k_stamp_begin / k_stamp_end   %globaltimer phase stamps on the training stream
 //   K2  k_commit                      in-flight record -> smem -> the HBM ring's hot and cold
-//                                     halves + memory byte, running stats
+//                                     halves, packed copy + memory byte, running stats
 //   K5  k_proc_commit                 64-B process sample into the proc ring
 //   K3a k_window_rows                 ring -> WindowRow[] (ns->ms), step ids, flags, bounds
 //   K3b k_presence                    presence bytes over [glo, glo+span)
@@ -50,9 +50,10 @@ static_assert(sizeof(tml_proc_record) == 64, "ProcRecord must be 64 B");
 static_assert(sizeof(tml_sys_gpu) == 32 && sizeof(tml_sys_record) == 576, "SysRecord must be 64 + 16 x 32 B");
 
 // ------------------------------------------------------------------ step ring layout (device only)
-// Slot k of the step ring is the public 128-B tml_step_record split in two 64-B halves plus a byte.
-// The window pass reads only the hot half and the memory byte (65 B per step, not 128); the cold
-// half holds what only the drain, the staged rows (h2d) and the live tick read.
+// Slot k of the step ring is the public 128-B tml_step_record split in two 64-B halves plus a byte,
+// and a 32-B packed copy of the hot half.  The window pass reads the hot half and the memory byte
+// (65 B per step, not 128), or for a certified window whose records fit it the packed copy alone
+// (32 B); the cold half holds what only the drain, the staged rows (h2d) and the live tick read.
 struct RingHot {
   u64 step;
   u64 dl, fwd, bwd, opt, wall;  // dur_ns[0], dur_ns[2..5]
@@ -67,13 +68,49 @@ struct RingCold {
   u64 seq;
   u64 pad;
 };
+// A 32-B copy of the hot half without the step id, as one 256-bit little-endian bit string:
+// dl [0,36) fwd [36,72) bwd [72,108) opt [108,144) wall [144,180) peak_alloc [180,218)
+// peak_resv [218,256).  Exact for durations below 2^36 ns (68.7 s) and peaks below 2^38 B (256 GiB);
+// a record outside those raises DevState::wide_mark and its packed copy is never read.
+struct __align__(32) RingPacked {
+  u64 w[4];
+};
+#define PACK_DUR_BITS 36
+#define PACK_MEM_BITS 38
 struct StepRing {
   RingHot* hot;
   RingCold* cold;
+  RingPacked* packed;
   u8* mem;  // 1 when the slot's flags have TML_REC_HAS_MEM (a copy of the bit in the cold half)
   u32 slots;
 };
 static_assert(sizeof(RingHot) == 64 && sizeof(RingCold) == 64, "ring halves must be 64 B");
+static_assert(sizeof(RingPacked) == 32, "packed record must be 32 B");
+
+// dl, fwd, bwd, opt, wall, peak_alloc, peak_resv (the hot half's words 1..7) -> the packed record
+__device__ __forceinline__ RingPacked pack_hot(u64 dl, u64 fwd, u64 bwd, u64 opt, u64 wall, u64 pa, u64 pr) {
+  RingPacked p;
+  p.w[0] = dl | (fwd << 36);
+  p.w[1] = (fwd >> 28) | (bwd << 8) | (opt << 44);
+  p.w[2] = (opt >> 20) | (wall << 16) | (pa << 52);
+  p.w[3] = (pa >> 12) | (pr << 26);
+  return p;
+}
+// does the record break the packed layout's ranges (DevState::wide_mark)?
+__device__ __forceinline__ bool pack_wide(u64 dl, u64 fwd, u64 bwd, u64 opt, u64 wall, u64 pa, u64 pr) {
+  return (((dl | fwd | bwd | opt | wall) >> PACK_DUR_BITS) | ((pa | pr) >> PACK_MEM_BITS)) != 0ull;
+}
+// the packed record's four words -> dl, fwd, bwd, opt, wall, peak_alloc, peak_resv
+__device__ __forceinline__ void unpack_hot(u64 w0, u64 w1, u64 w2, u64 w3, u64 (&v)[7]) {
+  const u64 md = (1ull << PACK_DUR_BITS) - 1ull, mm = (1ull << PACK_MEM_BITS) - 1ull;
+  v[0] = w0 & md;
+  v[1] = ((w0 >> 36) | (w1 << 28)) & md;
+  v[2] = (w1 >> 8) & md;
+  v[3] = ((w1 >> 44) | (w2 << 20)) & md;
+  v[4] = (w2 >> 16) & md;
+  v[5] = ((w2 >> 52) | (w3 << 12)) & mm;
+  v[6] = w3 >> 26;
+}
 // The mem array is read in 16-B pieces from the 16-B boundary at or below a tile's first slot:
 // it is allocated with this many bytes past the last slot.
 #define RING_MEM_PAD 32u
@@ -150,11 +187,13 @@ struct DevState {
   u64 layer_begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // deep profile: its own begin slots (hundreds of layer
                                                    // regions open and close while ONE phase region stays
                                                    // open), same two banks as begin_ts
-  // Dense-window certificate (window_certified): each mark is one past the newest commit number that
-  // breaks its condition, 0 = none.  Raised with atomicMax only, by k_commit and k_ring_split.
+  // Dense-window certificate (window_certified, window_packed): each mark is one past the newest
+  // commit number that breaks its condition, 0 = none.  Raised with atomicMax only, by k_commit,
+  // k_commit_dev and k_ring_split.
   u64 gap_mark;       // step id != the previous commit's step id + 1
   u64 nomem_mark;     // flags without TML_REC_HAS_MEM
   u64 unusable_mark;  // dl, fwd, bwd, opt and wall all 0 ns
+  u64 wide_mark;      // a duration >= 2^36 ns or a peak >= 2^38 B: the packed copy does not hold it
   // Device-committed mode (a step commit was captured into a CUDA graph): the commit number and the
   // step id live here, next to each other so that one copy refreshes the host's view of both
   u64 dc_head;    // == head, written by k_commit_dev and k_set_dc
@@ -184,6 +223,9 @@ __host__ __device__ __forceinline__ bool window_certified(u64 gap_mark, u64 nome
                                                           u64 first_k, u64 t_start) {
   return gap_mark <= first_k + 1 && nomem_mark <= first_k && unusable_mark <= first_k + t_start;
 }
+// A certified window is packed-streamable when every retained record fits its packed copy
+// (RingPacked): wide_mark follows the same rules as the certificate's marks.
+__host__ __device__ __forceinline__ bool window_packed(u64 wide_mark, u64 first_k) { return wide_mark <= first_k; }
 
 // host-mapped page: written by kernels, read by the sampler thread with no CUDA call
 struct HostPage {
@@ -300,7 +342,8 @@ __global__ void __maxnreg__(24) k_stamp_end(DevState* st, u32 slot, u32 phase, u
 
 // ------------------------------------------------------------------ K2: commit
 // 6 warps: warp p owns phase p's running statistics; warp 0 also assembles the
-// record in shared memory and writes its two 64-B ring halves (8 x 16-B stores) and the memory byte.
+// record in shared memory and writes its two 64-B ring halves (8 x 16-B stores), the memory byte
+// and the packed copy.
 
 // k_commit_dev's running statistics and ring store: k_commit's own code, which stays inline in
 // k_commit because calling these changes its SASS.
@@ -355,7 +398,7 @@ __device__ __forceinline__ void commit_stats(DevState* st, int warp, int lane, u
 }
 
 // Warp 0: the record staged in rec[16] (hot half, then cold half) -> ring slot `slot` as 8 x 16-B
-// stores, plus its memory byte.
+// stores, plus its memory byte and its packed copy.
 __device__ __forceinline__ void commit_store(const StepRing& ring, u64 slot, const u64* rec, int lane, u32 flags) {
   if (lane < 8) {
     uint4 v = reinterpret_cast<const uint4*>(rec)[lane];
@@ -363,6 +406,8 @@ __device__ __forceinline__ void commit_store(const StepRing& ring, u64 slot, con
     half[lane & 3] = v;
   } else if (lane == 8) {
     ring.mem[slot] = (flags & TML_REC_HAS_MEM) ? 1 : 0;
+  } else if (lane == 9) {
+    ring.packed[slot] = pack_hot(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7]);
   }
 }
 
@@ -479,6 +524,8 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, Com
       half[lane & 3] = v;
     } else if (lane == 8) {
       ring.mem[slot] = (a.flags & TML_REC_HAS_MEM) ? 1 : 0;
+    } else if (lane == 9) {
+      ring.packed[slot] = pack_hot(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7]);
     }
     __syncwarp();
     if (lane == 0) {
@@ -486,6 +533,7 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, Com
       if (a.gap) atomicMax(&st->gap_mark, seq + 1);
       if (a.nomem) atomicMax(&st->nomem_mark, seq + 1);
       if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
+      if (pack_wide(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7])) atomicMax(&st->wide_mark, seq + 1);
       __threadfence();  // the record is visible to every later reader of `head` on this GPU
       st->live.steps_committed = seq + 1;
       st->head = seq + 1;
@@ -587,6 +635,7 @@ __global__ void __launch_bounds__(192) k_commit_dev(DevState* st, StepRing ring,
       if (seq > 0 && !step_follows(last, step)) atomicMax(&st->gap_mark, seq + 1);
       if ((a.flags & TML_REC_HAS_MEM) == 0u) atomicMax(&st->nomem_mark, seq + 1);
       if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
+      if (pack_wide(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7])) atomicMax(&st->wide_mark, seq + 1);
       st->dc_step = step;
       st->dc_head = seq + 1;
       __threadfence();
@@ -1173,7 +1222,7 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // ------------------------------------------------------------------ K3a+K4 fused (single rank)
 // With ONE rank the cross-rank median and worst of a step are the rank's own value, so the
 // per-step series can be written straight from the ring records: 65 B in (the hot half and the memory
-// byte), 128 B out per step, and
+// byte; 32 B from the packed copies of a packed-streamable window), 128 B out per step, and
 // the 64-B WindowRows -- written by K3a only to be re-read by K4 (256 MB each way at
 // W = 4e6) -- never exist.  Same warp-private
 // cp.async pipeline as k_window_rows; lane = record, so each of the 16 series receives 32
@@ -1188,22 +1237,59 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // twice (tml_summary.cpp), so only the even rows are stored: 64 B out per step instead of 128.
 #define WF_WARP_U4 (WR_STAGES * WF_STAGE_U4)
 #define WF_SMEM_BYTES (WR_WARPS * WF_WARP_U4 * 16)
+// The packed stream's stages live in the same per-warp shared memory: a tile of 32 packed records
+// is 1 KB, half a tile of hot halves, so twice the stages keep at least as many bytes in flight
+// (7 KB per warp, 112 KB per SM at 2 CTAs).
+#define PK_STAGES 8
+#define TILE_PK_U4 (32 * 2)
+static_assert(PK_STAGES * TILE_PK_U4 <= WF_WARP_U4, "packed stages fit the warp's shared memory");
+
+// one warp fetches its tile of 32 packed records into one stage: 2 x cp.async per lane, each
+// instruction = 512 B contiguous, stored XOR-swizzled (16-B chunk q of record r at r*2 + (q ^ (r>>2 & 1)))
+// so that the per-lane 32-B read (two 16-B loads) is bank-conflict-free.
+__device__ __forceinline__ void packed_issue_tile(uint4* stage, const StepRing& ring, u64 slot0, u64 n, u64 base,
+                                                  int lane) {
+  const uint4* __restrict__ pk4 = reinterpret_cast<const uint4*>(ring.packed);
+  if (tile_linear(ring, slot0, n, base)) {
+    const uint4* src = pk4 + slot0 * 2;
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int idx = c * 32 + lane;
+      cp_async16(&stage[(idx & ~1) | ((idx ^ (idx >> 3)) & 1)], src + idx);
+    }
+    return;
+  }
+#pragma unroll
+  for (int c = 0; c < 2; ++c) {
+    const int idx = c * 32 + lane;
+    const int r = idx >> 1, q = idx & 1;
+    if (base + (u64)r < n) {
+      u64 slot = slot0 + (u64)r;
+      while (slot >= ring.slots) slot -= ring.slots;
+      cp_async16(&stage[r * 2 + (q ^ ((r >> 2) & 1))], &pk4[slot * 2 + q]);
+    }
+  }
+}
 
 // 2 CTAs of WR_THREADS per SM need <= 128 registers; left to itself ptxas takes 96 for the plain
 // instance, with the cap it keeps 94 with no spills.
 //
 // A window the ring's writers certified dense (window_certified, read once per CTA) takes a pure
-// stream of hot halves: every row is the first of its step id, has memory and a successor with a
-// new id, and every window row is usable, so the halo loads, memory bytes and neighbour shuffles
-// that decide this in general are not needed.  The tile -> warp -> CTA mapping and each lane's
-// order of additions are those of the general loop, so sums, maxima and counters are bit-identical.
-// Any other window takes the general loop.
+// stream: every row is the first of its step id, has memory and a successor with a new id, and
+// every window row is usable, so the halo loads, memory bytes and neighbour shuffles that decide
+// this in general are not needed.  When every retained record also fits its packed copy
+// (window_packed) the stream reads the 32-B packed records and takes the step ids from the first
+// retained row's (certified: they rise by exactly 1 per row); otherwise it reads the 64-B hot
+// halves.  Both streams share the per-row code, and their tile -> warp -> CTA mapping and each
+// lane's order of additions are those of the general loop, so sums, maxima and counters are
+// bit-identical.  Any other window takes the general loop.
 template <bool PAIRED>
 __global__ void __maxnreg__(94) k_window_fused(
     StepRing ring, u64 first_k, u64 n, u64 t_start,
     double* __restrict__ series, u64 ld, WinAcc* acc, double* partials, const DevState* st) {
   extern __shared__ __align__(16) unsigned char wr_smem[];
-  __shared__ u32 s_cert;
+  __shared__ u32 s_mode;  // 0: general, 1: certified (hot halves), 2: certified and packed
+  __shared__ u64 s_step0;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
 
@@ -1216,9 +1302,79 @@ __global__ void __maxnreg__(94) k_window_fused(
   const u64 wstride = (u64)gridDim.x * WR_WARPS;
   const u32 ring_slots = ring.slots;
 
-  if (tid == 0) s_cert = window_certified(st->gap_mark, st->nomem_mark, st->unusable_mark, first_k, t_start);
+  if (tid == 0) {
+    u32 mode = window_certified(st->gap_mark, st->nomem_mark, st->unusable_mark, first_k, t_start) ? 1u : 0u;
+    if (mode && window_packed(st->wide_mark, first_k)) {
+      mode = 2u;
+      s_step0 = ring.hot[first_k % ring_slots].step;
+    }
+    s_mode = mode;
+  }
   __syncthreads();
-  if (s_cert) {
+  // one certified row: row i of the window with step id `step` and the hot half's words 1..7
+  auto certified_row = [&](u64 i, u64 step, u64 d0, u64 d2, u64 d3, u64 d4, u64 d5, u64 pa, u64 pr) {
+    a_latest = step > a_latest ? step : a_latest;
+    a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1;
+    ++a_nr1;  // a memory candidate
+    if (i >= t_start) {  // a time candidate, usable
+      const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
+      const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4);
+      const double wall = ns_to_ms(d5);
+      a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0;
+      ++a_nr0;
+      const double compute = (fwd + bwd) + opt;
+      const double traced = fmax(wall, compute);
+      sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
+      sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
+      a_sa += pa; a_sr += pr;
+      mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
+      const double wait = fmax(0.0, traced - compute);
+      double* S = series + (i - t_start);
+      auto put = [&](int m, double v) {
+        S[(u64)(2 * m) * ld] = v;
+        if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
+      };
+      put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
+      put(4, traced); put(5, wait); put(6, (double)pa); put(7, (double)pr);
+    }
+  };
+  if (s_mode == 2u) {
+    const u64 step0 = s_step0;
+    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
+    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
+    u32 slot_iss = (u32)((first_k + wt * 32) % ring_slots);
+#pragma unroll
+    for (int s = 0; s < PK_STAGES - 1; ++s) {
+      const u64 t = wt + (u64)s * wstride;
+      if (t < nwt) packed_issue_tile(w_in + s * TILE_PK_U4, ring, slot_iss, n, t * 32, lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+    }
+    for (int it = 0; wt < nwt; wt += wstride, ++it) {
+      const uint4* cur = w_in + (it % PK_STAGES) * TILE_PK_U4;
+      const u64 base = wt * 32;
+      const u64 ahead = wt + (u64)(PK_STAGES - 1) * wstride;
+      if (ahead < nwt)
+        packed_issue_tile(w_in + ((it + PK_STAGES - 1) % PK_STAGES) * TILE_PK_U4, ring, slot_iss, n, ahead * 32,
+                          lane);
+      cp_async_commit();
+      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
+      cp_async_wait<PK_STAGES - 1>();
+      __syncwarp();
+      const u64 i = base + (u64)lane;
+      if (i < n) {
+        const int sw = (lane >> 2) & 1;
+        const uint4 p0 = cur[lane * 2 + sw], p1 = cur[lane * 2 + (sw ^ 1)];
+        u64 v[7];
+        unpack_hot((u64)p0.x | ((u64)p0.y << 32), (u64)p0.z | ((u64)p0.w << 32),
+                   (u64)p1.x | ((u64)p1.y << 32), (u64)p1.z | ((u64)p1.w << 32), v);
+        certified_row(i, step0 + i, v[0], v[1], v[2], v[3], v[4], v[5], v[6]);
+      }
+      __syncwarp();  // `cur` is free again
+    }
+    a_nc0 = a_tc = a_both = a_nr0;
+    a_nc1 = a_nr1;
+  } else if (s_mode == 1u) {
     u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
     const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
     u32 slot_iss = (u32)((first_k + wt * 32) % ring_slots);
@@ -1245,33 +1401,10 @@ __global__ void __maxnreg__(94) k_window_fused(
         const int sw = (lane >> 1) & 3;
         const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
         const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
-        const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-        a_latest = step > a_latest ? step : a_latest;
-        a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1;
-        ++a_nr1;  // a memory candidate
-        if (i >= t_start) {  // a time candidate, usable
-          const double dl = ns_to_ms((u64)c0.z | ((u64)c0.w << 32)), fwd = ns_to_ms((u64)c1.x | ((u64)c1.y << 32));
-          const double bwd = ns_to_ms((u64)c1.z | ((u64)c1.w << 32)), opt = ns_to_ms((u64)c2.x | ((u64)c2.y << 32));
-          const double wall = ns_to_ms((u64)c2.z | ((u64)c2.w << 32));
-          const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
-          const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
-          a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0;
-          ++a_nr0;
-          const double compute = (fwd + bwd) + opt;
-          const double traced = fmax(wall, compute);
-          sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
-          sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
-          a_sa += pa; a_sr += pr;
-          mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
-          const double wait = fmax(0.0, traced - compute);
-          double* S = series + (i - t_start);
-          auto put = [&](int m, double v) {
-            S[(u64)(2 * m) * ld] = v;
-            if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
-          };
-          put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
-          put(4, traced); put(5, wait); put(6, (double)pa); put(7, (double)pr);
-        }
+        certified_row(i, (u64)c0.x | ((u64)c0.y << 32), (u64)c0.z | ((u64)c0.w << 32),
+                      (u64)c1.x | ((u64)c1.y << 32), (u64)c1.z | ((u64)c1.w << 32),
+                      (u64)c2.x | ((u64)c2.y << 32), (u64)c2.z | ((u64)c2.w << 32),
+                      (u64)c3.x | ((u64)c3.y << 32), (u64)c3.z | ((u64)c3.w << 32));
       }
       __syncwarp();  // `cur` is free again
     }
@@ -2328,7 +2461,7 @@ struct tml_ctx {
   int n_sms = 132;
   u32 ring_slots = 0, proc_slots = 0, mirror_slots = 0, pmirror_slots = 0;
   DevState* d_state = nullptr;
-  StepRing ring = {nullptr, nullptr, nullptr, 0};  // one allocation: hot | cold | mem
+  StepRing ring = {nullptr, nullptr, nullptr, nullptr, 0};  // one allocation: hot | cold | packed | mem
   // tml_ring_load: two staging chunks (allocated on first use), the stream that fills them and
   // events for "chunk b copied" / "chunk b split, its buffer free"
   void* d_load_stage = nullptr;
@@ -2584,10 +2717,12 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
   CK(cudaMemset(c->d_state, 0, sizeof(DevState)));
   {
     char* p = nullptr;
-    CK(cudaMalloc(&p, (size_t)ring_slots * (sizeof(RingHot) + sizeof(RingCold) + 1) + RING_MEM_PAD));
+    const size_t per_slot = sizeof(RingHot) + sizeof(RingCold) + sizeof(RingPacked);
+    CK(cudaMalloc(&p, (size_t)ring_slots * (per_slot + 1) + RING_MEM_PAD));
     c->ring.hot = reinterpret_cast<RingHot*>(p);
     c->ring.cold = reinterpret_cast<RingCold*>(p + (size_t)ring_slots * sizeof(RingHot));
-    c->ring.mem = reinterpret_cast<u8*>(p + (size_t)ring_slots * (sizeof(RingHot) + sizeof(RingCold)));
+    c->ring.packed = reinterpret_cast<RingPacked*>(p + (size_t)ring_slots * (sizeof(RingHot) + sizeof(RingCold)));
+    c->ring.mem = reinterpret_cast<u8*>(p + (size_t)ring_slots * per_slot);
     c->ring.slots = ring_slots;
     CK(cudaMemset(c->ring.mem, 0, (size_t)ring_slots + RING_MEM_PAD));  // the pad is read, never used
   }
@@ -3246,11 +3381,13 @@ __global__ void k_set_heads(DevState* st, u64 head, u64 proc_head, int which) {
 
 // Public records -> the ring's halves and memory bytes: m records from `src` (device staging) into
 // the slots from pos0 on, ring wrap included (pos0 < slots, m <= slots).  One thread per 8-B word.
-// The thread of a record's step word also raises the certificate's marks for it (commit number
-// seq0 + its index); `pred`: the step id before the chunk's first record, has_pred = 0 if none.
+// The thread of a record's step word also writes its packed copy and raises the certificate's marks
+// for it (commit number seq0 + its index); `pred`: the step id before the chunk's first record,
+// has_pred = 0 if none.
+static_assert(ring_word(10) == 6 && ring_word(11) == 7, "public words 10, 11: the peaks");
 __global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, u64 pos0, DevState* st, u64 seq0,
                              u64 pred, u32 has_pred) {
-  u32 gap = 0, nomem = 0, unusable = 0;  // 1 + the chunk index of this thread's newest break, 0 = none
+  u32 gap = 0, nomem = 0, unusable = 0, wide = 0;  // 1 + the chunk index of this thread's newest break, 0 = none
   for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < m * 16; k += (u64)gridDim.x * blockDim.x) {
     const u64 r = k >> 4;
     u64 slot = pos0 + r;
@@ -3260,20 +3397,26 @@ __global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, 
     if (d < 8) reinterpret_cast<u64*>(&ring.hot[slot])[d] = v;
     else reinterpret_cast<u64*>(&ring.cold[slot])[d - 8] = v;
     if (w == RING_FLAGS_WORD) ring.mem[slot] = ((u32)(v >> 32) & TML_REC_HAS_MEM) ? 1 : 0;
-    if (w == 0) {  // public words: 1 dl, 3..6 fwd bwd opt wall, RING_FLAGS_WORD flags (high half)
+    if (w == 0) {  // public words: 1 dl, 3..6 fwd bwd opt wall, 10 11 peaks, RING_FLAGS_WORD flags (high half)
       const bool has_prev = r > 0 || has_pred != 0u;
       if (has_prev && !step_follows(r > 0 ? src[k - 16] : pred, v)) gap = (u32)r + 1u;
       if (!(((u32)(src[k + RING_FLAGS_WORD] >> 32)) & TML_REC_HAS_MEM)) nomem = (u32)r + 1u;
-      if ((src[k + 1] | src[k + 3] | src[k + 4] | src[k + 5] | src[k + 6]) == 0ull) unusable = (u32)r + 1u;
+      const u64 dl = src[k + 1], fwd = src[k + 3], bwd = src[k + 4], opt = src[k + 5], wall = src[k + 6];
+      const u64 pa = src[k + 10], pr = src[k + 11];
+      if ((dl | fwd | bwd | opt | wall) == 0ull) unusable = (u32)r + 1u;
+      if (pack_wide(dl, fwd, bwd, opt, wall, pa, pr)) wide = (u32)r + 1u;
+      ring.packed[slot] = pack_hot(dl, fwd, bwd, opt, wall, pa, pr);
     }
   }
   gap = __reduce_max_sync(0xffffffffu, gap);
   nomem = __reduce_max_sync(0xffffffffu, nomem);
   unusable = __reduce_max_sync(0xffffffffu, unusable);
+  wide = __reduce_max_sync(0xffffffffu, wide);
   if ((threadIdx.x & 31) == 0) {
     if (gap) atomicMax(&st->gap_mark, seq0 + gap);
     if (nomem) atomicMax(&st->nomem_mark, seq0 + nomem);
     if (unusable) atomicMax(&st->unusable_mark, seq0 + unusable);
+    if (wide) atomicMax(&st->wide_mark, seq0 + wide);
   }
 }
 
@@ -3302,17 +3445,33 @@ int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stre
   return TML_OK;
 }
 
-int tml_ring_certified_(tml_ctx* c, uint32_t window) {
-  if (!c || window == 0) return TML_ERR_ARG;
+// The verdicts k_window_fused reaches for the retained ring's last `window` rows: bit 0 certified,
+// bit 1 packed-streamable as well.
+static int ring_verdicts(tml_ctx* c, uint32_t window) {
   DeviceGuard dg(c);
-  u64 marks[3];
+  u64 marks[4];
   static_assert(offsetof(DevState, nomem_mark) == offsetof(DevState, gap_mark) + 8 &&
-                offsetof(DevState, unusable_mark) == offsetof(DevState, gap_mark) + 16, "marks are adjacent");
+                offsetof(DevState, unusable_mark) == offsetof(DevState, gap_mark) + 16 &&
+                offsetof(DevState, wide_mark) == offsetof(DevState, gap_mark) + 24, "marks are adjacent");
   CK(cudaDeviceSynchronize());
   CK(cudaMemcpy(marks, &c->d_state->gap_mark, sizeof(marks), cudaMemcpyDeviceToHost));
   DC_REFRESH(c);
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
-  return window_certified(marks[0], marks[1], marks[2], c->commits - n, n > window ? n - window : 0) ? 1 : 0;
+  const u64 first_k = c->commits - n;
+  if (!window_certified(marks[0], marks[1], marks[2], first_k, n > window ? n - window : 0)) return 0;
+  return window_packed(marks[3], first_k) ? 3 : 1;
+}
+
+int tml_ring_certified_(tml_ctx* c, uint32_t window) {
+  if (!c || window == 0) return TML_ERR_ARG;
+  const int v = ring_verdicts(c, window);
+  return v < 0 ? v : (v & 1);
+}
+
+int tml_ring_packed_(tml_ctx* c, uint32_t window) {
+  if (!c || window == 0) return TML_ERR_ARG;
+  const int v = ring_verdicts(c, window);
+  return v < 0 ? v : (v >> 1);
 }
 
 // The records arrive in the public AoS layout: each bounded chunk is copied into device staging on

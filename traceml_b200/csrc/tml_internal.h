@@ -45,6 +45,9 @@ uint64_t tml_ring_load_chunk_(void);
 // 1 if the ring's writers certify the retained ring's last `window` rows dense, else 0 (waits for
 // the device; tests compare it with the records)
 int tml_ring_certified_(tml_ctx* c, uint32_t window);
+// 1 if that window is certified and every retained record fits the ring's 32-B packed copy, so the
+// window pass streams the packed copies, else 0 (waits for the device)
+int tml_ring_packed_(tml_ctx* c, uint32_t window);
 
 #ifdef __cplusplus
 }

@@ -950,78 +950,255 @@ __device__ __forceinline__ u32 slot_next(u32 s, u32 adv, u32 slots) {
   return s >= slots - adv ? s - (slots - adv) : s + adv;
 }
 
-// K3a.  Persistent grid, WARP-PRIVATE software pipelines: every warp streams its own
-// 32-record tiles (cp.async, WR_STAGES buffers -> XOR-swizzled smem -> registers -> swizzled
-// smem -> coalesced 16-B stores) and synchronises only with __syncwarp; neighbour step
-// ids come from warp shuffles (tile edges: three small global reads).  No block barrier in
-// the loop (block barriers and waits dominate once the loads are asynchronous).
-__global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
-    StepRing ring, u64 first_k, u64 n, u64 t_start,
-    tml_window_row* __restrict__ rows, u64* __restrict__ steps, u8* __restrict__ flags,
-    WinAcc* acc, double* partials, double* __restrict__ csum, u64 csum_top) {
-  extern __shared__ __align__(16) unsigned char wr_smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WR_WARP_U4;
-  uint4* w_out = w_in + WR_STAGES * WR_STAGE_U4;
+__device__ __forceinline__ u64 u64_of(u32 lo, u32 hi) { return (u64)lo | ((u64)hi << 32); }
 
-  u64 a_lo0 = ~0ull, a_lo1 = ~0ull, a_hi0 = 0, a_hi1 = 0, a_latest = 0;
-  u32 a_nc0 = 0, a_nc1 = 0, a_nr0 = 0, a_nr1 = 0, a_viol = 0, a_dups = 0, a_tc = 0, a_both = 0;
-  u64 a_sa = 0, a_sr = 0;                        // exact integer byte sums (window rows)
+// record `lane` of a landed tile of hot halves (ring_issue_tile's swizzle): its step id and words 1..7
+// (dl, fwd, bwd, opt, wall, peak_alloc, peak_resv: unpack_hot's order)
+struct HotRow {
+  u64 step;
+  u64 w[7];
+};
+__device__ __forceinline__ HotRow hot_row(const uint4* stage, int lane) {
+  const int sw = (lane >> 1) & 3;
+  const uint4 c0 = stage[lane * 4 + (0 ^ sw)], c1 = stage[lane * 4 + (1 ^ sw)];
+  const uint4 c2 = stage[lane * 4 + (2 ^ sw)], c3 = stage[lane * 4 + (3 ^ sw)];
+  return {u64_of(c0.x, c0.y),
+          {u64_of(c0.z, c0.w), u64_of(c1.x, c1.y), u64_of(c1.z, c1.w), u64_of(c2.x, c2.y), u64_of(c2.z, c2.w),
+           u64_of(c3.x, c3.y), u64_of(c3.z, c3.w)}};
+}
+
+// a row's five summarised phases in ms and the two times model.py:241-247 derives from them
+struct RowMs {
+  double dl, fwd, bwd, opt, wall;
+  double compute, traced;
+};
+__device__ __forceinline__ RowMs row_ms(const u64 (&w)[7]) {
+  RowMs t;
+  t.dl = ns_to_ms(w[0]); t.fwd = ns_to_ms(w[1]); t.bwd = ns_to_ms(w[2]);
+  t.opt = ns_to_ms(w[3]); t.wall = ns_to_ms(w[4]);
+  t.compute = (t.fwd + t.bwd) + t.opt;
+  t.traced = fmax(t.wall, t.compute);
+  return t;
+}
+
+// A general tile's edge neighbours, straight from the ring: lane 0 gets the step id before the tile,
+// lane 31 the step id and memory byte after it.
+struct TileHalo {
+  u64 step = 0;
+  u32 mem = 0;
+};
+__device__ __forceinline__ TileHalo tile_halo(const StepRing& ring, u64 n, u64 base, u32 slot_tile, int lane) {
+  TileHalo h;
+  if (lane == 0 && base > 0) h.step = ring.hot[slot_tile == 0 ? ring.slots - 1 : slot_tile - 1].step;
+  if (lane == 31 && base + 32 < n) {
+    u64 hs = (u64)slot_tile + 32;
+    while (hs >= ring.slots) hs -= ring.slots;
+    h.step = ring.hot[hs].step; h.mem = ring.mem[hs];
+  }
+  return h;
+}
+
+// record `lane` of a landed general tile: its hot half and memory byte, the step id of the row before
+// it and the step id and memory byte of the row after it (warp shuffles; the halo at the tile's edges)
+struct TileRow : HotRow {
+  u32 mem;
+  u64 prev_step, next_step;
+  u32 next_mem;
+};
+__device__ __forceinline__ TileRow tile_row(const uint4* stage, const StepRing& ring, u64 n, u64 base,
+                                            u32 slot_tile, int lane, const TileHalo& halo) {
+  const HotRow h = hot_row(stage, lane);
+  const u32 mem = tile_mem(stage, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
+  TileRow r{h, mem, __shfl_up_sync(0xffffffffu, h.step, 1), __shfl_down_sync(0xffffffffu, h.step, 1),
+            __shfl_down_sync(0xffffffffu, mem, 1)};
+  if (lane == 0) r.prev_step = halo.step;
+  if (lane == 31) { r.next_step = halo.step; r.next_mem = halo.mem; }
+  return r;
+}
+
+// One thread's share of a window pass's results, in registers until flush(): the bounds and counts of
+// the time (0) and memory (1) candidates and the other WinAcc counters, the window rows' exact byte
+// sums and peaks, and the 7 time sums.  Each sum takes the thread's rows in the order warp_tiles
+// hands them out.
+struct WinTally {
+  u64 lo[2] = {~0ull, ~0ull}, hi[2] = {0, 0}, latest = 0;
+  u32 nc[2] = {0, 0}, nr[2] = {0, 0}, viol = 0, dups = 0, tc = 0, both = 0;
+  u64 msum[2] = {0, 0};                           // exact integer byte sums (window rows)
   double sums[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};  // 7 time sums (tree order) + 2 unused columns
-  double mx_a = -INFINITY, mx_r = -INFINITY;      // rank peaks over the window rows
+  double mx[2] = {-INFINITY, -INFINITY};          // rank peaks over the window rows
+
+  __device__ __forceinline__ void cand(int k, u64 step) {
+    lo[k] = step < lo[k] ? step : lo[k];
+    hi[k] = step > hi[k] ? step : hi[k];
+  }
+  // a usable window row (model.py:241-271, same expression order)
+  __device__ __forceinline__ void add_times(const RowMs& t) {
+    sums[0] += t.dl; sums[1] += t.fwd; sums[2] += t.bwd; sums[3] += t.opt;
+    sums[4] += t.wall; sums[5] += t.traced; sums[6] += t.dl + t.traced;
+  }
+  __device__ __forceinline__ void add_mem(u64 pa, u64 pr) {
+    msum[0] += pa; msum[1] += pr;
+    mx[0] = fmax(mx[0], (double)pa); mx[1] = fmax(mx[1], (double)pr);
+  }
+
+  // A row of a certified window: the first of its step id, with memory and a successor with a new
+  // id, so a memory candidate, and inside the time window a usable time candidate.  `t` is read only
+  // there.
+  __device__ __forceinline__ void certified_row(u64 step, bool in_time, const RowMs& t, u64 pa, u64 pr) {
+    latest = step > latest ? step : latest;
+    cand(1, step);
+    ++nr[1];
+    if (in_time) {
+      cand(0, step);
+      ++nr[0];
+      add_times(t);
+      add_mem(pa, pr);
+    }
+  }
+  // after a certified window's last row: the counts certified_row leaves implied
+  __device__ __forceinline__ void certified_done() {
+    nc[0] = tc = both = nr[0];
+    nc[1] = nr[1];
+  }
+  // window row i of a general tile; cand_t / cand_m: the caller's time / memory candidate verdicts
+  __device__ __forceinline__ void general_row(const TileRow& r, u64 i, bool in_time, bool usable, bool cand_t,
+                                              bool cand_m, const RowMs& t) {
+    latest = r.step > latest ? r.step : latest;
+    viol += (i > 0 && r.step < r.prev_step) ? 1u : 0u;
+    dups += (i > 0 && r.step == r.prev_step) ? 1u : 0u;
+    nr[0] += in_time ? 1u : 0u;
+    nr[1] += r.mem != 0u ? 1u : 0u;
+    if (cand_t) { cand(0, r.step); ++nc[0]; }
+    if (cand_m) { cand(1, r.step); ++nc[1]; }
+    both += (cand_t && cand_m) ? 1u : 0u;
+    if (usable && in_time) { add_times(t); ++tc; }
+    if (in_time) add_mem(r.w[5], r.w[6]);
+  }
+
+  // The pass's epilogue, by every thread of the CTA after its last tile: the bounds and counters go to
+  // `acc` (one atomic per warp and field), the time sums to the CTA's partial columns 0..8 and the two
+  // peaks to columns 9, 10.
+  __device__ __forceinline__ void flush(WinAcc* acc, double* partials) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) {
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        u64 t;
+        t = __shfl_xor_sync(0xffffffffu, lo[k], m); lo[k] = t < lo[k] ? t : lo[k];
+        t = __shfl_xor_sync(0xffffffffu, hi[k], m); hi[k] = t > hi[k] ? t : hi[k];
+        msum[k] += __shfl_xor_sync(0xffffffffu, msum[k], m);
+      }
+      const u64 t = __shfl_xor_sync(0xffffffffu, latest, m);
+      latest = t > latest ? t : latest;
+    }
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+      nc[k] = __reduce_add_sync(0xffffffffu, nc[k]);
+      nr[k] = __reduce_add_sync(0xffffffffu, nr[k]);
+    }
+    viol = __reduce_add_sync(0xffffffffu, viol); dups = __reduce_add_sync(0xffffffffu, dups);
+    tc = __reduce_add_sync(0xffffffffu, tc); both = __reduce_add_sync(0xffffffffu, both);
+    if (lane == 0) {
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        if (nc[k]) { atomicMin(&acc->lo[k], lo[k]); atomicMax(&acc->hi[k], hi[k]); atomicAdd(&acc->ncand[k], (u64)nc[k]); }
+        if (nr[k]) atomicAdd(&acc->nrows[k], (u64)nr[k]);
+        if (msum[k]) atomicAdd(&acc->msum[k], msum[k]);
+      }
+      atomicMax(&acc->latest_step, latest);
+      if (viol) atomicAdd(&acc->violations, (u64)viol);
+      if (dups) atomicAdd(&acc->dups, (u64)dups);
+      if (tc) atomicAdd(&acc->t_count, (u64)tc);
+      if (both) atomicAdd(&acc->n_both, (u64)both);
+    }
+    __syncthreads();
+    block_sum<9, WR_THREADS>(sums, partials + (size_t)blockIdx.x * 11);
+    // the two maxima: warp shuffle + shared memory
+    __shared__ double s_mx[WR_WARPS][2];
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) {
+      mx[0] = fmax(mx[0], shfl_xor_f64(mx[0], m));
+      mx[1] = fmax(mx[1], shfl_xor_f64(mx[1], m));
+    }
+    if (lane == 0) { s_mx[warp][0] = mx[0]; s_mx[warp][1] = mx[1]; }
+    __syncthreads();
+    if (tid < 2) {
+      double x = -INFINITY;
+      for (int w = 0; w < WR_WARPS; ++w) x = fmax(x, s_mx[w][tid]);
+      partials[(size_t)blockIdx.x * 11 + 9 + tid] = x;
+    }
+  }
+};
+
+// One warp's software pipeline over its 32-record tiles of the retained rows [0, n) (ring slot of row
+// 0: first_k % slots), private to the warp: it synchronises only with __syncwarp.  Warp w of CTA b takes
+// tiles b * WR_WARPS + w, then every gridDim.x * WR_WARPS-th; STAGES - 1 tiles stay in flight while
+// one is consumed.  Every window pass walks its tiles through here, so the tile -> warp -> CTA
+// mapping and each lane's order of rows are the same in all of them.
+//   issue: ring_issue_tile<H2D, MEM> or packed_issue_tile, into stages of STAGE_U4 uint4s
+//   HALO:  load each tile's tile_halo after the tile ahead is issued and before this tile is waited
+//          on, so those loads overlap the tiles in flight
+//   body(stage, base, slot_tile, halo): the landed tile of window rows base.., ring slots slot_tile..
+template <int STAGES, int STAGE_U4, bool HALO, class Issue, class Body>
+__device__ __forceinline__ void warp_tiles(uint4* w_in, const StepRing& ring, u64 first_k, u64 n, Issue issue,
+                                           Body body) {
+  const int lane = threadIdx.x & 31;
   const u64 nwt = (n + 31) / 32;
   const u64 wstride = (u64)gridDim.x * WR_WARPS;
   const u32 ring_slots = ring.slots;
-  uint4* rows4 = reinterpret_cast<uint4*>(rows);
-
-  u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
+  u64 wt = (u64)blockIdx.x * WR_WARPS + (threadIdx.x >> 5);
   // ring slots of this warp's current tile and of the next tile to issue, and the per-trip advance,
   // all kept < ring_slots: two 64-bit modulos per warp for the whole kernel instead of one per lane per tile
   u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
   const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
   u32 slot_iss = slot_cur;
 #pragma unroll
-  for (int s = 0; s < WR_STAGES - 1; ++s) {
+  for (int s = 0; s < STAGES - 1; ++s) {
     const u64 t = wt + (u64)s * wstride;
-    if (t < nwt) ring_issue_tile<true>(w_in + s * WR_STAGE_U4, ring, slot_iss, n, t * 32, lane);
+    if (t < nwt) issue(w_in + s * STAGE_U4, ring, slot_iss, n, t * 32, lane);
     cp_async_commit();
     slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
   }
-
   for (int it = 0; wt < nwt; wt += wstride, ++it) {
-    uint4* cur = w_in + (it % WR_STAGES) * WR_STAGE_U4;
+    const uint4* cur = w_in + (it % STAGES) * STAGE_U4;
     const u64 base = wt * 32;
-    const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
-    if (ahead < nwt)
-      ring_issue_tile<true>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WR_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
+    const u64 ahead = wt + (u64)(STAGES - 1) * wstride;
+    if (ahead < nwt) issue(w_in + ((it + STAGES - 1) % STAGES) * STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
     cp_async_commit();
     slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-    const u32 slot_tile = slot_cur;  // ring slot of this tile's first record
-    // tile-edge neighbours (first/last-of-step tests) straight from the ring
-    u64 halo_step = 0;
-    u32 halo_mem = 0;
-    if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
-    if (lane == 31 && base + 32 < n) {
-      u64 hs = (u64)slot_cur + 32;
-      while (hs >= ring_slots) hs -= ring_slots;
-      halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
-    }
+    const u32 slot_tile = slot_cur;
+    const TileHalo halo = HALO ? tile_halo(ring, n, base, slot_tile, lane) : TileHalo{};
     slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
-    cp_async_wait<WR_STAGES - 1>();  // this tile has landed; the next ones stay in flight
+    cp_async_wait<STAGES - 1>();  // this tile has landed; the next ones stay in flight
     __syncwarp();
+    body(cur, base, slot_tile, halo);
+    __syncwarp();  // `cur` is free again
+  }
+  cp_async_wait<0>();
+}
 
+// K3a.  Persistent grid of warp_tiles pipelines: every warp streams its own 32-record tiles
+// (cp.async, WR_STAGES buffers -> XOR-swizzled smem -> registers -> swizzled smem -> coalesced 16-B
+// stores); neighbour step ids come from warp shuffles (tile edges: three small global reads).  No
+// block barrier in the loop (block barriers and waits dominate once the loads are asynchronous).
+__global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
+    StepRing ring, u64 first_k, u64 n, u64 t_start,
+    tml_window_row* __restrict__ rows, u64* __restrict__ steps, u8* __restrict__ flags,
+    WinAcc* acc, double* partials, double* __restrict__ csum, u64 csum_top) {
+  extern __shared__ __align__(16) unsigned char wr_smem[];
+  const int lane = threadIdx.x & 31;
+  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + (threadIdx.x >> 5) * WR_WARP_U4;
+  uint4* w_out = w_in + WR_STAGES * WR_STAGE_U4;
+  uint4* rows4 = reinterpret_cast<uint4*>(rows);
+  WinTally tally;
+
+  warp_tiles<WR_STAGES, WR_STAGE_U4, true>(w_in, ring, first_k, n, ring_issue_tile<true>,
+                                           [&](const uint4* cur, u64 base, u32 slot_tile, const TileHalo& halo) {
     const u64 i = base + (u64)lane;
     const bool live = i < n;
-    const int sw = (lane >> 1) & 3;
-    const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
-    const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
-    const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
-    const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-    u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
-    u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
-    u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
-    if (lane == 0) prev_step = halo_step;
-    if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
+    const TileRow rec = tile_row(cur, ring, n, base, slot_tile, lane, halo);
+    const u64 step = rec.step;
     double t_dl = 0.0, t_fwd = 0.0, t_bwd = 0.0, t_opt = 0.0, t_wall = 0.0, t_tr = 0.0;  // K3e chunk sums
 
     // Time candidate: the OLDEST USABLE row of its step id inside the window.  The reference reads the
@@ -1029,20 +1206,18 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     // step (model.py:226-248), so a step whose oldest row is unusable is kept through a newer row.
     // A run of one step id is contiguous in a monotone ring; runs are cut at t_start.
     const bool uit_row = live && i >= t_start &&
-                         ((((u64)c0.z | ((u64)c0.w << 32)) | ((u64)c1.x | ((u64)c1.y << 32)) |
-                           ((u64)c1.z | ((u64)c1.w << 32)) | ((u64)c2.x | ((u64)c2.y << 32)) |
-                           ((u64)c2.z | ((u64)c2.w << 32))) != 0ull);  // usable: a summarised phase > 0 ns
-    const u32 heads = __ballot_sync(0xffffffffu, lane == 0 || i == t_start || prev_step != step);
+                         (rec.w[0] | rec.w[1] | rec.w[2] | rec.w[3] | rec.w[4]) != 0ull;  // usable: a summarised phase > 0 ns
+    const u32 heads = __ballot_sync(0xffffffffu, lane == 0 || i == t_start || rec.prev_step != step);
     const u32 uits = __ballot_sync(0xffffffffu, uit_row);
     const int head = 31 - __clz(heads & (0xffffffffu >> (31 - lane)));  // lane where this row's run starts
     bool older_usable = (uits & ((1u << lane) - 1u) & ~((1u << head) - 1u)) != 0u;
     {
       bool carry = false;  // the run of lane 0 began in an earlier tile: a usable window row before it?
-      if (lane == 0 && live && base > t_start && prev_step == step) {
+      if (lane == 0 && live && base > t_start && rec.prev_step == step) {
         u64 j = base, sl = slot_tile;
         while (j > t_start) {
           --j;
-          sl = sl == 0 ? ring_slots - 1 : sl - 1;
+          sl = sl == 0 ? ring.slots - 1 : sl - 1;
           const RingHot* p = &ring.hot[sl];
           if (p->step != step) break;
           if ((p->dl | p->fwd | p->bwd | p->opt | p->wall) != 0ull) { carry = true; break; }
@@ -1053,22 +1228,14 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
     }
 
     if (live) {
-      const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
-      const u64 d1 = reinterpret_cast<const u64*>(cur + TILE_HOT_U4 + TILE_MEM_U4)[lane];
-      const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
-      const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
-      const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
-      const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
-      const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
-      const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
-      const double dl = ns_to_ms(d0), h2d = ns_to_ms(d1), fwd = ns_to_ms(d2);
-      const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
-      const bool has_mem = rmem != 0u;
-      const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
+      const RowMs t = row_ms(rec.w);
+      const double h2d = ns_to_ms(reinterpret_cast<const u64*>(cur + TILE_HOT_U4 + TILE_MEM_U4)[lane]);
+      const u64 pa = rec.w[5], pr = rec.w[6];
+      const bool has_mem = rec.mem != 0u;
+      const bool usable = (t.dl > 0.0) || (t.fwd > 0.0) || (t.bwd > 0.0) || (t.opt > 0.0) || (t.wall > 0.0);
       const bool in_time = i >= t_start;
       const bool uit = usable && in_time;
-      const bool has_prev = i > 0, has_next = (i + 1) < n;
-      const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
+      const bool last_m = (i + 1) >= n || (rec.next_step != step) || rec.next_mem == 0u;
       u8 f = 0;
       if (usable) f |= RF_USABLE;
       if (has_mem) f |= RF_HAS_MEM;
@@ -1079,34 +1246,14 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
       if (cand_m) f |= RF_CAND_M;
       steps[i] = step;
       flags[i] = f;
+      tally.general_row(rec, i, in_time, usable, cand_t, cand_m, t);
 
-      a_latest = step > a_latest ? step : a_latest;
-      a_viol += (has_prev && step < prev_step) ? 1u : 0u;
-      a_dups += (has_prev && step == prev_step) ? 1u : 0u;
-      a_nr0 += in_time ? 1u : 0u;
-      a_nr1 += has_mem ? 1u : 0u;
-      if (cand_t) { a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0; ++a_nc0; }
-      if (cand_m) { a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1; ++a_nc1; }
-      a_both += (cand_t && cand_m) ? 1u : 0u;
-
-      if (usable && in_time) {  // model.py:241-271, same expression order
-        const double compute = (fwd + bwd) + opt;
-        const double traced = fmax(wall, compute);
-        sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
-        sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
-        ++a_tc;
-      }
-      if (in_time) {
-        a_sa += pa; a_sr += pr;
-        mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
-      }
-
-      if (csum) { t_dl = uit ? dl : 0.0; t_fwd = uit ? fwd : 0.0; t_bwd = uit ? bwd : 0.0; t_opt = uit ? opt : 0.0;
-                  t_wall = uit ? wall : 0.0; t_tr = uit ? fmax(wall, (fwd + bwd) + opt) : 0.0; }
+      if (csum) { t_dl = uit ? t.dl : 0.0; t_fwd = uit ? t.fwd : 0.0; t_bwd = uit ? t.bwd : 0.0;
+                  t_opt = uit ? t.opt : 0.0; t_wall = uit ? t.wall : 0.0; t_tr = uit ? t.traced : 0.0; }
 
       // row -> swizzled staging (4 x 16 B)
-      double2 o0 = make_double2(dl, h2d), o1 = make_double2(fwd, bwd);
-      double2 o2 = make_double2(opt, wall), o3 = make_double2((double)pa, (double)pr);
+      double2 o0 = make_double2(t.dl, h2d), o1 = make_double2(t.fwd, t.bwd);
+      double2 o2 = make_double2(t.opt, t.wall), o3 = make_double2((double)pa, (double)pr);
       const int so = (lane >> 1) & 3;
       w_out[lane * 4 + (0 ^ so)] = *reinterpret_cast<uint4*>(&o0);
       w_out[lane * 4 + (1 ^ so)] = *reinterpret_cast<uint4*>(&o1);
@@ -1166,55 +1313,8 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
         if (ii < n) rows4[ii * 4 + q] = w_out[r * 4 + (q ^ ((r >> 1) & 3))];
       }
     }
-    __syncwarp();  // w_out and `cur` are free again
-  }
-  cp_async_wait<0>();
-  {
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      u64 t;
-      t = __shfl_xor_sync(0xffffffffu, a_lo0, m); a_lo0 = t < a_lo0 ? t : a_lo0;
-      t = __shfl_xor_sync(0xffffffffu, a_lo1, m); a_lo1 = t < a_lo1 ? t : a_lo1;
-      t = __shfl_xor_sync(0xffffffffu, a_hi0, m); a_hi0 = t > a_hi0 ? t : a_hi0;
-      t = __shfl_xor_sync(0xffffffffu, a_hi1, m); a_hi1 = t > a_hi1 ? t : a_hi1;
-      t = __shfl_xor_sync(0xffffffffu, a_latest, m); a_latest = t > a_latest ? t : a_latest;
-      a_sa += __shfl_xor_sync(0xffffffffu, a_sa, m); a_sr += __shfl_xor_sync(0xffffffffu, a_sr, m);
-    }
-    a_nc0 = __reduce_add_sync(0xffffffffu, a_nc0); a_nc1 = __reduce_add_sync(0xffffffffu, a_nc1);
-    a_nr0 = __reduce_add_sync(0xffffffffu, a_nr0); a_nr1 = __reduce_add_sync(0xffffffffu, a_nr1);
-    a_viol = __reduce_add_sync(0xffffffffu, a_viol); a_dups = __reduce_add_sync(0xffffffffu, a_dups);
-    a_tc = __reduce_add_sync(0xffffffffu, a_tc); a_both = __reduce_add_sync(0xffffffffu, a_both);
-    if (lane == 0) {
-      if (a_nc0) { atomicMin(&acc->lo[0], a_lo0); atomicMax(&acc->hi[0], a_hi0); atomicAdd(&acc->ncand[0], (u64)a_nc0); }
-      if (a_nc1) { atomicMin(&acc->lo[1], a_lo1); atomicMax(&acc->hi[1], a_hi1); atomicAdd(&acc->ncand[1], (u64)a_nc1); }
-      if (a_nr0) atomicAdd(&acc->nrows[0], (u64)a_nr0);
-      if (a_nr1) atomicAdd(&acc->nrows[1], (u64)a_nr1);
-      atomicMax(&acc->latest_step, a_latest);
-      if (a_viol) atomicAdd(&acc->violations, (u64)a_viol);
-      if (a_dups) atomicAdd(&acc->dups, (u64)a_dups);
-      if (a_tc) atomicAdd(&acc->t_count, (u64)a_tc);
-      if (a_both) atomicAdd(&acc->n_both, (u64)a_both);
-      if (a_sa) atomicAdd(&acc->msum[0], a_sa);
-      if (a_sr) atomicAdd(&acc->msum[1], a_sr);
-    }
-  }
-  __syncthreads();
-  block_sum<9, WR_THREADS>(sums, partials + (size_t)blockIdx.x * 11);
-  {  // the two maxima: warp shuffle + shared memory, written as partial columns 9, 10
-    __shared__ double s_mx[WR_THREADS / 32][2];
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      mx_a = fmax(mx_a, shfl_xor_f64(mx_a, m));
-      mx_r = fmax(mx_r, shfl_xor_f64(mx_r, m));
-    }
-    if (lane == 0) { s_mx[warp][0] = mx_a; s_mx[warp][1] = mx_r; }
-    __syncthreads();
-    if (tid < 2) {
-      double x = -INFINITY;
-      for (int w = 0; w < WR_THREADS / 32; ++w) x = fmax(x, s_mx[w][tid]);
-      partials[(size_t)blockIdx.x * 11 + 9 + tid] = x;
-    }
-  }
+  });  // warp_tiles' closing __syncwarp frees w_out too
+  tally.flush(acc, partials);
 }
 
 
@@ -1224,10 +1324,9 @@ __global__ void __launch_bounds__(WR_THREADS, 2) k_window_rows(
 // per-step series can be written straight from the ring records: 65 B in (the hot half and the memory
 // byte; 32 B from the packed copies of a packed-streamable window), 128 B out per step, and
 // the 64-B WindowRows -- written by K3a only to be re-read by K4 (256 MB each way at
-// W = 4e6) -- never exist.  Same warp-private
-// cp.async pipeline as k_window_rows; lane = record, so each of the 16 series receives 32
+// W = 4e6) -- never exist.  Lane = record, so each of the 16 series receives 32
 // consecutive doubles per tile: 256-B fully coalesced stores, no staging buffer.  Bounds, counters,
-// tree sums and maxima are produced as in k_window_rows, except that a time candidate is simply the
+// tree sums and maxima are those of k_window_rows, except that a time candidate is simply the
 // oldest row of its step id in the window: the two rules differ only where a step id repeats, and
 // such a window is never dense under either.  The host accepts the series only
 // if the window turns out dense (every row a candidate of both kinds, consecutive step ids),
@@ -1280,9 +1379,8 @@ __device__ __forceinline__ void packed_issue_tile(uint4* stage, const StepRing& 
 // this in general are not needed.  When every retained record also fits its packed copy
 // (window_packed) the stream reads the 32-B packed records and takes the step ids from the first
 // retained row's (certified: they rise by exactly 1 per row); otherwise it reads the 64-B hot
-// halves.  Both streams share the per-row code, and their tile -> warp -> CTA mapping and each
-// lane's order of additions are those of the general loop, so sums, maxima and counters are
-// bit-identical.  Any other window takes the general loop.
+// halves.  Any other window takes the general loop.  All three walk the tiles with warp_tiles and
+// add into a WinTally, so sums, maxima and counters are the same bits whichever one runs.
 template <bool PAIRED>
 __global__ void __maxnreg__(94) k_window_fused(
     StepRing ring, u64 first_k, u64 n, u64 t_start,
@@ -1290,272 +1388,81 @@ __global__ void __maxnreg__(94) k_window_fused(
   extern __shared__ __align__(16) unsigned char wr_smem[];
   __shared__ u32 s_mode;  // 0: general, 1: certified (hot halves), 2: certified and packed
   __shared__ u64 s_step0;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + warp * WF_WARP_U4;
-
-  u64 a_lo0 = ~0ull, a_lo1 = ~0ull, a_hi0 = 0, a_hi1 = 0, a_latest = 0;
-  u32 a_nc0 = 0, a_nc1 = 0, a_nr0 = 0, a_nr1 = 0, a_viol = 0, a_dups = 0, a_tc = 0, a_both = 0;
-  u64 a_sa = 0, a_sr = 0;
-  double sums[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  double mx_a = -INFINITY, mx_r = -INFINITY;
-  const u64 nwt = (n + 31) / 32;
-  const u64 wstride = (u64)gridDim.x * WR_WARPS;
-  const u32 ring_slots = ring.slots;
+  const int tid = threadIdx.x, lane = tid & 31;
+  uint4* w_in = reinterpret_cast<uint4*>(wr_smem) + (tid >> 5) * WF_WARP_U4;
+  WinTally tally;
 
   if (tid == 0) {
     u32 mode = window_certified(st->gap_mark, st->nomem_mark, st->unusable_mark, first_k, t_start) ? 1u : 0u;
     if (mode && window_packed(st->wide_mark, first_k)) {
       mode = 2u;
-      s_step0 = ring.hot[first_k % ring_slots].step;
+      s_step0 = ring.hot[first_k % ring.slots].step;
     }
     s_mode = mode;
   }
   __syncthreads();
+  // window row i's series values; one rank: median == worst == the value (adapters.py:92-139 with a
+  // single column)
+  auto put_series = [&](u64 i, const RowMs& t, u64 pa, u64 pr) {
+    double* S = series + (i - t_start);
+    auto put = [&](int m, double v) {  // metric m: median row 2m, worst row 2m+1
+      S[(u64)(2 * m) * ld] = v;
+      if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
+    };
+    put(0, t.dl); put(1, t.fwd); put(2, t.bwd); put(3, t.opt);
+    put(4, t.traced); put(5, fmax(0.0, t.traced - t.compute));  // model.py:247
+    put(6, (double)pa); put(7, (double)pr);
+  };
   // one certified row: row i of the window with step id `step` and the hot half's words 1..7
-  auto certified_row = [&](u64 i, u64 step, u64 d0, u64 d2, u64 d3, u64 d4, u64 d5, u64 pa, u64 pr) {
-    a_latest = step > a_latest ? step : a_latest;
-    a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1;
-    ++a_nr1;  // a memory candidate
-    if (i >= t_start) {  // a time candidate, usable
-      const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
-      const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4);
-      const double wall = ns_to_ms(d5);
-      a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0;
-      ++a_nr0;
-      const double compute = (fwd + bwd) + opt;
-      const double traced = fmax(wall, compute);
-      sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
-      sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
-      a_sa += pa; a_sr += pr;
-      mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
-      const double wait = fmax(0.0, traced - compute);
-      double* S = series + (i - t_start);
-      auto put = [&](int m, double v) {
-        S[(u64)(2 * m) * ld] = v;
-        if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
-      };
-      put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
-      put(4, traced); put(5, wait); put(6, (double)pa); put(7, (double)pr);
-    }
+  auto certified_row = [&](u64 i, u64 step, const u64 (&w)[7]) {
+    const bool in_time = i >= t_start;
+    const RowMs t = row_ms(w);
+    tally.certified_row(step, in_time, t, w[5], w[6]);
+    if (in_time) put_series(i, t, w[5], w[6]);
   };
   if (s_mode == 2u) {
     const u64 step0 = s_step0;
-    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
-    u32 slot_iss = (u32)((first_k + wt * 32) % ring_slots);
-#pragma unroll
-    for (int s = 0; s < PK_STAGES - 1; ++s) {
-      const u64 t = wt + (u64)s * wstride;
-      if (t < nwt) packed_issue_tile(w_in + s * TILE_PK_U4, ring, slot_iss, n, t * 32, lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-    }
-    for (int it = 0; wt < nwt; wt += wstride, ++it) {
-      const uint4* cur = w_in + (it % PK_STAGES) * TILE_PK_U4;
-      const u64 base = wt * 32;
-      const u64 ahead = wt + (u64)(PK_STAGES - 1) * wstride;
-      if (ahead < nwt)
-        packed_issue_tile(w_in + ((it + PK_STAGES - 1) % PK_STAGES) * TILE_PK_U4, ring, slot_iss, n, ahead * 32,
-                          lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-      cp_async_wait<PK_STAGES - 1>();
-      __syncwarp();
+    warp_tiles<PK_STAGES, TILE_PK_U4, false>(w_in, ring, first_k, n, packed_issue_tile,
+                                             [&](const uint4* cur, u64 base, u32, const TileHalo&) {
       const u64 i = base + (u64)lane;
       if (i < n) {
         const int sw = (lane >> 2) & 1;
         const uint4 p0 = cur[lane * 2 + sw], p1 = cur[lane * 2 + (sw ^ 1)];
-        u64 v[7];
-        unpack_hot((u64)p0.x | ((u64)p0.y << 32), (u64)p0.z | ((u64)p0.w << 32),
-                   (u64)p1.x | ((u64)p1.y << 32), (u64)p1.z | ((u64)p1.w << 32), v);
-        certified_row(i, step0 + i, v[0], v[1], v[2], v[3], v[4], v[5], v[6]);
+        u64 w[7];
+        unpack_hot(u64_of(p0.x, p0.y), u64_of(p0.z, p0.w), u64_of(p1.x, p1.y), u64_of(p1.z, p1.w), w);
+        certified_row(i, step0 + i, w);
       }
-      __syncwarp();  // `cur` is free again
-    }
-    a_nc0 = a_tc = a_both = a_nr0;
-    a_nc1 = a_nr1;
+    });
+    tally.certified_done();
   } else if (s_mode == 1u) {
-    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
-    u32 slot_iss = (u32)((first_k + wt * 32) % ring_slots);
-#pragma unroll
-    for (int s = 0; s < WR_STAGES - 1; ++s) {
-      const u64 t = wt + (u64)s * wstride;
-      if (t < nwt) ring_issue_tile<false, false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-    }
-    for (int it = 0; wt < nwt; wt += wstride, ++it) {
-      const uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
-      const u64 base = wt * 32;
-      const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
-      if (ahead < nwt)
-        ring_issue_tile<false, false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n,
-                                      ahead * 32, lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-      cp_async_wait<WR_STAGES - 1>();
-      __syncwarp();
+    warp_tiles<WR_STAGES, WF_STAGE_U4, false>(w_in, ring, first_k, n, ring_issue_tile<false, false>,
+                                              [&](const uint4* cur, u64 base, u32, const TileHalo&) {
       const u64 i = base + (u64)lane;
       if (i < n) {
-        const int sw = (lane >> 1) & 3;
-        const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
-        const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
-        certified_row(i, (u64)c0.x | ((u64)c0.y << 32), (u64)c0.z | ((u64)c0.w << 32),
-                      (u64)c1.x | ((u64)c1.y << 32), (u64)c1.z | ((u64)c1.w << 32),
-                      (u64)c2.x | ((u64)c2.y << 32), (u64)c2.z | ((u64)c2.w << 32),
-                      (u64)c3.x | ((u64)c3.y << 32), (u64)c3.z | ((u64)c3.w << 32));
+        const HotRow h = hot_row(cur, lane);
+        certified_row(i, h.step, h.w);
       }
-      __syncwarp();  // `cur` is free again
-    }
-    a_nc0 = a_tc = a_both = a_nr0;
-    a_nc1 = a_nr1;
+    });
+    tally.certified_done();
   } else {
-    u64 wt = (u64)blockIdx.x * WR_WARPS + warp;
-    u32 slot_cur = (u32)((first_k + wt * 32) % ring_slots);
-    const u32 slot_adv = (u32)((wstride * 32) % ring_slots);
-    u32 slot_iss = slot_cur;
-#pragma unroll
-    for (int s = 0; s < WR_STAGES - 1; ++s) {
-      const u64 t = wt + (u64)s * wstride;
-      if (t < nwt) ring_issue_tile<false>(w_in + s * WF_STAGE_U4, ring, slot_iss, n, t * 32, lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-    }
-
-    for (int it = 0; wt < nwt; wt += wstride, ++it) {
-      uint4* cur = w_in + (it % WR_STAGES) * WF_STAGE_U4;
-      const u64 base = wt * 32;
-      const u64 ahead = wt + (u64)(WR_STAGES - 1) * wstride;
-      if (ahead < nwt)
-        ring_issue_tile<false>(w_in + ((it + WR_STAGES - 1) % WR_STAGES) * WF_STAGE_U4, ring, slot_iss, n, ahead * 32, lane);
-      cp_async_commit();
-      slot_iss = slot_next(slot_iss, slot_adv, ring_slots);
-      const u32 slot_tile = slot_cur;
-      u64 halo_step = 0;
-      u32 halo_mem = 0;
-      if (lane == 0 && base > 0) halo_step = ring.hot[slot_cur == 0 ? ring_slots - 1 : slot_cur - 1].step;
-      if (lane == 31 && base + 32 < n) {
-        u64 hs = (u64)slot_cur + 32;
-        while (hs >= ring_slots) hs -= ring_slots;
-        halo_step = ring.hot[hs].step; halo_mem = ring.mem[hs];
-      }
-      slot_cur = slot_next(slot_cur, slot_adv, ring_slots);
-      cp_async_wait<WR_STAGES - 1>();
-      __syncwarp();
-
+    warp_tiles<WR_STAGES, WF_STAGE_U4, true>(w_in, ring, first_k, n, ring_issue_tile<false>,
+                                             [&](const uint4* cur, u64 base, u32 slot_tile, const TileHalo& halo) {
       const u64 i = base + (u64)lane;
-      const bool live = i < n;
-      const int sw = (lane >> 1) & 3;
-      const uint4 c0 = cur[lane * 4 + (0 ^ sw)], c1 = cur[lane * 4 + (1 ^ sw)];
-      const uint4 c2 = cur[lane * 4 + (2 ^ sw)], c3 = cur[lane * 4 + (3 ^ sw)];
-      const u32 rmem = tile_mem(cur, tile_linear(ring, slot_tile, n, base), slot_tile, lane);
-      const u64 step = (u64)c0.x | ((u64)c0.y << 32);
-      u64 prev_step = __shfl_up_sync(0xffffffffu, step, 1);
-      u64 next_step = __shfl_down_sync(0xffffffffu, step, 1);
-      u32 next_mem = __shfl_down_sync(0xffffffffu, rmem, 1);
-      if (lane == 0) prev_step = halo_step;
-      if (lane == 31) { next_step = halo_step; next_mem = halo_mem; }
-
-      if (live) {
-        const u64 d0 = (u64)c0.z | ((u64)c0.w << 32);
-        const u64 d2 = (u64)c1.x | ((u64)c1.y << 32);
-        const u64 d3 = (u64)c1.z | ((u64)c1.w << 32);
-        const u64 d4 = (u64)c2.x | ((u64)c2.y << 32);
-        const u64 d5 = (u64)c2.z | ((u64)c2.w << 32);
-        const u64 pa = (u64)c3.x | ((u64)c3.y << 32);
-        const u64 pr = (u64)c3.z | ((u64)c3.w << 32);
-        const double dl = ns_to_ms(d0), fwd = ns_to_ms(d2);
-        const double bwd = ns_to_ms(d3), opt = ns_to_ms(d4), wall = ns_to_ms(d5);
-        const bool has_mem = rmem != 0u;
-        const bool usable = (dl > 0.0) || (fwd > 0.0) || (bwd > 0.0) || (opt > 0.0) || (wall > 0.0);
+      const TileRow rec = tile_row(cur, ring, n, base, slot_tile, lane, halo);
+      if (i < n) {
+        const RowMs t = row_ms(rec.w);
+        const bool usable = (t.dl > 0.0) || (t.fwd > 0.0) || (t.bwd > 0.0) || (t.opt > 0.0) || (t.wall > 0.0);
         const bool in_time = i >= t_start;
-        const bool has_prev = i > 0, has_next = (i + 1) < n;
-        const bool first_in_win = (i == t_start) || !has_prev || (prev_step != step);
-        const bool last_m = !has_next || (next_step != step) || next_mem == 0u;
+        const bool first_in_win = (i == t_start) || i == 0 || (rec.prev_step != rec.step);
+        const bool last_m = (i + 1) >= n || (rec.next_step != rec.step) || rec.next_mem == 0u;
         const bool cand_t = usable && in_time && first_in_win;
-        const bool cand_m = has_mem && last_m;
-        a_latest = step > a_latest ? step : a_latest;
-        a_viol += (has_prev && step < prev_step) ? 1u : 0u;
-        a_dups += (has_prev && step == prev_step) ? 1u : 0u;
-        a_nr0 += in_time ? 1u : 0u;
-        a_nr1 += has_mem ? 1u : 0u;
-        if (cand_t) { a_lo0 = step < a_lo0 ? step : a_lo0; a_hi0 = step > a_hi0 ? step : a_hi0; ++a_nc0; }
-        if (cand_m) { a_lo1 = step < a_lo1 ? step : a_lo1; a_hi1 = step > a_hi1 ? step : a_hi1; ++a_nc1; }
-        a_both += (cand_t && cand_m) ? 1u : 0u;
-        const double compute = (fwd + bwd) + opt;
-        const double traced = fmax(wall, compute);      // model.py:246
-        if (usable && in_time) {
-          sums[0] += dl; sums[1] += fwd; sums[2] += bwd; sums[3] += opt;
-          sums[4] += wall; sums[5] += traced; sums[6] += dl + traced;
-          ++a_tc;
-        }
-        if (in_time) {
-          a_sa += pa; a_sr += pr;
-          mx_a = fmax(mx_a, (double)pa); mx_r = fmax(mx_r, (double)pr);
-          // one rank: median == worst == the value (adapters.py:92-139 with a single column)
-          const u64 j = i - t_start;
-          const double wait = fmax(0.0, traced - compute);  // model.py:247
-          const double va = (double)pa, vr = (double)pr;
-          double* S = series + j;
-          auto put = [&](int m, double v) {  // metric m: median row 2m, worst row 2m+1
-            S[(u64)(2 * m) * ld] = v;
-            if (!PAIRED) S[(u64)(2 * m + 1) * ld] = v;
-          };
-          put(0, dl); put(1, fwd); put(2, bwd); put(3, opt);
-          put(4, traced); put(5, wait); put(6, va); put(7, vr);
-        }
+        const bool cand_m = rec.mem != 0u && last_m;
+        tally.general_row(rec, i, in_time, usable, cand_t, cand_m, t);
+        if (in_time) put_series(i, t, rec.w[5], rec.w[6]);
       }
-      __syncwarp();  // `cur` is free again
-    }
+    });
   }
-  cp_async_wait<0>();
-  {
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      u64 t;
-      t = __shfl_xor_sync(0xffffffffu, a_lo0, m); a_lo0 = t < a_lo0 ? t : a_lo0;
-      t = __shfl_xor_sync(0xffffffffu, a_lo1, m); a_lo1 = t < a_lo1 ? t : a_lo1;
-      t = __shfl_xor_sync(0xffffffffu, a_hi0, m); a_hi0 = t > a_hi0 ? t : a_hi0;
-      t = __shfl_xor_sync(0xffffffffu, a_hi1, m); a_hi1 = t > a_hi1 ? t : a_hi1;
-      t = __shfl_xor_sync(0xffffffffu, a_latest, m); a_latest = t > a_latest ? t : a_latest;
-      a_sa += __shfl_xor_sync(0xffffffffu, a_sa, m); a_sr += __shfl_xor_sync(0xffffffffu, a_sr, m);
-    }
-    a_nc0 = __reduce_add_sync(0xffffffffu, a_nc0); a_nc1 = __reduce_add_sync(0xffffffffu, a_nc1);
-    a_nr0 = __reduce_add_sync(0xffffffffu, a_nr0); a_nr1 = __reduce_add_sync(0xffffffffu, a_nr1);
-    a_viol = __reduce_add_sync(0xffffffffu, a_viol); a_dups = __reduce_add_sync(0xffffffffu, a_dups);
-    a_tc = __reduce_add_sync(0xffffffffu, a_tc); a_both = __reduce_add_sync(0xffffffffu, a_both);
-    if (lane == 0) {
-      if (a_nc0) { atomicMin(&acc->lo[0], a_lo0); atomicMax(&acc->hi[0], a_hi0); atomicAdd(&acc->ncand[0], (u64)a_nc0); }
-      if (a_nc1) { atomicMin(&acc->lo[1], a_lo1); atomicMax(&acc->hi[1], a_hi1); atomicAdd(&acc->ncand[1], (u64)a_nc1); }
-      if (a_nr0) atomicAdd(&acc->nrows[0], (u64)a_nr0);
-      if (a_nr1) atomicAdd(&acc->nrows[1], (u64)a_nr1);
-      atomicMax(&acc->latest_step, a_latest);
-      if (a_viol) atomicAdd(&acc->violations, (u64)a_viol);
-      if (a_dups) atomicAdd(&acc->dups, (u64)a_dups);
-      if (a_tc) atomicAdd(&acc->t_count, (u64)a_tc);
-      if (a_both) atomicAdd(&acc->n_both, (u64)a_both);
-      if (a_sa) atomicAdd(&acc->msum[0], a_sa);
-      if (a_sr) atomicAdd(&acc->msum[1], a_sr);
-    }
-  }
-  __syncthreads();
-  block_sum<9, WR_THREADS>(sums, partials + (size_t)blockIdx.x * 11);
-  {
-    __shared__ double s_mx[WR_THREADS / 32][2];
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) {
-      mx_a = fmax(mx_a, shfl_xor_f64(mx_a, m));
-      mx_r = fmax(mx_r, shfl_xor_f64(mx_r, m));
-    }
-    if (lane == 0) { s_mx[warp][0] = mx_a; s_mx[warp][1] = mx_r; }
-    __syncthreads();
-    if (tid < 2) {
-      double x = -INFINITY;
-      for (int w = 0; w < WR_THREADS / 32; ++w) x = fmax(x, s_mx[w][tid]);
-      partials[(size_t)blockIdx.x * 11 + 9 + tid] = x;
-    }
-  }
+  tally.flush(acc, partials);
 }
 
 // ------------------------------------------------------------------ K3b: presence
@@ -3714,6 +3621,23 @@ static int select_finish(tml_ctx* c, int grid, const XsSrc* exact, bool selected
   return TML_OK;
 }
 
+// What a window pass (k_window_rows, k_window_fused) over n records needs before its launch: the
+// kernels' dynamic shared memory allowed (once per process), the events that time it (once per
+// context) and *grid: a CTA per WR_THREADS records, at most the 2 that stay resident per SM.
+static int window_pass_setup(tml_ctx* c, u64 n, int* grid) {
+  static bool attr = false;
+  if (!attr) {
+    CK(cudaFuncSetAttribute(k_window_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, WR_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    CK(cudaFuncSetAttribute(k_window_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
+    attr = true;
+  }
+  if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
+  *grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
+  if (*grid > c->n_sms * 2) *grid = c->n_sms * 2;
+  return TML_OK;
+}
+
 extern "C" {
 
 int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out) {
@@ -3755,14 +3679,9 @@ int tml_win_prepare(tml_ctx* c, uint32_t window, void* stream, tml_win_info* out
   memset(&init, 0, sizeof(init));
   init.lo[0] = init.lo[1] = ~0ull;
   CK(cudaMemcpyAsync(&c->d_final->win.acc, &init, sizeof(init), cudaMemcpyHostToDevice, s));
-  static bool wr_attr = false;
-  if (!wr_attr) {
-    CK(cudaFuncSetAttribute(k_window_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, WR_SMEM_BYTES));
-    wr_attr = true;
-  }
-  int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
-  if (grid > c->n_sms * 2) grid = c->n_sms * 2;  // 2 resident CTAs per SM (90 KB smem each)
-  if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
+  int grid = 0;
+  const int sr = window_pass_setup(c, n, &grid);
+  if (sr != TML_OK) return sr;
   // K3e (reference-order sums) needs approximate 256-row chunk sums for its plan: K3a has every row
   // in registers anyway and adds them up on the way (tml_exact_sum.cuh: X1 without a pass of its own)
   bool exact_win = c->world > 1 || (n - c->win_tstart) <= TML_EXACT_SUM_MAX;
@@ -3851,19 +3770,11 @@ static int fused_pass(tml_ctx* c, uint32_t window, double* series, u64 ld, bool 
   if (ld < n - t_start) return set_err(TML_ERR_ARG, "series row stride %llu below the window's %llu rows",
                                        (unsigned long long)ld, (unsigned long long)(n - t_start));
   if (c->xs_pending) { CK(cudaStreamWaitEvent(s, c->xs_done, 0)); c->xs_pending = false; }
-  static bool wf_attr = false;
-  if (!wf_attr) {
-    CK(cudaFuncSetAttribute(k_window_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
-    CK(cudaFuncSetAttribute(k_window_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, WF_SMEM_BYTES));
-    wf_attr = true;
-  }
-  int grid = (int)((n + WR_THREADS - 1) / WR_THREADS);
-  if (grid > c->n_sms * 2) grid = c->n_sms * 2;
-  *grid_out = grid;
-  if (!c->ev0) { CK(cudaEventCreate(&c->ev0)); CK(cudaEventCreate(&c->ev1)); }
+  const int sr = window_pass_setup(c, n, grid_out);
+  if (sr != TML_OK) return sr;
   CK(cudaEventRecord(c->ev0, s));
   auto* kern = paired ? k_window_fused<true> : k_window_fused<false>;
-  kern<<<grid, WR_THREADS, WF_SMEM_BYTES, s>>>(c->ring, first_k, n, t_start, series, ld,
+  kern<<<*grid_out, WR_THREADS, WF_SMEM_BYTES, s>>>(c->ring, first_k, n, t_start, series, ld,
                                                &c->d_final->chain_acc, c->d_partials, c->d_state);
   CK(cudaPeekAtLastError());
   CK(cudaEventRecord(c->ev1, s));

@@ -71,7 +71,7 @@ struct RingCold {
 // A 32-B copy of the hot half without the step id, as one 256-bit little-endian bit string:
 // dl [0,36) fwd [36,72) bwd [72,108) opt [108,144) wall [144,180) peak_alloc [180,218)
 // peak_resv [218,256).  Exact for durations below 2^36 ns (68.7 s) and peaks below 2^38 B (256 GiB);
-// a record outside those raises DevState::wide_mark and its packed copy is never read.
+// a record outside those raises DevState::marks[MARK_WIDE] and its packed copy is never read.
 struct __align__(32) RingPacked {
   u64 w[4];
 };
@@ -96,7 +96,7 @@ __device__ __forceinline__ RingPacked pack_hot(u64 dl, u64 fwd, u64 bwd, u64 opt
   p.w[3] = (pa >> 12) | (pr << 26);
   return p;
 }
-// does the record break the packed layout's ranges (DevState::wide_mark)?
+// does the record break the packed layout's ranges (MARK_WIDE)?
 __device__ __forceinline__ bool pack_wide(u64 dl, u64 fwd, u64 bwd, u64 opt, u64 wall, u64 pa, u64 pr) {
   return (((dl | fwd | bwd | opt | wall) >> PACK_DUR_BITS) | ((pa | pr) >> PACK_MEM_BITS)) != 0ull;
 }
@@ -174,6 +174,15 @@ struct DevAcc {
   u32 _pad;
 };
 
+// The certificate's marks (DevState::marks), by the condition a record breaks:
+enum {
+  MARK_GAP,       // step id != the previous commit's step id + 1
+  MARK_NOMEM,     // flags without TML_REC_HAS_MEM
+  MARK_UNUSABLE,  // dl, fwd, bwd, opt and wall all 0 ns
+  MARK_WIDE,      // a duration >= 2^36 ns or a peak >= 2^38 B: the packed copy does not hold it
+  N_MARKS
+};
+
 struct DevState {
   u64 begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // host-launched regions rotate through the first bank;
                                              // graph regions own slot TML_N_SLOTS + capture depth
@@ -187,13 +196,10 @@ struct DevState {
   u64 layer_begin_ts[TML_N_SLOTS + TML_N_GSLOTS];  // deep profile: its own begin slots (hundreds of layer
                                                    // regions open and close while ONE phase region stays
                                                    // open), same two banks as begin_ts
-  // Dense-window certificate (window_certified, window_packed): each mark is one past the newest
-  // commit number that breaks its condition, 0 = none.  Raised with atomicMax only, by k_commit,
-  // k_commit_dev and k_ring_split.
-  u64 gap_mark;       // step id != the previous commit's step id + 1
-  u64 nomem_mark;     // flags without TML_REC_HAS_MEM
-  u64 unusable_mark;  // dl, fwd, bwd, opt and wall all 0 ns
-  u64 wide_mark;      // a duration >= 2^36 ns or a peak >= 2^38 B: the packed copy does not hold it
+  // Dense-window certificate (window_certified, window_packed): marks[m] is one past the newest
+  // commit number whose record breaks condition m (record_marks), 0 = none.  Raised with atomicMax
+  // only, by K2 (k_commit, k_commit_dev) and k_ring_split.
+  u64 marks[N_MARKS];
   // Device-committed mode (a step commit was captured into a CUDA graph): the commit number and the
   // step id live here, next to each other so that one copy refreshes the host's view of both
   u64 dc_head;    // == head, written by k_commit_dev and k_set_dc
@@ -212,20 +218,32 @@ struct DevState {
 // window row usable (c).  Conversely under (a)-(c) every row is a candidate of both kinds with
 // consecutive ids, hi[0] == hi[1] is the newest id, and there are no violations or duplicates.
 // A decreasing or repeated id breaks (a).  A break at first_k itself is allowed (its predecessor is
-// no longer retained), hence gap_mark <= first_k + 1.  Marks only grow and first_k only grows, so a
-// verdict can be lost to later commits but never gained.  The marks are read by the pass that
-// reads the ring, so they cover the same commits as its ring reads: the build must be ordered
-// after the commits it summarises, as for the records themselves.
+// no longer retained), hence marks[MARK_GAP] <= first_k + 1.  Marks only grow and first_k only
+// grows, so a verdict can be lost to later commits but never gained.  The marks are read by the
+// pass that reads the ring, so they cover the same commits as its ring reads: the build must be
+// ordered after the commits it summarises, as for the records themselves.
 __host__ __device__ __forceinline__ bool step_follows(u64 prev, u64 step) {
   return prev != ~0ull && step == prev + 1;
 }
-__host__ __device__ __forceinline__ bool window_certified(u64 gap_mark, u64 nomem_mark, u64 unusable_mark,
-                                                          u64 first_k, u64 t_start) {
-  return gap_mark <= first_k + 1 && nomem_mark <= first_k && unusable_mark <= first_k + t_start;
+__host__ __device__ __forceinline__ bool window_certified(const u64 (&marks)[N_MARKS], u64 first_k, u64 t_start) {
+  // `&`, not `&&`: all three are read before any is tested (in device memory one round trip, not three)
+  return (marks[MARK_GAP] <= first_k + 1) & (marks[MARK_NOMEM] <= first_k) &
+         (marks[MARK_UNUSABLE] <= first_k + t_start);
 }
 // A certified window is packed-streamable when every retained record fits its packed copy
-// (RingPacked): wide_mark follows the same rules as the certificate's marks.
-__host__ __device__ __forceinline__ bool window_packed(u64 wide_mark, u64 first_k) { return wide_mark <= first_k; }
+// (RingPacked): marks[MARK_WIDE] follows the same rules as the certificate's marks.
+__host__ __device__ __forceinline__ bool window_packed(const u64 (&marks)[N_MARKS], u64 first_k) {
+  return marks[MARK_WIDE] <= first_k;
+}
+// The one rule of every ring writer: the set of marks (bit m: MARK_m) a record breaks.  `gap` is the
+// writer's verdict that the step id does not follow the previous commit's; dl..wall are the five
+// summarised durations and pa, pr the peaks.
+__device__ __forceinline__ u32 record_marks(bool gap, u32 flags, u64 dl, u64 fwd, u64 bwd, u64 opt, u64 wall,
+                                            u64 pa, u64 pr) {
+  return (gap ? 1u << MARK_GAP : 0u) | ((flags & TML_REC_HAS_MEM) ? 0u : 1u << MARK_NOMEM) |
+         ((dl | fwd | bwd | opt | wall) == 0ull ? 1u << MARK_UNUSABLE : 0u) |
+         (pack_wide(dl, fwd, bwd, opt, wall, pa, pr) ? 1u << MARK_WIDE : 0u);
+}
 
 // host-mapped page: written by kernels, read by the sampler thread with no CUDA call
 struct HostPage {
@@ -244,12 +262,11 @@ struct CommitArgs {
   u64 peak_alloc;  // c10 allocator peaks of the step (host state: they travel as launch arguments)
   u64 peak_resv;
   u64 seq;         // commit number = ring position (the host counts them)
-  u32 gap;         // the host's verdicts for the certificate: step != the previous step id + 1,
-  u32 nomem;       // no TML_REC_HAS_MEM (k_commit decides "unusable" itself)
+  u32 gap;         // the host's gap verdict for the certificate: step != the previous step id + 1
 };
 
 // k_commit_dev: what is left once the commit number, the epoch, the step id and the certificate's
-// verdicts come from the device.  A captured commit's arguments are frozen at capture.
+// gap verdict come from the device.  A captured commit's arguments are frozen at capture.
 #define TML_NO_WALL_SLOT 0xffffffffu
 struct DevCommitArgs {
   double host_ts;  // host commits (captured ones stamp %globaltimer)
@@ -343,10 +360,9 @@ __global__ void __maxnreg__(24) k_stamp_end(DevState* st, u32 slot, u32 phase, u
 // ------------------------------------------------------------------ K2: commit
 // 6 warps: warp p owns phase p's running statistics; warp 0 also assembles the
 // record in shared memory and writes its two 64-B ring halves (8 x 16-B stores), the memory byte
-// and the packed copy.
+// and the packed copy.  One kernel per commit mode, each with its own front end: the fetch of ONE
+// global round trip on the critical path.  All that follows the fetch is commit_body.
 
-// k_commit_dev's running statistics and ring store: k_commit's own code, which stays inline in
-// k_commit because calling these changes its SASS.
 // Running statistics of phase `warp` after a step of `dur` ns / `calls` calls: count / sum / worst
 // exactly, median from the log histogram by a warp-shuffle inclusive scan of per-lane bin counts.
 // c[8]: this lane's 8 bins of h, already fetched; run_sum / run_max: lane 0's.
@@ -411,129 +427,69 @@ __device__ __forceinline__ void commit_store(const StepRing& ring, u64 slot, con
   }
 }
 
+// K2 once a front end has fetched its inputs.  Every thread: phase `warp`'s duration and calls of
+// the step (dur, calls), its histogram (h, with this lane's 8 bins in c) and, in lane 0, its running
+// sum and worst; acc: the step's accumulator set, mask: its gpu mask (warp 0, lane 0).  Warp 0: the
+// record's commit number, step id, gap verdict, peaks, host timestamp and flags.  `dev`:
+// device-committed mode, which also keeps the step id and the commit count in dc_step / dc_head.
 // Nothing in here leaves the GPU: writing the record and the live statistics into host-mapped
 // memory and closing with __threadfence_system would cost the TRAINING stream time every step for
 // the benefit of a sampler that looks twice a second.  The sampler instead fetches what it needs itself (k_mirror, on its own stream, tml_drain / tml_live).
-__global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, CommitArgs a) {
+__device__ __forceinline__ void commit_body(DevState* st, const StepRing& ring, DevAcc* acc, u32* h, u32 (&c)[8],
+                                            u64 dur, u32 calls, u32 mask, u64 run_sum, u64 run_max, u64 seq,
+                                            u64 step, bool gap, u64 peak_alloc, u64 peak_resv, double host_ts,
+                                            u32 flags, bool dev) {
   __shared__ __align__(16) u64 rec[16];
   __shared__ u64 s_dur[TML_MAX_PHASES];
   __shared__ u32 s_calls[TML_MAX_PHASES];
   __shared__ u32 s_mask;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  DevAcc* acc = &st->acc[a.epoch];
-
-  // ONE global round trip on the critical path: the phase accumulator and the 256-bin histogram
-  // (8 bins per lane) are fetched together; the +1 of this step is applied in registers and
-  // written back without being waited for (instead of accumulator -> histogram RMW -> histogram
-  // re-read -> head read: four dependent round trips).
-  u32* h = st->hist[warp];
-  u32 c[8];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) c[k] = h[lane * 8 + k];
-  u64 dur = 0, run_sum = 0, run_max = 0;
-  u32 calls = 0;
   if (lane == 0) {
-    dur = acc->dur_ns[warp] + a.host_dur[warp];
-    calls = acc->n_calls[warp] + a.host_calls[warp];
-    run_sum = st->live_sum[warp];
-    run_max = st->live_max[warp];
     s_dur[warp] = dur;
     s_calls[warp] = calls;
     acc->dur_ns[warp] = 0;
     acc->n_calls[warp] = 0;
     if (warp == 0) {
-      s_mask = acc->gpu_mask;
+      s_mask = mask;
       acc->gpu_mask = 0;
       // spare accumulator slots ("other" regions) are reset, not recorded
       acc->dur_ns[6] = 0; acc->dur_ns[7] = 0; acc->n_calls[6] = 0; acc->n_calls[7] = 0;
     }
   }
-  dur = __shfl_sync(0xffffffffu, dur, 0);
-  calls = __shfl_sync(0xffffffffu, calls, 0);
-
-  // running statistics of phase `warp`: count / sum / worst exactly, median from
-  // the log histogram by a warp-shuffle inclusive scan of per-lane bin counts.
-  if (calls > 0u) {
-    const u32 bin = hist_bin(dur);
-    if ((int)(bin >> 3) == lane) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) c[k] += ((bin & 7u) == (u32)k) ? 1u : 0u;
-      h[bin] = c[0] * ((bin & 7u) == 0u) + c[1] * ((bin & 7u) == 1u) + c[2] * ((bin & 7u) == 2u) +
-               c[3] * ((bin & 7u) == 3u) + c[4] * ((bin & 7u) == 4u) + c[5] * ((bin & 7u) == 5u) +
-               c[6] * ((bin & 7u) == 6u) + c[7] * ((bin & 7u) == 7u);
-    }
-    u32 local = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) local += c[k];
-    u32 incl = local;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      u32 n = __shfl_up_sync(0xffffffffu, incl, off);
-      if (lane >= off) incl += n;
-    }
-    u32 total = __shfl_sync(0xffffffffu, incl, 31);
-    u32 target = (total + 1u) >> 1;
-    u32 excl = incl - local;
-    unsigned hit = __ballot_sync(0xffffffffu, (excl < target) && (target <= incl));
-    int src = __ffs(hit) - 1;
-    const u64 sum = __shfl_sync(0xffffffffu, run_sum, 0) + dur;
-    u64 mx = __shfl_sync(0xffffffffu, run_max, 0);
-    mx = dur > mx ? dur : mx;
-    if (lane == src) {
-      u32 run = excl;
-      u32 mbin = lane * 8;
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        run += c[k];
-        if (run >= target) { mbin = lane * 8 + k; break; }
-      }
-      st->live_sum[warp] = sum;
-      st->live_max[warp] = mx;
-      tml_live_phase* lp = &st->live.phase[warp];
-      lp->count = total;
-      lp->sum_ns = sum;
-      lp->worst_ns = mx;
-      lp->median_ns = hist_bin_center(mbin);
-    }
-  }
+  commit_stats(st, warp, lane, h, c, dur, calls, run_sum, run_max);
   __syncthreads();
 
   if (warp == 0) {
-    const u64 seq = a.seq;  // the host counts commits: no read of the head on the critical path
     const u64 slot = seq % ring.slots;
     if (lane == 0) {  // rec[0..8): the hot half, rec[8..16): the cold half
-      rec[0] = a.step;
+      rec[0] = step;
       rec[1] = s_dur[0];
 #pragma unroll
       for (int p = 2; p < 6; ++p) rec[p] = s_dur[p];
-      rec[6] = a.peak_alloc;
-      rec[7] = a.peak_resv;
+      rec[6] = peak_alloc;
+      rec[7] = peak_resv;
       rec[8] = s_dur[1];
       rec[9] = (u64)s_calls[0] | ((u64)s_calls[1] << 32);
       rec[10] = (u64)s_calls[2] | ((u64)s_calls[3] << 32);
       rec[11] = (u64)s_calls[4] | ((u64)s_calls[5] << 32);
-      rec[12] = (u64)__double_as_longlong(a.host_ts);
-      rec[13] = (u64)s_mask | ((u64)a.flags << 32);
+      rec[12] = (u64)__double_as_longlong(host_ts);
+      rec[13] = (u64)s_mask | ((u64)flags << 32);
       rec[14] = seq;
       rec[15] = 0;
     }
     __syncwarp();
-    if (lane < 8) {
-      uint4 v = reinterpret_cast<const uint4*>(rec)[lane];
-      uint4* half = lane < 4 ? reinterpret_cast<uint4*>(&ring.hot[slot]) : reinterpret_cast<uint4*>(&ring.cold[slot]);
-      half[lane & 3] = v;
-    } else if (lane == 8) {
-      ring.mem[slot] = (a.flags & TML_REC_HAS_MEM) ? 1 : 0;
-    } else if (lane == 9) {
-      ring.packed[slot] = pack_hot(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7]);
-    }
+    commit_store(ring, slot, rec, lane, flags);
     __syncwarp();
     if (lane == 0) {
       // the certificate's marks: rare, and not waited for (nothing reads them back here)
-      if (a.gap) atomicMax(&st->gap_mark, seq + 1);
-      if (a.nomem) atomicMax(&st->nomem_mark, seq + 1);
-      if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
-      if (pack_wide(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7])) atomicMax(&st->wide_mark, seq + 1);
+      const u32 m = record_marks(gap, flags, rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7]);
+#pragma unroll
+      for (int i = 0; i < N_MARKS; ++i)
+        if ((m >> i) & 1u) atomicMax(&st->marks[i], seq + 1);
+      if (dev) {
+        st->dc_step = step;
+        st->dc_head = seq + 1;
+      }
       __threadfence();  // the record is visible to every later reader of `head` on this GPU
       st->live.steps_committed = seq + 1;
       st->head = seq + 1;
@@ -541,18 +497,41 @@ __global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, Com
   }
 }
 
+// K2 in host mode: the host counts commits and steps, so the commit number, the epoch, the step id
+// and the gap verdict are launch arguments.  Its ONE global round trip: the phase accumulator and
+// the 256-bin histogram (8 bins per lane) are fetched together; the +1 of this step is applied in
+// registers and written back without being waited for (instead of accumulator -> histogram RMW ->
+// histogram re-read -> head read: four dependent round trips).
+__global__ void __launch_bounds__(192) k_commit(DevState* st, StepRing ring, CommitArgs a) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  DevAcc* acc = &st->acc[a.epoch];
+  u32* h = st->hist[warp];
+  u32 c[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) c[k] = h[lane * 8 + k];
+  u64 dur = 0, run_sum = 0, run_max = 0;
+  u32 calls = 0, mask = 0;
+  if (lane == 0) {
+    dur = acc->dur_ns[warp] + a.host_dur[warp];
+    calls = acc->n_calls[warp] + a.host_calls[warp];
+    run_sum = st->live_sum[warp];
+    run_max = st->live_max[warp];
+    if (warp == 0) mask = acc->gpu_mask;
+  }
+  dur = __shfl_sync(0xffffffffu, dur, 0);
+  calls = __shfl_sync(0xffffffffu, calls, 0);
+  commit_body(st, ring, acc, h, c, dur, calls, mask, run_sum, run_max, a.seq, a.step, a.gap != 0u, a.peak_alloc,
+              a.peak_resv, a.host_ts, a.flags, false);
+}
+
 // K2 in device-committed mode: launched by the host, or captured into a CUDA graph and run on every
 // replay.  The commit number (ring slot, epoch) is the head, the step id the device's last id +
-// a.advance, and the certificate's gap / no-memory verdicts are decided here with the host path's
-// definitions.  The epoch is only known once the head has arrived, so lanes 0..7 fetch phase `warp`'s
-// word of all 8 accumulator sets alongside the head and the histogram: the critical path keeps ONE
-// global round trip, and the epoch's words are picked by shuffle.  A captured commit's wall
-// (phase 5) is %globaltimer minus the begin stamp its tml_graph_step_begin captured.
+// a.advance, and the gap verdict is decided here with the host mode's definition.  The epoch is
+// only known once the head has arrived, so lanes 0..7 fetch phase `warp`'s word of all 8
+// accumulator sets alongside the head and the histogram: the critical path keeps ONE global round
+// trip, and the epoch's words are picked by shuffle.  A captured commit's wall (phase 5) is
+// %globaltimer minus the begin stamp its tml_graph_step_begin captured.
 __global__ void __launch_bounds__(192) k_commit_dev(DevState* st, StepRing ring, DevCommitArgs a) {
-  __shared__ __align__(16) u64 rec[16];
-  __shared__ u64 s_dur[TML_MAX_PHASES];
-  __shared__ u32 s_calls[TML_MAX_PHASES];
-  __shared__ u32 s_mask;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool captured = a.wall_slot != TML_NO_WALL_SLOT;
   const u64 t1 = globaltimer_ns();
@@ -587,62 +566,16 @@ __global__ void __launch_bounds__(192) k_commit_dev(DevState* st, StepRing ring,
   u32 calls = __shfl_sync(0xffffffffu, e_calls, epoch) + a.host_calls[warp];
   const u32 mask = __shfl_sync(0xffffffffu, e_mask, epoch);
   const u64 run_sum = __shfl_sync(0xffffffffu, x, 9), run_max = __shfl_sync(0xffffffffu, x, 10);
-  const u64 x11 = __shfl_sync(0xffffffffu, x, 11);
+  const u64 x11 = __shfl_sync(0xffffffffu, x, 11);  // warp 0: the last step id; warp 5: the wall's begin
   if (warp == 5 && captured) {
     dur += t1 > x11 ? t1 - x11 : 0ull;
     calls += 1u;
   }
-  if (lane == 0) {
-    DevAcc* acc = &st->acc[epoch];
-    s_dur[warp] = dur;
-    s_calls[warp] = calls;
-    acc->dur_ns[warp] = 0;
-    acc->n_calls[warp] = 0;
-    if (warp == 0) {
-      s_mask = mask;
-      acc->gpu_mask = 0;
-      acc->dur_ns[6] = 0; acc->dur_ns[7] = 0; acc->n_calls[6] = 0; acc->n_calls[7] = 0;
-    }
-  }
-  commit_stats(st, warp, lane, h, c, dur, calls, run_sum, run_max);
-  __syncthreads();
-
-  if (warp == 0) {
-    const u64 last = x11;
-    const u64 m_alloc = __shfl_sync(0xffffffffu, x, 12), m_resv = __shfl_sync(0xffffffffu, x, 13);
-    const u64 step = last + a.advance;
-    const u64 slot = seq % ring.slots;
-    if (lane == 0) {
-      rec[0] = step;
-      rec[1] = s_dur[0];
-#pragma unroll
-      for (int p = 2; p < 6; ++p) rec[p] = s_dur[p];
-      rec[6] = captured ? m_alloc : a.peak_alloc;
-      rec[7] = captured ? m_resv : a.peak_resv;
-      rec[8] = s_dur[1];
-      rec[9] = (u64)s_calls[0] | ((u64)s_calls[1] << 32);
-      rec[10] = (u64)s_calls[2] | ((u64)s_calls[3] << 32);
-      rec[11] = (u64)s_calls[4] | ((u64)s_calls[5] << 32);
-      rec[12] = (u64)__double_as_longlong(captured ? (double)t1 * 1.0e-9 : a.host_ts);
-      rec[13] = (u64)s_mask | ((u64)a.flags << 32);
-      rec[14] = seq;
-      rec[15] = 0;
-    }
-    __syncwarp();
-    commit_store(ring, slot, rec, lane, a.flags);
-    __syncwarp();
-    if (lane == 0) {
-      if (seq > 0 && !step_follows(last, step)) atomicMax(&st->gap_mark, seq + 1);
-      if ((a.flags & TML_REC_HAS_MEM) == 0u) atomicMax(&st->nomem_mark, seq + 1);
-      if ((rec[1] | rec[2] | rec[3] | rec[4] | rec[5]) == 0ull) atomicMax(&st->unusable_mark, seq + 1);
-      if (pack_wide(rec[1], rec[2], rec[3], rec[4], rec[5], rec[6], rec[7])) atomicMax(&st->wide_mark, seq + 1);
-      st->dc_step = step;
-      st->dc_head = seq + 1;
-      __threadfence();
-      st->live.steps_committed = seq + 1;
-      st->head = seq + 1;
-    }
-  }
+  const u64 m_alloc = __shfl_sync(0xffffffffu, x, 12), m_resv = __shfl_sync(0xffffffffu, x, 13);
+  const u64 step = x11 + a.advance;
+  commit_body(st, ring, &st->acc[epoch], h, c, dur, calls, mask, run_sum, run_max, seq, step,
+              seq > 0 && !step_follows(x11, step), captured ? m_alloc : a.peak_alloc,
+              captured ? m_resv : a.peak_resv, captured ? (double)t1 * 1.0e-9 : a.host_ts, a.flags, true);
 }
 
 // The device words of device-committed mode: the commit count and the last step id (the host's
@@ -707,9 +640,17 @@ __global__ void k_layer_end(DevState* st, LayerAcc* acc, u32 slot, u32 layer, u3
   }
 }
 
-// one thread per layer: accumulators -> ring slot of this step (48-B records, coalesced), reset
+// one thread per layer: accumulators -> ring slot of this step (48-B records, coalesced), reset.
+// Host mode (st == nullptr): the ring position and the step id are `seq` and `step`.
+// Device-committed mode: the ring position is the layer head and the step id the device's last one
+// (k_commit_dev ran just before on the same stream).  With several CTAs every CTA must have read the
+// head before it moves, so k_layer_head (host mode) or k_layer_head_inc moves it afterwards.
 __global__ void k_layer_commit(LayerAcc* acc, tml_layer_record* ring, u32 n_layers, u32 ring_steps, u64 seq,
-                               u64 step, u64* head) {
+                               u64 step, const DevState* st, u64* head) {
+  if (st) {
+    seq = *head;
+    step = st->dc_step;
+  }
   const u32 l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l < n_layers) {
     LayerAcc a = acc[l];
@@ -727,29 +668,6 @@ __global__ void k_layer_commit(LayerAcc* acc, tml_layer_record* ring, u32 n_laye
   }
 }
 __global__ void k_layer_head(u64* head, u64 v) { *head = v; }
-
-// Device-committed mode: the ring position is the layer head and the step id the device's last one
-// (k_commit_dev ran just before on the same stream).  With several CTAs every CTA must have read the
-// head before it moves, so k_layer_head_inc moves it afterwards.
-__global__ void k_layer_commit_dev(LayerAcc* acc, tml_layer_record* ring, u32 n_layers, u32 ring_steps,
-                                   const DevState* st, u64* head) {
-  const u64 seq = *head, step = st->dc_step;
-  const u32 l = blockIdx.x * blockDim.x + threadIdx.x;
-  if (l < n_layers) {
-    LayerAcc a = acc[l];
-    tml_layer_record r;
-    r.step = step; r.fwd_ns = a.fwd_ns; r.bwd_ns = a.bwd_ns; r.fwd_calls = a.fwd_calls; r.bwd_calls = a.bwd_calls;
-    r.fwd_bytes = a.fwd_bytes; r.bwd_bytes = a.bwd_bytes;
-    ring[(size_t)(seq % ring_steps) * n_layers + l] = r;
-    LayerAcc z;
-    memset(&z, 0, sizeof(z));
-    acc[l] = z;
-  }
-  __syncthreads();
-  if (gridDim.x == 1) {
-    if (threadIdx.x == 0) { __threadfence(); *head = seq + 1; }
-  }
-}
 __global__ void k_layer_head_inc(u64* head) { *head += 1; }
 
 // ------------------------------------------------------------------ K5: proc commit
@@ -1393,8 +1311,8 @@ __global__ void __maxnreg__(94) k_window_fused(
   WinTally tally;
 
   if (tid == 0) {
-    u32 mode = window_certified(st->gap_mark, st->nomem_mark, st->unusable_mark, first_k, t_start) ? 1u : 0u;
-    if (mode && window_packed(st->wide_mark, first_k)) {
+    u32 mode = window_certified(st->marks, first_k, t_start) ? 1u : 0u;
+    if (mode && window_packed(st->marks, first_k)) {
       mode = 2u;
       s_step0 = ring.hot[first_k % ring.slots].step;
     }
@@ -3039,8 +2957,8 @@ int tml_graph_layer_end(tml_ctx* c, uint32_t layer, uint32_t direction, int slot
 // device's last one.  Launched by the host or captured into a graph (`captured`: not a launch).
 static int layer_commit_dev(tml_ctx* c, cudaStream_t s, bool captured) {
   const int blocks = (int)((c->n_layers + 255) / 256);
-  k_layer_commit_dev<<<blocks, 256, 0, s>>>(c->d_layer_acc, c->d_layer_ring, c->n_layers, c->layer_steps,
-                                            c->d_state, c->d_layer_head);
+  k_layer_commit<<<blocks, 256, 0, s>>>(c->d_layer_acc, c->d_layer_ring, c->n_layers, c->layer_steps, 0, 0,
+                                        c->d_state, c->d_layer_head);
   if (blocks > 1) k_layer_head_inc<<<1, 1, 0, s>>>(c->d_layer_head);
   if (cudaPeekAtLastError() != cudaSuccess)
     return set_err(TML_ERR_CUDA, "layer commit: %s", cudaGetErrorString(cudaGetLastError()));
@@ -3069,7 +2987,7 @@ int tml_layer_commit(tml_ctx* c, uint64_t step, void* stream) {
   const int blocks = (int)((c->n_layers + 255) / 256);
   if (c->dc_on) return layer_commit_dev(c, s, false);  // `step` is the device's
   k_layer_commit<<<blocks, 256, 0, s>>>(c->d_layer_acc, c->d_layer_ring, c->n_layers, c->layer_steps,
-                                        c->layer_commits, step, c->d_layer_head);
+                                        c->layer_commits, step, nullptr, c->d_layer_head);
   if (blocks > 1) k_layer_head<<<1, 1, 0, s>>>(c->d_layer_head, c->layer_commits + 1);
   CK(cudaPeekAtLastError());
   c->launches += blocks > 1 ? 2 : 1;
@@ -3139,32 +3057,26 @@ int tml_step_commit(tml_ctx* c, uint64_t step, uint64_t peak_alloc, uint64_t pea
     d.advance = step != 0 ? 1u : 0u;
     d.wall_slot = TML_NO_WALL_SLOT;
     k_commit_dev<<<1, 192, 0, s>>>(c->d_state, c->ring, d);
-    memset(c->host_dur, 0, sizeof(c->host_dur));
-    memset(c->host_calls, 0, sizeof(c->host_calls));
-    if (cudaPeekAtLastError() != cudaSuccess)
-      return set_err(TML_ERR_CUDA, "commit launch: %s", cudaGetErrorString(cudaGetLastError()));
-    c->launches += 1;
-    c->win_ready = false;
-    return TML_OK;
+  } else {
+    CommitArgs a;
+    a.step = step; a.host_ts = host_ts;
+    memcpy(a.host_dur, c->host_dur, sizeof(a.host_dur));
+    memcpy(a.host_calls, c->host_calls, sizeof(a.host_calls));
+    a.epoch = (u32)(c->commits % TML_N_EPOCHS);
+    a.flags = flags;
+    a.peak_alloc = peak_alloc;
+    a.peak_resv = peak_resv;
+    a.seq = c->commits;
+    a.gap = c->commits > 0 && !step_follows(c->last_step, step);
+    k_commit<<<1, 192, 0, s>>>(c->d_state, c->ring, a);
   }
-  CommitArgs a;
-  a.step = step; a.host_ts = host_ts;
-  memcpy(a.host_dur, c->host_dur, sizeof(a.host_dur));
-  memcpy(a.host_calls, c->host_calls, sizeof(a.host_calls));
-  a.epoch = (u32)(c->commits % TML_N_EPOCHS);
-  a.flags = flags;
-  a.peak_alloc = peak_alloc;
-  a.peak_resv = peak_resv;
-  a.seq = c->commits;
-  a.gap = c->commits > 0 && !step_follows(c->last_step, step);
-  a.nomem = (flags & TML_REC_HAS_MEM) == 0u;
-  k_commit<<<1, 192, 0, s>>>(c->d_state, c->ring, a);
-  memset(c->host_dur, 0, sizeof(c->host_dur));
-  memset(c->host_calls, 0, sizeof(c->host_calls));
+  tml_step_discard(c);  // the host-timed phases went with the commit
   if (cudaPeekAtLastError() != cudaSuccess)
     return set_err(TML_ERR_CUDA, "commit launch: %s", cudaGetErrorString(cudaGetLastError()));
-  c->commits += 1;
-  c->last_step = step;
+  if (!c->dc_on) {
+    c->commits += 1;
+    c->last_step = step;
+  }
   c->launches += 1;
   c->win_ready = false;
   return TML_OK;
@@ -3294,7 +3206,7 @@ __global__ void k_set_heads(DevState* st, u64 head, u64 proc_head, int which) {
 static_assert(ring_word(10) == 6 && ring_word(11) == 7, "public words 10, 11: the peaks");
 __global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, u64 pos0, DevState* st, u64 seq0,
                              u64 pred, u32 has_pred) {
-  u32 gap = 0, nomem = 0, unusable = 0, wide = 0;  // 1 + the chunk index of this thread's newest break, 0 = none
+  u32 brk[N_MARKS] = {};  // per mark: 1 + the chunk index of this thread's newest break, 0 = none
   for (u64 k = (u64)blockIdx.x * blockDim.x + threadIdx.x; k < m * 16; k += (u64)gridDim.x * blockDim.x) {
     const u64 r = k >> 4;
     u64 slot = pos0 + r;
@@ -3306,24 +3218,20 @@ __global__ void k_ring_split(StepRing ring, const u64* __restrict__ src, u64 m, 
     if (w == RING_FLAGS_WORD) ring.mem[slot] = ((u32)(v >> 32) & TML_REC_HAS_MEM) ? 1 : 0;
     if (w == 0) {  // public words: 1 dl, 3..6 fwd bwd opt wall, 10 11 peaks, RING_FLAGS_WORD flags (high half)
       const bool has_prev = r > 0 || has_pred != 0u;
-      if (has_prev && !step_follows(r > 0 ? src[k - 16] : pred, v)) gap = (u32)r + 1u;
-      if (!(((u32)(src[k + RING_FLAGS_WORD] >> 32)) & TML_REC_HAS_MEM)) nomem = (u32)r + 1u;
       const u64 dl = src[k + 1], fwd = src[k + 3], bwd = src[k + 4], opt = src[k + 5], wall = src[k + 6];
       const u64 pa = src[k + 10], pr = src[k + 11];
-      if ((dl | fwd | bwd | opt | wall) == 0ull) unusable = (u32)r + 1u;
-      if (pack_wide(dl, fwd, bwd, opt, wall, pa, pr)) wide = (u32)r + 1u;
+      const u32 marks = record_marks(has_prev && !step_follows(r > 0 ? src[k - 16] : pred, v),
+                                     (u32)(src[k + RING_FLAGS_WORD] >> 32), dl, fwd, bwd, opt, wall, pa, pr);
+#pragma unroll
+      for (int i = 0; i < N_MARKS; ++i)
+        if ((marks >> i) & 1u) brk[i] = (u32)r + 1u;
       ring.packed[slot] = pack_hot(dl, fwd, bwd, opt, wall, pa, pr);
     }
   }
-  gap = __reduce_max_sync(0xffffffffu, gap);
-  nomem = __reduce_max_sync(0xffffffffu, nomem);
-  unusable = __reduce_max_sync(0xffffffffu, unusable);
-  wide = __reduce_max_sync(0xffffffffu, wide);
-  if ((threadIdx.x & 31) == 0) {
-    if (gap) atomicMax(&st->gap_mark, seq0 + gap);
-    if (nomem) atomicMax(&st->nomem_mark, seq0 + nomem);
-    if (unusable) atomicMax(&st->unusable_mark, seq0 + unusable);
-    if (wide) atomicMax(&st->wide_mark, seq0 + wide);
+#pragma unroll
+  for (int i = 0; i < N_MARKS; ++i) {
+    const u32 b = __reduce_max_sync(0xffffffffu, brk[i]);
+    if ((threadIdx.x & 31) == 0 && b) atomicMax(&st->marks[i], seq0 + b);
   }
 }
 
@@ -3356,17 +3264,14 @@ int tml_ring_read_(tml_ctx* c, uint64_t first, uint64_t n, void* out, void* stre
 // bit 1 packed-streamable as well.
 static int ring_verdicts(tml_ctx* c, uint32_t window) {
   DeviceGuard dg(c);
-  u64 marks[4];
-  static_assert(offsetof(DevState, nomem_mark) == offsetof(DevState, gap_mark) + 8 &&
-                offsetof(DevState, unusable_mark) == offsetof(DevState, gap_mark) + 16 &&
-                offsetof(DevState, wide_mark) == offsetof(DevState, gap_mark) + 24, "marks are adjacent");
+  u64 marks[N_MARKS];
   CK(cudaDeviceSynchronize());
-  CK(cudaMemcpy(marks, &c->d_state->gap_mark, sizeof(marks), cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(marks, c->d_state->marks, sizeof(marks), cudaMemcpyDeviceToHost));
   DC_REFRESH(c);
   const u64 n = c->commits < c->ring_slots ? c->commits : c->ring_slots;
   const u64 first_k = c->commits - n;
-  if (!window_certified(marks[0], marks[1], marks[2], first_k, n > window ? n - window : 0)) return 0;
-  return window_packed(marks[3], first_k) ? 3 : 1;
+  if (!window_certified(marks, first_k, n > window ? n - window : 0)) return 0;
+  return window_packed(marks, first_k) ? 3 : 1;
 }
 
 int tml_ring_certified_(tml_ctx* c, uint32_t window) {

@@ -9,8 +9,8 @@ and ``step_overhead.api_cost_us.step_commit``, and the device time of one ring l
 records (``profiles/ring_load.py`` of this tree run against each tree, once per round, median of its
 loads); plus ``parity.ok`` / ``series.bit_equal`` of every run,
 whether the ``--dump-outputs`` files of the first round are byte-identical between the trees,
-``profiles/single_rank_build.py``'s pass-vs-copy-ceiling figures of each tree (one run each, after
-the rounds) and the card's name, power limit and max SM clock (read-only ``nvidia-smi`` query).
+``profiles/single_rank_build.py``'s pass-vs-copy-ceiling figures, device idle time, timeline gaps and
+host segments of each tree (one run each, after the rounds) and the card's name, power limit and max SM clock (read-only ``nvidia-smi`` query).
 
 Both trees must already be built (``__graft_entry__.build()``).  Tree A is usually the parent commit
 and tree B the change under test: any two trees whose bench and profile take these arguments.
@@ -84,6 +84,8 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--out", required=True, help="directory for the dumped outputs and the raw runs")
+    ap.add_argument("--no-overhead", action="store_true",
+                    help="pass --no-overhead to bench.py: skip the step-overhead leg (its metrics stay empty)")
     args = ap.parse_args()
     trees = {"A": os.path.abspath(args.a), "B": os.path.abspath(args.b)}
     os.makedirs(args.out, exist_ok=True)
@@ -91,7 +93,7 @@ def main() -> None:
     for r in range(args.rounds):
         for name, tree in trees.items():
             cmd = [os.path.join(tree, "bench.py"), "--gpus", "1", "--steps", str(args.steps),
-                   "--warmup", str(args.warmup), "--no-cpu-baseline"]
+                   "--warmup", str(args.warmup), "--no-cpu-baseline"] + (["--no-overhead"] if args.no_overhead else [])
             if r == 0:
                 cmd += ["--dump-outputs", os.path.join(os.path.abspath(args.out), f"dump_{name}")]
             res = run(tree, cmd)
@@ -114,7 +116,9 @@ def main() -> None:
         srb = run(tree, [os.path.join(tree, "profiles", "single_rank_build.py"), "--steps", "300"])
         report[name]["single_rank_build"] = {"fused_pass": srb.get("fused_pass"),
                                              "copy_ceiling": srb.get("copy_ceiling"),
-                                             "build_ms": srb.get("build_ms"), "error": srb.get("error")}
+                                             "build_ms": srb.get("build_ms"), "device_idle_ms": srb.get("device_idle_ms"),
+                                             "timeline_ms": srb.get("timeline_ms"), "segments_ms": srb.get("segments_ms"),
+                                             "error": srb.get("error")}
     print(json.dumps(report), flush=True)
 
 

@@ -14,6 +14,8 @@ line:
     Python after it;
   * ``kernel_ms``: device time per build of each kernel (torch.profiler, a run of its own), and
     ``device_idle_ms``: ``build_ms`` minus the pass and the band kernel;
+  * ``timeline_ms``: the device timeline around one build (torch.profiler, another run of its own):
+    pass end -> ``k_bands`` start, ``k_bands`` end -> last copy end, last copy end -> next pass start;
   * ``copy_ceiling``: ``dst.copy_(src)`` on 512 MB device tensors (1.024 GB moved), CUDA events,
     median of 25 after warm-up; the fused pass against it, counting the bytes it moves by the stream
     that ran (``stream``): 32 B per step for a packed-streamable window (the ring's packed records),
@@ -129,7 +131,54 @@ def kernel_times(torch, summ, W: int, n: int = 30) -> dict:
     return out
 
 
-def measure(steps: int, window: int, warmup: int) -> dict:
+def timeline_gaps(torch, summ, W: int, n: int = 30, trace_path: str = "") -> dict:
+    """The device timeline around one build, from a torch.profiler trace of ``n`` back-to-back builds
+    (a run of its own).  Per build, medians in ms:
+
+      * ``pass_end_to_bands``: the fused pass's end -> ``k_bands``' start;
+      * ``bands_to_last_copy``: ``k_bands``' end -> the end of the last device-to-host copy of the
+        build (0 when no copy ends after ``k_bands``);
+      * ``results_to_next_pass``: the later of those two ends -> the next build's pass start: the
+        host round trip the GPU waits on.
+    ``trace_path``: also write the Chrome trace there."""
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(n):
+            summ.build(W, PROC_ROWS)
+        torch.cuda.synchronize()
+    if trace_path:
+        prof.export_chrome_trace(trace_path)
+    passes, bands, copies = [], [], []
+    for e in prof.events():
+        if e.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        a, b = e.time_range.start / 1e3, e.time_range.end / 1e3  # us -> ms
+        if "k_window_fused" in e.name:
+            passes.append((a, b))
+        elif "k_bands" in e.name:
+            bands.append((a, b))
+        elif "DtoH" in e.name or "Device -> Pinned" in e.name:
+            copies.append((a, b))
+    passes.sort(); bands.sort(); copies.sort()
+    rows = {"pass_end_to_bands": [], "bands_to_last_copy": [], "results_to_next_pass": []}
+    for (p0, p1), (q0, _) in zip(passes, passes[1:]):
+        bd = [x for x in bands if p1 <= x[0] < q0]
+        if not bd:
+            continue
+        b0, b1 = bd[0]
+        ends = [c1 for c0, c1 in copies if p0 <= c0 < q0 and c1 > b1]
+        last = max(ends) if ends else b1
+        rows["pass_end_to_bands"].append(b0 - p1)
+        rows["bands_to_last_copy"].append(last - b1)
+        rows["results_to_next_pass"].append(q0 - last)
+    out = {k: (statistics.median(v) if v else None) for k, v in rows.items()}
+    out["builds"] = len(rows["results_to_next_pass"])
+    out["copies_per_build"] = len(copies) / max(1, len(passes))
+    return out
+
+
+def measure(steps: int, window: int, warmup: int, trace: str = "") -> dict:
     sys.path.insert(0, ROOT)
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import numpy as np
@@ -186,6 +235,7 @@ def measure(steps: int, window: int, warmup: int) -> dict:
         sj.append((time.perf_counter() - t0) * 1e3)
     seg = segments(summ, W, steps)
     kern = kernel_times(torch, summ, W)
+    gaps = timeline_gaps(torch, summ, W, trace_path=trace)
     from traceml_b200 import _abi
 
     stream = ("packed" if _abi.lib().tml_ring_packed_(eng.handle, W) == 1 else
@@ -209,6 +259,7 @@ def measure(steps: int, window: int, warmup: int) -> dict:
         "segments_ms": seg, "kernel_ms": kern,
         # what the device does not spend in the pass or the band sums (both timed on the device)
         "device_idle_ms": build_ms - k3a - (kern.get("k_bands") or 0.0),
+        "timeline_ms": gaps,
         "copy_ceiling": ceil,
         "fused_pass": {"bytes": fused_bytes, "ms": k3a, "GBps": fused_gbps,
                        "of_copy_ceiling": (fused_gbps / ceil["GBps"]) if fused_gbps else None,
@@ -222,10 +273,11 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=1000, help="K: builds per timed loop")
     ap.add_argument("--window", type=int, default=4_000_000, help="W: step records")
     ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--trace", default="", help="also write the timeline's Chrome trace to this path")
     args = ap.parse_args()
     if args.steps < 1 or args.window < 1:
         ap.error("--steps and --window must be at least 1")
-    print(json.dumps(measure(args.steps, args.window, args.warmup)), flush=True)
+    print(json.dumps(measure(args.steps, args.window, args.warmup, args.trace)), flush=True)
 
 
 if __name__ == "__main__":

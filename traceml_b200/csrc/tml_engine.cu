@@ -295,9 +295,11 @@ struct WinAcc {  // integer side results of k_window_rows (atomics; order-indepe
 #define WINACC_WORDS 15
 static_assert(sizeof(WinAcc) == WINACC_WORDS * sizeof(u64), "WinAcc is re-armed word by word");
 
-// The chained single-rank build (tml_win_fused_chain_launch_ / _finish_): everything the host
-// reads back, packed so that ONE device-to-host copy fetches it.  Bands and tails have slots of
-// their own: nothing here is shared with the staged path's results or d_partials.
+// The chained single-rank build (tml_win_fused_chain_launch_ / _bands_ / _finish_): everything the
+// host reads back.  Its k_bands launch writes it straight into the pinned page (StagePage::chain,
+// through the page's device alias), so no copy sits between the kernel and the host's wait.  Bands
+// and tails have slots of their own: nothing here is shared with the staged path's results or
+// d_partials.
 struct ChainOut {
   double fin[16];       // k_finalize's columns of k_window_fused: 7 tree sums, 2 byte sums, 2 maxima
   WinAcc acc;           // the pass's integer side results
@@ -2227,14 +2229,13 @@ struct DevFinal {
   double sel_fin[16];    // tml_win_select*: k_finalize of k_gather's partials, layout [q][k]
   double sel_exact[7];   // ... and K3e's reference-order sums of the aligned rows
   double band_sum[48];   // tml_win_bands: [series][band]
-  ChainOut chain;        // the chained build's results (one copy)
-  WinAcc chain_acc;      // ... and its pass's accumulator: armed at context creation and re-armed
+  WinAcc chain_acc;      // the chained pass's accumulator: armed at context creation and re-armed
                          // by the k_bands launch that reads it, so no host copy sits in front of the pass
 };
 
 // The pinned page the result readbacks land in (tml_ctx::h_stage), one member per readback.  The
-// process aggregates' copy is still in flight while the chained build copies its block, so no two
-// members may share bytes.
+// process aggregates' copy may still be in flight while the chained build's k_bands writes its
+// block, so no two members may share bytes.
 struct StagePage {
   WinFinal prepare;
   struct {
@@ -2375,8 +2376,12 @@ struct tml_ctx {
   DevFinal* d_final = nullptr;
   u64* d_bandcnt = nullptr;
   u64 chain_n = 0, chain_window = 0;    // the chained pass in flight: retained rows, window
+  double* chain_series = nullptr;       // ... its series and their row stride
+  u64 chain_ld = 0;
+  int chain_grid = 0;                   // ... its CTAs (k_bands folds their partials)
   bool chain_pending = false;
   StagePage* h_stage = nullptr;  // pinned
+  StagePage* d_stage = nullptr;  // h_stage's device alias: the chained k_bands writes through it
   std::unordered_map<std::string, void*> peers;
   void* comb[2] = {nullptr, nullptr};  // live step-combined workspaces, per kind (tml_combined.cuh)
   void* run_ws = nullptr;        // tml_reduce_run's workspace (tml_summary.cpp)
@@ -2575,7 +2580,8 @@ int tml_init(int device, int rank, int world, uint32_t ring_slots, uint32_t proc
     armed.lo[0] = armed.lo[1] = ~0ull;
     CK(cudaMemcpy(&c->d_final->chain_acc, &armed, sizeof(armed), cudaMemcpyHostToDevice));
   }
-  CK(cudaHostAlloc(&c->h_stage, sizeof(StagePage), cudaHostAllocDefault));
+  CK(cudaHostAlloc(&c->h_stage, sizeof(StagePage), cudaHostAllocMapped));
+  CK(cudaHostGetDevicePointer((void**)&c->d_stage, c->h_stage, 0));
   *out = c;
   return TML_OK;
 }
@@ -3710,10 +3716,10 @@ static int fused_result(tml_ctx* c, u64 n, u64 window, const WinAcc& acc, const 
 }
 
 // The single-rank bulk pass as one device submission with the band sums chained behind it
-// (tml_internal.h).
+// (tml_internal.h): the pass first, so that nothing the host does for the bands delays it.
 int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uint64_t ld, uint32_t paired,
-                                const tml_band_args* bands, void* stream) {
-  if (!c || !series || !bands || window == 0) return TML_ERR_ARG;
+                                void* stream) {
+  if (!c || !series || window == 0) return TML_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
   DC_REFRESH(c);
@@ -3726,24 +3732,36 @@ int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uin
   int grid = 0;
   int rc = fused_pass(c, window, series, ld, paired != 0, s, &grid);
   if (rc != TML_OK) return rc;
-  // k_bands as tml_win_bands launches it, into the packed block's own slots, plus the row of CTAs
-  // that finishes the pass
-  BandParams p;
-  p.series = series; p.ld = ld;
-  p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
-  memcpy(p.lo, bands->band_lo, sizeof(p.lo));
-  memcpy(p.hi, bands->band_hi, sizeof(p.hi));
-  memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
-  ChainOut* co = &c->d_final->chain;
-  p.fin_partials = c->d_partials; p.fin_nblk = grid; p.fin_acc = &c->d_final->chain_acc; p.fin_out = co;
-  k_bands<<<dim3(16, 5), 256, 0, s>>>(p, co->band_sum, co->band_cnt, co->tail);
-  CK(cudaPeekAtLastError());
-  c->launches += 1;
+  c->chain_series = series;
+  c->chain_ld = ld;
+  c->chain_grid = grid;
   c->chain_pending = true;
   return TML_OK;
 }
 
-// The launched chain's results: one copy, one wait.
+// k_bands behind the launched pass, as tml_win_bands launches it, plus the row of CTAs that finishes
+// the pass; every result lands in the pinned page.  Nothing orders the process aggregates (side
+// stream) in front of it: a cross-stream wait there delays k_bands by microseconds even when the
+// aggregates finished long before, and tml_proc_reduce_collect waits on their own event.
+int tml_win_fused_chain_bands_(tml_ctx* c, const tml_band_args* bands, void* stream) {
+  if (!c || !bands) return TML_ERR_ARG;
+  if (!c->chain_pending) return set_err(TML_ERR_STATE, "tml_win_fused_chain_bands_ without a launch");
+  cudaStream_t s = (cudaStream_t)stream;
+  BandParams p;
+  p.series = c->chain_series; p.ld = c->chain_ld;
+  p.n_common = bands->n_common; p.shard_lo = bands->shard_lo; p.shard_hi = bands->shard_hi;
+  memcpy(p.lo, bands->band_lo, sizeof(p.lo));
+  memcpy(p.hi, bands->band_hi, sizeof(p.hi));
+  memcpy(p.tail_first, bands->tail_first, sizeof(p.tail_first));
+  ChainOut* co = &c->d_stage->chain;
+  p.fin_partials = c->d_partials; p.fin_nblk = c->chain_grid; p.fin_acc = &c->d_final->chain_acc; p.fin_out = co;
+  k_bands<<<dim3(16, 5), 256, 0, s>>>(p, co->band_sum, co->band_cnt, co->tail);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  return TML_OK;
+}
+
+// The launched chain's results: one wait, then the pinned page holds them.
 static int chain_result(tml_ctx* c, cudaStream_t s, tml_win_info* out, tml_align_info* aligned,
                         tml_band_out* band_out, uint32_t* ok) {
   c->chain_pending = false;
@@ -3753,7 +3771,6 @@ static int chain_result(tml_ctx* c, cudaStream_t s, tml_win_info* out, tml_align
   out->n_retained = c->chain_n;
   out->monotone = 1;
   const ChainOut& r = c->h_stage->chain;
-  CK(cudaMemcpyAsync(&c->h_stage->chain, &c->d_final->chain, sizeof(ChainOut), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   memcpy(band_out->sum, r.band_sum, sizeof(band_out->sum));
   memcpy(band_out->cnt, r.band_cnt, sizeof(band_out->cnt));
@@ -3767,8 +3784,6 @@ int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml
   if (!c->chain_pending) return set_err(TML_ERR_STATE, "tml_win_fused_chain_finish_ without a launch");
   cudaStream_t s = (cudaStream_t)stream;
   CK(cudaSetDevice(c->device));
-  // the process aggregates (side stream) land in their own staging slot before the one wait
-  if (c->proc_pending && c->proc_pending_n > 0) CK(cudaStreamWaitEvent(s, c->ev_proc, 0));
   return chain_result(c, s, out, aligned, band_out, ok);
 }
 
@@ -3792,7 +3807,8 @@ int tml_win_fused(tml_ctx* c, uint32_t window, double* series, void* stream, tml
   if (n == 0) return TML_OK;
   tml_band_args none;
   memset(&none, 0, sizeof(none));
-  int rc = tml_win_fused_chain_launch_(c, window, series, n > window ? window : n, 0, &none, stream);
+  int rc = tml_win_fused_chain_launch_(c, window, series, n > window ? window : n, 0, stream);
+  if (rc == TML_OK) rc = tml_win_fused_chain_bands_(c, &none, stream);
   if (rc != TML_OK) return rc;
   tml_band_out dropped;
   return chain_result(c, s, out, aligned, &dropped, ok);

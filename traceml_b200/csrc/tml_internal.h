@@ -14,13 +14,16 @@ void** tml_run_ws_slot_(tml_ctx* ctx);
 void tml_run_ws_free_(void* ws);
 
 // The dense single-rank build as one device submission (tml_reduce_run's world == 1 branch).
-// launch: k_window_fused, then k_bands over `series` with `bands` (the host knows n_window, so the
-// band layout, before the pass) and one more row of CTAs that finalises the pass.  finish: one
-// device-to-host copy, one stream wait; then reports what tml_win_fused and tml_win_bands would.
+// launch: k_window_fused over the window into `series`.  bands (always next, on the same stream):
+// k_bands over that series with `bands` (the host knows n_window, so the band layout, before the
+// pass ends) and one more row of CTAs that finalises the pass; it writes every result into the
+// context's pinned page.  finish: one stream wait; then reports what tml_win_fused and
+// tml_win_bands would (tml_proc_reduce_collect waits for the process aggregates on their own event).
 // *ok = 0: not dense, drop the bands.  Series row s starts at series + s * ld (ld >= the window's
 // rows); paired = 1: rows 2m and 2m+1 share their memory and only the even rows are stored.
 int tml_win_fused_chain_launch_(tml_ctx* c, uint32_t window, double* series, uint64_t ld, uint32_t paired,
-                                const tml_band_args* bands, void* stream);
+                                void* stream);
+int tml_win_fused_chain_bands_(tml_ctx* c, const tml_band_args* bands, void* stream);
 int tml_win_fused_chain_finish_(tml_ctx* c, void* stream, tml_win_info* out, tml_align_info* aligned,
                                 tml_band_out* band_out, uint32_t* ok);
 

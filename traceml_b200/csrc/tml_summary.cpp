@@ -792,7 +792,6 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   const u32 window = args->window;
   const u32 exchange = args->exchange;
   if (exchange > TML_XCHG_A2A) return TML_ERR_ARG;
-  memset(out, 0, sizeof(*out));
   Run r;
   r.c = c; r.comm = comm; r.s = (cudaStream_t)stream; r.rank = rank; r.world = world;
   CKT(ensure_ws(c, &r.w));
@@ -801,7 +800,8 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   // ---- stage 1: local window + bounds; process aggregates and the speculative alignment ride along
   // K6 on the side stream: three tiny kernels that would otherwise sit in front of K3a;
   // tml_proc_reduce_collect waits on their own event.  The side stream waits for what r.s held at
-  // entry (ring loads), not for the window pass, which the chained build enqueues first.
+  // entry (ring loads), not for the window pass, which the chained build enqueues first: on that
+  // path nothing that does not gate the pass comes before its launch (the GPU idles until then).
   u64 n_win = 0;
   CKT(tml_win_peek(c, window, nullptr, &n_win));
   const bool bulk = world == 1 && n_win > (u64)TML_FUSED_MIN_ROWS;
@@ -810,21 +810,25 @@ int reduce_run(tml_ctx* c, const tml_comm* comm, const tml_reduce_run_args* args
   u64 bulk_ld = 0;
   u32 bulk_paired = 0;
   if (bulk) {
-    // the dense series has n_win columns, so the band layout is known before the pass
     CKT(bulk_series(r.w, n_win, &bulk_ser, &bulk_ld, &bulk_paired));
-    tml_band_args ba;
-    band_args(n_win, 0, n_win, &ba);
-    CKT(tml_win_fused_chain_launch_(c, window, bulk_ser, bulk_ld, bulk_paired, &ba, r.s));
+    CKT(tml_win_fused_chain_launch_(c, window, bulk_ser, bulk_ld, bulk_paired, r.s));
   }
+  memset(out, 0, sizeof(*out));
   if (args->proc_rows) {
     CKC(cudaStreamWaitEvent(r.w->side, r.w->side_gate, 0));
     CKT(tml_proc_reduce_launch(c, args->proc_rows, r.w->side));
+  }
+  if (bulk) {
+    // the dense series has n_win columns, so the band layout is known before the pass ends
+    tml_band_args ba;
+    band_args(n_win, 0, n_win, &ba);
+    CKT(tml_win_fused_chain_bands_(c, &ba, r.s));
   }
   const double tl = now_ms();
   // ---- single rank, bulk window: ring -> series in ONE pass (k_window_fused); the WindowRows
   // that K3a would write for K4 to re-read never exist.  Falls through to the staged path when the
   // window is not dense (re-flushed step ids, rows without memory, ...).  Pass, bands and process
-  // aggregates are one device submission with one copy and one wait.
+  // aggregates are one device submission with one wait, and no copy: the kernels write the results.
   if (bulk) {
     tml_win_info finfo;
     tml_align_info fal;

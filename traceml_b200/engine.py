@@ -55,6 +55,8 @@ class Engine:
         self._drain_buf = np.zeros(4096, dtype=STEP_RECORD_DTYPE)
         self._pdrain_buf = np.zeros(8192, dtype=PROC_RECORD_DTYPE)
         self._run_out = _abi.ReduceRunOut()
+        self._run_key = None  # reduce_run's last (comm, args) values and their structs
+        self._run_structs = None
 
     # ------------------------------------------------------------ lifecycle
     @property
@@ -228,13 +230,20 @@ class Engine:
         return int(p.value) + int.from_bytes(handle[64:72], "little")
 
     def reduce_run(self, window: int, proc_rows: int, exchange: str, speculate: bool, comm_ptr: int,
-                   rank: int, world: int, stream: int = 0, prev=None) -> _abi.ReduceRunOut:
+                   rank: int, world: int, stream: int = 0, prev=None, out=None) -> _abi.ReduceRunOut:
         """The whole staged reduce, sequenced natively (csrc/tml_summary.cpp).  ``prev``: sections
         (``_abi.Sections``) of an earlier reduce whose text is still to be emitted; the driver emits
-        it while this reduce's window pass runs."""
-        comm = _abi.Comm(comm_ptr or None, int(rank), int(world))
-        args = _abi.ReduceRunArgs(int(window), int(proc_rows or 0), _abi.XCHG[exchange], 1 if speculate else 0)
-        out = self._run_out  # ~45 KB: reused, not reallocated per call
+        it while this reduce's window pass runs.  ``out``: the ``ReduceRunOut`` the driver writes
+        into; by default the engine's own, reused by every call."""
+        key = (window, proc_rows, exchange, speculate, comm_ptr, rank, world)
+        if key != self._run_key:  # back-to-back builds pass the same values: keep their structs
+            self._run_structs = (_abi.Comm(comm_ptr or None, int(rank), int(world)),
+                                 _abi.ReduceRunArgs(int(window), int(proc_rows or 0), _abi.XCHG[exchange],
+                                                    1 if speculate else 0))
+            self._run_key = key
+        comm, args = self._run_structs
+        if out is None:
+            out = self._run_out  # ~35 KB: reused, not reallocated per call
         if prev is not None:
             _abi.summary_run(self._h, comm, args, out, stream, prev)
             return out

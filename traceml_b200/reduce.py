@@ -204,7 +204,11 @@ def trend_layout(n: int, *, min_points: int, warmup_frac: float):
 
 
 def _stream_of(device: torch.device) -> int:
-    return int(torch.cuda.current_stream(device).cuda_stream) if device.type == "cuda" else 0
+    """The raw handle of ``device``'s current stream (0 off CUDA), without a ``torch.cuda.Stream``."""
+    if device.type != "cuda":
+        return 0
+    index = device.index if device.index is not None else torch.cuda.current_device()
+    return torch._C._cuda_getCurrentRawStream(index)
 
 
 class ReduceKind:
@@ -513,9 +517,10 @@ class WindowReducer:
             return True
         return bool(getattr(self.comm, "nccl_comm_ptr", lambda d: None)(self.device))
 
-    def run_native(self, window: int, proc_rows: Optional[int], stream: Optional[int] = None, prev=None):
-        """tml_reduce_run on this process's engine; the raw result struct (valid until the next run).
-        ``prev``: see ``Engine.reduce_run``."""
+    def run_native(self, window: int, proc_rows: Optional[int], stream: Optional[int] = None, prev=None,
+                   out=None):
+        """tml_reduce_run on this process's engine; the raw result struct: ``out`` if given, else the
+        engine's own (valid until the next run).  ``prev``: see ``Engine.reduce_run``."""
         eng = self.engines[0]
         world = self.comm.world
         ptr = self.comm.nccl_comm_ptr(self.device) if world > 1 else 0
@@ -524,20 +529,21 @@ class WindowReducer:
             xchg = "a2a"  # the native driver's own "auto" assumes one host (p2p from 10^6 rows)
         return eng.reduce_run(window, int(proc_rows or 0), xchg,
                               self.speculate, ptr or 0, self.comm.index, world,
-                              _stream_of(self.device) if stream is None else stream, prev=prev)
+                              _stream_of(self.device) if stream is None else stream, prev=prev, out=out)
 
     @staticmethod
     def native_timings(o) -> Dict[str, float]:
-        names = ("prepare", "align", "reduce", "bands", "total")
-        t = {"host_" + nm: float(o.stage_ms[i]) for i, nm in enumerate(names)}
-        t.update({nm: float(o.stage_ms[i]) for i, nm in enumerate(names)})  # stages end in a sync
-        t["k3a"], t["k4"] = float(o.k3a_ms), max(0.0, float(o.k4_ms))
-        return t
+        p, a, r, b, t = o.stage_ms[:]  # the stages end in a sync: host and device times are one
+        return {"host_prepare": p, "host_align": a, "host_reduce": r, "host_bands": b, "host_total": t,
+                "prepare": p, "align": a, "reduce": r, "bands": b, "total": t,
+                "k3a": o.k3a_ms, "k4": max(0.0, o.k4_ms)}
 
-    def native_result(self, o, window: int) -> ReduceResult:
-        """The view of a ``run_native`` result, over its own copy: the engine reuses its struct."""
-        return ReduceResult(type(o).from_buffer_copy(o), window, _abi.XCHG_NAME[int(o.exchange_used)],
-                            self.native_timings(o), device=self.device)
+    def native_result(self, o, window: int, *, owned: bool = False) -> ReduceResult:
+        """The view of a ``run_native`` result: over ``o`` itself when the caller hands it over
+        (``owned``, a struct no later run writes), else over its own copy, since the engine reuses
+        its struct."""
+        return ReduceResult(o if owned else type(o).from_buffer_copy(o), window,
+                            _abi.XCHG_NAME[o.exchange_used], self.native_timings(o), device=self.device)
 
     # ------------------------------------------------------------------ alignment
     def _spec_len(self) -> int:

@@ -162,6 +162,8 @@ class SummaryEngine:
         self.ram_total = ram_total
         self.gpu_count = gpu_count
         self._unemitted: Optional[_abi.Sections] = None  # the last native build's sections
+        self._sec_key = None  # the sections' args, shared by builds with the same values
+        self._sec_args: Optional[_abi.SectionsArgs] = None
         # the System section has one source per node: the engine of local rank 0, whose system
         # ring the sampler fills; its node identity comes from the launcher's environment.  On one
         # node that is comm index 0; on several, every node leader reduces its own ring and the
@@ -247,17 +249,24 @@ class SummaryEngine:
         seng = self._system_launch(rows)  # K6s beside the window pass; nothing without samples
         if native:
             # one rank per process: stages, exchanges and rule engines all native (csrc/tml_summary.cpp).
-            # The text is emitted from the result's own copy: on first access, or by the next build
-            # while its window pass runs, whichever comes first -- so back-to-back builds keep the
-            # JSON emitter out of the time the GPU waits for the host.
+            # The driver writes into a struct the result owns, so nothing is copied after the wait.
+            # The text is emitted from that struct: on first access, or by the next build while its
+            # window pass runs, whichever comes first -- so back-to-back builds keep the JSON
+            # emitter out of the time the GPU waits for the host.
             prev = self._unemitted
-            o = self.reducer.run_native(w, rows, prev=prev if prev is not None and prev._raw is None else None)
-            red = self.reducer.native_result(o, w)
+            o = self.reducer.run_native(w, rows, prev=prev if prev is not None and prev._raw is None else None,
+                                        out=_abi.ReduceRunOut())
+            red = self.reducer.native_result(o, w, owned=True)
         else:
             red = self.reducer.reduce(w, proc_rows=rows, stage_timings=timings)
         # ram_total / gpu_count are per-host constants (psutil.virtual_memory().total,
-        # torch.cuda.device_count()); single-node scope: identical on every rank
-        res = _abi.Sections(src=red.out, args=_abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0))
+        # torch.cuda.device_count()); single-node scope: identical on every rank.  The emitter only
+        # reads its args, so builds with the same values share one struct.
+        key = (self.ram_total, gpu_count, w, rows)
+        if key != self._sec_key:
+            self._sec_args = _abi.SectionsArgs(float(self.ram_total), int(gpu_count), w, rows, 0)
+            self._sec_key = key
+        res = _abi.Sections(src=red.out, args=self._sec_args)
         res["reduce"] = red
         res["system"] = self._system_section(seng)
         if native:

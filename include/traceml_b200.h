@@ -865,6 +865,75 @@ int tml_graph_layer_begin(tml_ctx* ctx, void* stream);
 int tml_graph_layer_end(tml_ctx* ctx, uint32_t layer, uint32_t direction, int slot, uint64_t bytes,
                         void* stream);
 
+/* ---------------------------------------------------------------- LAYER TIME TICK
+ * The render-tick twin of the reference's live layer-time panel, LayerCombinedTimerData
+ * (renderers/layer_combined_time/compute.py:77-253), read from this rank's layer ring on a
+ * caller-given stream (never the training stream).  The ring head is read on the device
+ * (d_layer_head, which both commit modes advance only after a step's records are written), so
+ * only completed commits count.  A "forward row" / "backward row" is a ring step in which some
+ * layer has fwd_calls / bwd_calls > 0: the steps the reference's Layer{Forward,Backward}Time
+ * tables hold a row for (LayerProfile.wire_rows).
+ *
+ * tml_layer_tick_bounds replaces _compute_candidate_safe_step's per-rank part and _db_last_step
+ * (compute.py:111-135, 334-342): the step id of the newest forward row and of the newest backward
+ * row (kept apart: an eval step writes no backward row) and of the oldest retained step.  Returns
+ * a status < 0, else TML_LAYER_HAS_FWD | TML_LAYER_HAS_BWD for the directions that have any row
+ * (the outputs of a direction without rows are 0).  It fixes the ring view (head) the next
+ * tml_layer_tick_snapshot reads.
+ *
+ * tml_layer_tick_snapshot replaces _compute_step_snapshot and _load_samples_backwards for one
+ * rank (compute.py:137-215): `out` (device) receives one tml_layer_snap per layer.  Per direction:
+ *   window  the rows newer than the newest row whose step id is < safe_step (the backward scan's
+ *           early stop; with non-decreasing step ids: every row with step >= safe_step)
+ *   current the newest row of the window whose step id == safe_step (duplicated ids of re-run
+ *           steps: the newest wins); none: the rank is missing in that direction
+ *   has     the layer's *_calls > 0 in a row (wire_rows leaves other layers out)
+ *   peak    max *_ns over the window's rows that have the layer; only on a rank with a current
+ *           row (the reference skips the others before its peak loop)
+ *
+ * tml_layer_tick_fold replaces the cross-rank part of _compute_step_snapshot and
+ * _compute_worst_ranks (compute.py:170-198, 239-253) over `n_ranks` gathered snapshot arrays
+ * (snaps[r * n_layers + l], rank order).  `out` (device): n_layers tml_layer_tick_rows, then
+ * n_ranks uint32 rank flags (TML_LSNAP_RANK_*).  Times are float(ns) / 1e6 like wire_rows, maxima
+ * start from 0.0 like the reference's dict.get(k, 0.0).                                      */
+#define TML_LAYER_HAS_FWD 1
+#define TML_LAYER_HAS_BWD 2
+/* tml_layer_snap.flags (bit << 1 for backward) */
+#define TML_LSNAP_CUR_FWD 1u       /* the layer is in this rank's current forward row */
+#define TML_LSNAP_CUR_BWD 2u
+#define TML_LSNAP_PEAK_FWD 4u      /* ... in some row of this rank's forward window */
+#define TML_LSNAP_PEAK_BWD 8u
+#define TML_LSNAP_RANK_FWD 16u     /* this rank has a current forward row (not missing) */
+#define TML_LSNAP_RANK_BWD 32u
+
+typedef struct tml_layer_snap {    /* 48 B per (rank, layer) */
+  uint64_t cur_fwd_ns, cur_bwd_ns;
+  uint64_t peak_fwd_ns, peak_bwd_ns;
+  uint32_t flags;
+  /* ring position (0 = oldest retained step) of the newest window row holding the layer: the
+   * order in which the reference's peak loop first meets the layers, which fixes the iteration
+   * order of its Python sets and so the order of its float sums */
+  uint32_t last_fwd, last_bwd;
+  uint32_t _pad;
+} tml_layer_snap;
+
+/* tml_layer_tick_row.flags: the TML_LSNAP_CUR_* / _PEAK_* bits OR-ed over the ranks */
+typedef struct tml_layer_tick_row {  /* 56 B per layer */
+  double cur_fwd_ms, cur_bwd_ms;     /* max over ranks of the current values */
+  double peak_fwd_ms, peak_bwd_ms;   /* max over ranks of the peaks */
+  int32_t worst_rank;                /* argmax of cur_fwd + cur_bwd, the reference's tie rule; -1: none */
+  uint32_t flags;
+  uint32_t peak_last[2];             /* last_fwd / last_bwd on rank peak_rank[d] */
+  uint16_t cur_rank[2];              /* first rank with TML_LSNAP_CUR_* (fwd, bwd) */
+  uint16_t peak_rank[2];             /* first rank with TML_LSNAP_PEAK_* */
+} tml_layer_tick_row;
+
+int tml_layer_tick_bounds(tml_ctx* ctx, uint64_t* newest_fwd_step, uint64_t* newest_bwd_step,
+                          uint64_t* oldest_step, void* stream);
+int tml_layer_tick_snapshot(tml_ctx* ctx, uint64_t safe_step, void* out_dev, void* stream);
+int tml_layer_tick_fold(tml_ctx* ctx, const void* snaps_dev, uint32_t n_ranks, uint32_t n_layers,
+                        void* out_dev, void* stream);
+
 /* ---------------------------------------------------------------- TEST HOOK
  * Host emulation of K3e -- the reference-order window sums (``s += x`` per row:
  * reporting/sections/step_time/model.py:262-268, alignment.py:59-75) computed as composed

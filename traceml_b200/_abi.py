@@ -46,6 +46,22 @@ class LayerRecord(C.Structure):
                 ("fwd_bytes", u64), ("bwd_bytes", u64)]
 
 
+class LayerSnap(C.Structure):
+    _fields_ = [("cur_fwd_ns", u64), ("cur_bwd_ns", u64), ("peak_fwd_ns", u64), ("peak_bwd_ns", u64),
+                ("flags", u32), ("last_fwd", u32), ("last_bwd", u32), ("_pad", u32)]
+
+
+class LayerTickRow(C.Structure):
+    _fields_ = [("cur_fwd_ms", f64), ("cur_bwd_ms", f64), ("peak_fwd_ms", f64), ("peak_bwd_ms", f64),
+                ("worst_rank", i32), ("flags", u32), ("peak_last", u32 * 2), ("cur_rank", C.c_uint16 * 2),
+                ("peak_rank", C.c_uint16 * 2)]
+
+
+LAYER_HAS_FWD, LAYER_HAS_BWD = 1, 2
+LSNAP_CUR_FWD, LSNAP_CUR_BWD, LSNAP_PEAK_FWD, LSNAP_PEAK_BWD = 1, 2, 4, 8
+LSNAP_RANK_FWD, LSNAP_RANK_BWD = 16, 32
+
+
 class LivePhase(C.Structure):
     _fields_ = [("count", u64), ("sum_ns", u64), ("worst_ns", u64), ("median_ns", u64)]
 
@@ -231,6 +247,7 @@ class ProcDiagIn(C.Structure):
 
 
 assert C.sizeof(StepRecord) == 128 and C.sizeof(ProcRecord) == 64 and C.sizeof(SysRecord) == 576
+assert C.sizeof(LayerSnap) == 48 and C.sizeof(LayerTickRow) == 56
 
 # name -> (restype, argtypes); every symbol include/traceml_b200.h declares
 SIGNATURES = {
@@ -287,6 +304,9 @@ SIGNATURES = {
     "tml_layer_end": (C.c_int, [vp, u32, u32, C.c_int, u64, vp]),
     "tml_layer_commit": (C.c_int, [vp, u64, vp]),
     "tml_layer_drain": (C.c_int, [vp, vp, u32, C.POINTER(u32), C.POINTER(u32), C.POINTER(u64)]),
+    "tml_layer_tick_bounds": (C.c_int, [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), vp]),
+    "tml_layer_tick_snapshot": (C.c_int, [vp, u64, vp, vp]),
+    "tml_layer_tick_fold": (C.c_int, [vp, vp, u32, u32, vp, vp]),
     "tml_xs_host_sum": (C.c_int, [vp, u64, C.c_int, C.POINTER(f64), C.POINTER(u64)]),
     "tml_reduce_run": (C.c_int, [vp, C.POINTER(Comm), C.POINTER(ReduceRunArgs), vp, C.POINTER(ReduceRunOut)]),
     "tml_combined_prepare": (C.c_int, [vp, u32, u32, vp, C.POINTER(CombinedInfo)]),
@@ -328,6 +348,8 @@ SIGNATURES = {
     "tml_ring_certified_": (C.c_int, [vp, u32]),
     # private: that certificate and every retained record within the ring's packed copy
     "tml_ring_packed_": (C.c_int, [vp, u32]),
+    # private: the layer ring's contents replaced by host records (tests seed the layer tick with it)
+    "tml_layer_load_": (C.c_int, [vp, vp, u64, vp]),
 }
 
 _LIB: Optional[C.CDLL] = None

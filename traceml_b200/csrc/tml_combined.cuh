@@ -445,3 +445,286 @@ int tml_combined_series(tml_ctx* c, const void* const* rank_rows, uint32_t n_ran
 }
 
 }  // extern "C"
+
+// ============================================================================ layer time tick
+// The live layer-time panel's device stages (include/traceml_b200.h, LAYER TIME TICK).  The layer
+// ring is [ring_steps][n_layers] 48-B records; the snapshot gives a warp 32 consecutive layers
+// (lane = layer) and walks the retained steps, so each step it loads is one contiguous 1.5-KB run.
+// Like K7 these kernels run on the tick's own stream while the step path may commit: the head is
+// read once on the device (k_lt_head) and the bounds and the snapshot both use that view.
+
+#define LT_THREADS 128
+
+struct LTickHdr {
+  u64 head, n;                          // completed commits, retained steps (<= ring_steps)
+  u64 fwd_rows, bwd_rows;               // 1 + newest position holding a forward / backward row; 0: none
+  u64 newest_fwd, newest_bwd, oldest;   // step ids of those rows and of the oldest retained step
+};
+
+__global__ void k_lt_head(const u64* head, u32 ring_steps, LTickHdr* h) {
+  const u64 v = *reinterpret_cast<const volatile u64*>(head);
+  h->head = v;
+  h->n = v < (u64)ring_steps ? v : (u64)ring_steps;
+  h->fwd_rows = h->bwd_rows = 0;
+}
+
+// one warp per retained step: its step id and whether any layer has a forward / backward call
+// (whether the reference's forward / backward table holds a row for it)
+__global__ void __launch_bounds__(LT_THREADS) k_lt_rows(const tml_layer_record* __restrict__ ring, u32 n_layers,
+                                                        u32 ring_steps, LTickHdr* h, u64* __restrict__ steps,
+                                                        u8* __restrict__ dirs) {
+  const u64 n = h->n, first = h->head - n;
+  const u32 lane = threadIdx.x & 31;
+  const u64 nwarps = ((u64)gridDim.x * blockDim.x) >> 5;
+  for (u64 i = ((u64)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
+    const tml_layer_record* row = ring + ((first + i) % ring_steps) * (u64)n_layers;
+    u64 calls = 0;  // fwd_calls | bwd_calls << 32
+    for (u32 l = lane; l < n_layers; l += 32) calls |= *reinterpret_cast<const u64*>(&row[l].fwd_calls);
+    const bool f = __any_sync(0xffffffffu, (u32)calls != 0u);
+    const bool b = __any_sync(0xffffffffu, (u32)(calls >> 32) != 0u);
+    if (lane == 0) {
+      steps[i] = row[0].step;
+      dirs[i] = (f ? 1 : 0) | (b ? 2 : 0);
+      if (f) atomicMax(&h->fwd_rows, i + 1);
+      if (b) atomicMax(&h->bwd_rows, i + 1);
+    }
+  }
+}
+
+__global__ void k_lt_bounds(LTickHdr* h, const u64* __restrict__ steps) {
+  h->oldest = h->n ? steps[0] : 0;
+  h->newest_fwd = h->fwd_rows ? steps[h->fwd_rows - 1] : 0;
+  h->newest_bwd = h->bwd_rows ? steps[h->bwd_rows - 1] : 0;
+}
+
+__global__ void __launch_bounds__(LT_THREADS) k_lt_snap(const tml_layer_record* __restrict__ ring, u32 n_layers,
+                                                        u32 ring_steps, const LTickHdr* __restrict__ h,
+                                                        const u64* __restrict__ steps, const u8* __restrict__ dirs,
+                                                        u64 safe, tml_layer_snap* __restrict__ out) {
+  const u32 lane = threadIdx.x & 31;
+  const u32 warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (warp * 32u >= n_layers) return;  // warp-uniform
+  const u64 n = h->n, first = h->head - n;
+  // per direction, over that direction's rows: lo = 1 + the newest with a step id < safe (where the
+  // reference's backward scan stops), cur = the newest with step id == safe
+  int lo0 = 0, lo1 = 0, cur0 = -1, cur1 = -1;
+  for (u32 i = lane; i < (u32)n; i += 32) {
+    const u64 s = steps[i];
+    const u32 d = dirs[i];
+    if (d & 1u) { if (s < safe) lo0 = (int)i + 1; else if (s == safe) cur0 = (int)i; }
+    if (d & 2u) { if (s < safe) lo1 = (int)i + 1; else if (s == safe) cur1 = (int)i; }
+  }
+  lo0 = __reduce_max_sync(0xffffffffu, lo0); lo1 = __reduce_max_sync(0xffffffffu, lo1);
+  cur0 = __reduce_max_sync(0xffffffffu, cur0); cur1 = __reduce_max_sync(0xffffffffu, cur1);
+  const bool has0 = cur0 >= lo0, has1 = cur1 >= lo1;  // else the rank is missing in that direction
+  const u32 l = warp * 32u + lane;
+  if (l >= n_layers) return;
+  u64 cf = 0, cb = 0, pf = 0, pb = 0;
+  u32 flags = (has0 ? TML_LSNAP_RANK_FWD : 0u) | (has1 ? TML_LSNAP_RANK_BWD : 0u), lf = 0, lb = 0;
+  if (has0 || has1) {
+    const u32 start = (u32)(has0 && has1 ? min(lo0, lo1) : has0 ? lo0 : lo1);
+#pragma unroll 4
+    for (u32 i = start; i < (u32)n; ++i) {
+      const tml_layer_record* r = ring + ((first + i) % ring_steps) * (u64)n_layers + l;
+      const u64 fns = r->fwd_ns, bns = r->bwd_ns;
+      const u64 calls = *reinterpret_cast<const u64*>(&r->fwd_calls);
+      if (has0 && (int)i >= lo0 && (u32)calls != 0u) {
+        pf = fns > pf ? fns : pf;
+        lf = i;
+        flags |= TML_LSNAP_PEAK_FWD;
+        if ((int)i == cur0) { cf = fns; flags |= TML_LSNAP_CUR_FWD; }
+      }
+      if (has1 && (int)i >= lo1 && (u32)(calls >> 32) != 0u) {
+        pb = bns > pb ? bns : pb;
+        lb = i;
+        flags |= TML_LSNAP_PEAK_BWD;
+        if ((int)i == cur1) { cb = bns; flags |= TML_LSNAP_CUR_BWD; }
+      }
+    }
+  }
+  tml_layer_snap o;
+  o.cur_fwd_ns = cf; o.cur_bwd_ns = cb; o.peak_fwd_ns = pf; o.peak_bwd_ns = pb;
+  o.flags = flags; o.last_fwd = lf; o.last_bwd = lb; o._pad = 0;
+  out[l] = o;
+}
+
+// wire_rows' float(int(ns)) / 1.0e6, the point where the reference's values become floats:
+// ns_to_ms is that correctly rounded quotient without the division's slow-path call
+__device__ __forceinline__ double lt_ms(u64 ns) { return ns_to_ms(ns); }
+
+// one direction of one layer on one rank: max over ranks (from 0.0, like the reference's
+// dict.get(k, 0.0)) and the first rank that has a current / a peak value
+struct LtDir {
+  double cur = 0.0, peak = 0.0;
+  u32 cur_rank = 0, peak_rank = 0, peak_last = 0;
+  bool has_cur = false, has_peak = false;
+  __device__ __forceinline__ void add(u32 r, bool c, u64 cur_ns, bool p, u64 peak_ns, u32 last) {
+    if (c) {
+      const double v = lt_ms(cur_ns);
+      cur = v > cur ? v : cur;
+      if (!has_cur) cur_rank = r;
+      has_cur = true;
+    }
+    if (p) {
+      const double v = lt_ms(peak_ns);
+      peak = v > peak ? v : peak;
+      if (!has_peak) { peak_rank = r; peak_last = last; }
+      has_peak = true;
+    }
+  }
+};
+
+// one thread per layer over the R gathered snapshots (rank order)
+__global__ void __launch_bounds__(LT_THREADS) k_lt_fold(const tml_layer_snap* __restrict__ snaps, u32 n_ranks,
+                                                        u32 n_layers, tml_layer_tick_row* __restrict__ out,
+                                                        u32* __restrict__ rank_flags) {
+  if (blockIdx.x == 0)
+    for (u32 r = threadIdx.x; r < n_ranks; r += blockDim.x)
+      rank_flags[r] = snaps[(u64)r * n_layers].flags & (TML_LSNAP_RANK_FWD | TML_LSNAP_RANK_BWD);
+  const u32 l = blockIdx.x * blockDim.x + threadIdx.x;
+  if (l >= n_layers) return;
+  LtDir f, b;
+  // worst rank (compute.py:239-253): `totals` gets the ranks with a current forward value in rank
+  // order, then the ranks with only a backward one; a rank's total is fwd + bwd in that order, and
+  // max(totals.items(), key=...) keeps the FIRST maximum -- so only a strictly larger total wins
+  int worst = -1;
+  double wv = 0.0;
+  for (u32 r = 0; r < n_ranks; ++r) {
+    const tml_layer_snap* s = &snaps[(u64)r * n_layers + l];
+    const u32 fl = s->flags;
+    const u64 cfn = s->cur_fwd_ns, cbn = s->cur_bwd_ns;
+    f.add(r, fl & TML_LSNAP_CUR_FWD, cfn, fl & TML_LSNAP_PEAK_FWD, s->peak_fwd_ns, s->last_fwd);
+    b.add(r, fl & TML_LSNAP_CUR_BWD, cbn, fl & TML_LSNAP_PEAK_BWD, s->peak_bwd_ns, s->last_bwd);
+    if (fl & TML_LSNAP_CUR_FWD) {
+      double t = lt_ms(cfn);
+      if (fl & TML_LSNAP_CUR_BWD) t = t + lt_ms(cbn);
+      if (worst < 0 || t > wv) { worst = (int)r; wv = t; }
+    }
+  }
+  for (u32 r = 0; r < n_ranks; ++r) {
+    const tml_layer_snap* s = &snaps[(u64)r * n_layers + l];
+    if ((s->flags & (TML_LSNAP_CUR_FWD | TML_LSNAP_CUR_BWD)) == TML_LSNAP_CUR_BWD) {
+      const double t = lt_ms(s->cur_bwd_ns);
+      if (worst < 0 || t > wv) { worst = (int)r; wv = t; }
+    }
+  }
+  tml_layer_tick_row o;
+  o.cur_fwd_ms = f.cur; o.cur_bwd_ms = b.cur; o.peak_fwd_ms = f.peak; o.peak_bwd_ms = b.peak;
+  o.worst_rank = worst;
+  o.flags = (f.has_cur ? TML_LSNAP_CUR_FWD : 0u) | (b.has_cur ? TML_LSNAP_CUR_BWD : 0u)
+          | (f.has_peak ? TML_LSNAP_PEAK_FWD : 0u) | (b.has_peak ? TML_LSNAP_PEAK_BWD : 0u);
+  o.peak_last[0] = f.peak_last; o.peak_last[1] = b.peak_last;
+  o.cur_rank[0] = (uint16_t)f.cur_rank; o.cur_rank[1] = (uint16_t)b.cur_rank;
+  o.peak_rank[0] = (uint16_t)f.peak_rank; o.peak_rank[1] = (uint16_t)b.peak_rank;
+  out[l] = o;
+}
+
+struct LTickWs {
+  u64 cap = 0;
+  u64* d_steps = nullptr;
+  u8* d_dirs = nullptr;
+  LTickHdr* d_hdr = nullptr;
+  LTickHdr* h_hdr = nullptr;  // pinned
+  u32 n_layers = 0, ring_steps = 0;  // the layer ring the bounds were taken on
+  bool ready = false;
+};
+
+static void ltick_free(tml_ctx* c) {
+  LTickWs* w = (LTickWs*)c->ltick;
+  if (!w) return;
+  cudaFree(w->d_steps); cudaFree(w->d_dirs); cudaFree(w->d_hdr);
+  cudaFreeHost(w->h_hdr);
+  delete w;
+  c->ltick = nullptr;
+}
+
+extern "C" {
+
+int tml_layer_tick_bounds(tml_ctx* c, uint64_t* newest_fwd_step, uint64_t* newest_bwd_step,
+                          uint64_t* oldest_step, void* stream) {
+  if (!c || !newest_fwd_step || !newest_bwd_step || !oldest_step) return TML_ERR_ARG;
+  if (!c->n_layers) return set_err(TML_ERR_STATE, "tml_layer_tick_bounds before tml_layer_init");
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  if (!c->ltick) {
+    LTickWs* w = new LTickWs();
+    c->ltick = w;
+    CK(cudaMalloc(&w->d_hdr, sizeof(LTickHdr)));
+    CK(cudaHostAlloc(&w->h_hdr, sizeof(LTickHdr), cudaHostAllocDefault));
+  }
+  LTickWs* w = (LTickWs*)c->ltick;
+  w->ready = false;
+  if (w->cap < c->layer_steps) {
+    cudaFree(w->d_steps); cudaFree(w->d_dirs);
+    w->d_steps = nullptr; w->d_dirs = nullptr; w->cap = 0;
+    CK(cudaMalloc(&w->d_steps, (size_t)c->layer_steps * sizeof(u64)));
+    CK(cudaMalloc(&w->d_dirs, (size_t)c->layer_steps));
+    w->cap = c->layer_steps;
+  }
+  k_lt_head<<<1, 1, 0, s>>>(c->d_layer_head, c->layer_steps, w->d_hdr);
+  CK(cudaPeekAtLastError());
+  int grid = (int)(((u64)c->layer_steps * 32 + LT_THREADS - 1) / LT_THREADS);
+  if (grid > c->n_sms * 4) grid = c->n_sms * 4;
+  k_lt_rows<<<grid, LT_THREADS, 0, s>>>(c->d_layer_ring, c->n_layers, c->layer_steps, w->d_hdr, w->d_steps,
+                                        w->d_dirs);
+  CK(cudaPeekAtLastError());
+  k_lt_bounds<<<1, 1, 0, s>>>(w->d_hdr, w->d_steps);
+  CK(cudaPeekAtLastError());
+  c->launches += 3;
+  CK(cudaMemcpyAsync(w->h_hdr, w->d_hdr, sizeof(LTickHdr), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  const LTickHdr h = *w->h_hdr;
+  *newest_fwd_step = h.newest_fwd;
+  *newest_bwd_step = h.newest_bwd;
+  *oldest_step = h.oldest;
+  w->n_layers = c->n_layers; w->ring_steps = c->layer_steps; w->ready = true;
+  return (h.fwd_rows ? TML_LAYER_HAS_FWD : 0) | (h.bwd_rows ? TML_LAYER_HAS_BWD : 0);
+}
+
+int tml_layer_tick_snapshot(tml_ctx* c, uint64_t safe_step, void* out_dev, void* stream) {
+  if (!c || !out_dev) return TML_ERR_ARG;
+  LTickWs* w = (LTickWs*)c->ltick;
+  if (!w || !w->ready || w->n_layers != c->n_layers || w->ring_steps != c->layer_steps)
+    return set_err(TML_ERR_STATE, "tml_layer_tick_snapshot without tml_layer_tick_bounds on this layer ring");
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  const u64 warps = ((u64)c->n_layers + 31) / 32;
+  const int grid = (int)((warps * 32 + LT_THREADS - 1) / LT_THREADS);
+  k_lt_snap<<<grid, LT_THREADS, 0, s>>>(c->d_layer_ring, c->n_layers, c->layer_steps, w->d_hdr, w->d_steps,
+                                        w->d_dirs, safe_step, (tml_layer_snap*)out_dev);
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  return TML_OK;
+}
+
+int tml_layer_tick_fold(tml_ctx* c, const void* snaps_dev, uint32_t n_ranks, uint32_t n_layers, void* out_dev,
+                        void* stream) {
+  if (!c || !snaps_dev || !out_dev || n_ranks == 0 || n_ranks > 0xffffu || n_layers == 0) return TML_ERR_ARG;
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  tml_layer_tick_row* rows = (tml_layer_tick_row*)out_dev;
+  const int grid = (int)(((u64)n_layers + LT_THREADS - 1) / LT_THREADS);
+  k_lt_fold<<<grid, LT_THREADS, 0, s>>>((const tml_layer_snap*)snaps_dev, n_ranks, n_layers, rows,
+                                        reinterpret_cast<u32*>(rows + n_layers));
+  CK(cudaPeekAtLastError());
+  c->launches += 1;
+  return TML_OK;
+}
+
+int tml_layer_load_(tml_ctx* c, const tml_layer_record* recs, uint64_t n_steps, void* stream) {
+  if (!c || (!recs && n_steps)) return TML_ERR_ARG;
+  if (!c->n_layers) return set_err(TML_ERR_STATE, "tml_layer_load_ before tml_layer_init");
+  cudaStream_t s = (cudaStream_t)stream;
+  DeviceGuard dg(c);
+  const u64 L = c->n_layers, keep = n_steps < (u64)c->layer_steps ? n_steps : (u64)c->layer_steps;
+  for (u64 k = n_steps - keep; k < n_steps; ++k)
+    CK(cudaMemcpyAsync(c->d_layer_ring + (k % c->layer_steps) * L, recs + k * L, L * sizeof(tml_layer_record),
+                       cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(c->d_layer_head, &n_steps, sizeof(u64), cudaMemcpyHostToDevice, s));
+  CK(cudaStreamSynchronize(s));
+  c->layer_commits = n_steps;
+  c->layer_tail = 0;
+  return TML_OK;
+}
+
+}  // extern "C"

@@ -2384,6 +2384,7 @@ struct tml_ctx {
   StagePage* d_stage = nullptr;  // h_stage's device alias: the chained k_bands writes through it
   std::unordered_map<std::string, void*> peers;
   void* comb[2] = {nullptr, nullptr};  // live step-combined workspaces, per kind (tml_combined.cuh)
+  void* ltick = nullptr;               // live layer-time tick workspace (tml_combined.cuh)
   void* run_ws = nullptr;        // tml_reduce_run's workspace (tml_summary.cpp)
   // system ring and its reduce (tml_sys_*): allocated by the first commit / load
   tml_sys_record* d_sring = nullptr;
@@ -2408,6 +2409,7 @@ struct tml_ctx {
 };
 
 static void comb_free(tml_ctx* c);
+static void ltick_free(tml_ctx* c);
 extern "C" void** tml_run_ws_slot_(tml_ctx* c) { return &c->run_ws; }
 
 static int grid_for(const tml_ctx* c, u64 work_items, int per_block) {
@@ -2628,6 +2630,7 @@ int tml_shutdown(tml_ctx* c) {
   if (c->ev_sys_cluster) cudaEventDestroy(c->ev_sys_cluster);
   cudaFreeHost(c->h_stage);
   comb_free(c);
+  ltick_free(c);
   tml_run_ws_free_(c->run_ws);
   delete c;
   return graphs_live ? (int)(graphs_live < 0x7fffffffull ? graphs_live : 0x7fffffffull) : TML_OK;

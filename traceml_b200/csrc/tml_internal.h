@@ -51,6 +51,10 @@ int tml_ring_certified_(tml_ctx* c, uint32_t window);
 // 1 if that window is certified and every retained record fits the ring's 32-B packed copy, so the
 // window pass streams the packed copies, else 0 (waits for the device)
 int tml_ring_packed_(tml_ctx* c, uint32_t window);
+// Replace the layer ring's contents by `n_steps` x n_layers host records (the newest ring_steps of
+// them are kept), as if they had been committed in that order; waits for the copy.  Tests seed the
+// layer tick's edge cases (duplicated ids, eval steps, wrapped rings) with it.
+int tml_layer_load_(tml_ctx* c, const tml_layer_record* recs, uint64_t n_steps, void* stream);
 
 #ifdef __cplusplus
 }

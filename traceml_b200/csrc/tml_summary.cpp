@@ -1061,7 +1061,7 @@ extern "C" uint64_t tml_struct_size(const char* name) {
   TML_SZ(tml_band_out); TML_SZ(tml_proc_agg); TML_SZ(tml_comm); TML_SZ(tml_reduce_run_args);
   TML_SZ(tml_kind_result); TML_SZ(tml_reduce_run_out); TML_SZ(tml_combined_info); TML_SZ(tml_combined_align);
   TML_SZ(tml_st_diag_in); TML_SZ(tml_mem_diag_in); TML_SZ(tml_proc_diag_in);
-  TML_SZ(tml_layer_record);
+  TML_SZ(tml_layer_record); TML_SZ(tml_layer_snap); TML_SZ(tml_layer_tick_row);
   TML_SZ(tml_sys_gpu); TML_SZ(tml_sys_record); TML_SZ(tml_sys_gpu_agg); TML_SZ(tml_sys_agg); TML_SZ(tml_sys_diag_in);
   TML_SZ(tml_sys_part); TML_SZ(tml_sys_node_ident); TML_SZ(tml_sys_node_record); TML_SZ(tml_sys_cluster_out);
   TML_SZ(tml_sections_args); TML_SZ(tml_live_phase); TML_SZ(tml_rank_means); TML_SZ(tml_trend_in); TML_SZ(tml_mem_metric_in);

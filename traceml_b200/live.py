@@ -14,11 +14,14 @@ points, stale handling and result shape (``asdict(StepCombinedTimeResult)``) as 
 reference; only the data source differs (engines + a comm instead of a db path).
 
 ``StepMemoryMetricsComputer`` is the same for the step-memory panel
-(``renderers/step_memory/{computer,cli_compute,common}.py``).
+(``renderers/step_memory/{computer,cli_compute,common}.py``), and ``LayerCombinedTimerData`` for
+the deep profile's layer-time panel (``renderers/layer_combined_time/compute.py``), reduced from
+the layer rings.
 """
 
 from __future__ import annotations
 
+import ctypes as C
 import time
 from typing import Any, Dict, List, Optional, Sequence
 
@@ -417,3 +420,235 @@ class StepMemoryMetricsComputer:
 
     def compute_dashboard(self) -> Dict[str, Any]:
         return self._dashboard.compute()
+
+
+# =============================================================================== layer time
+_LAYER_ROW_DTYPE = np.dtype([("cur_ms", "<f8", (2,)), ("peak_ms", "<f8", (2,)), ("worst_rank", "<i4"),
+                             ("flags", "<u4"), ("peak_last", "<u4", (2,)), ("cur_rank", "<u2", (2,)),
+                             ("peak_rank", "<u2", (2,))])
+assert _LAYER_ROW_DTYPE.itemsize == 56
+_SNAP_BYTES = 48
+_WAITING = "Waiting for timing data from all ranks."
+
+
+def _layer_names_hash(names: Sequence[str]) -> List[float]:
+    """64-bit digest of an ordered layer-name list, as two exact f64 halves."""
+    import hashlib
+
+    h = int.from_bytes(hashlib.blake2b("\0".join(names).encode(), digest_size=8).digest(), "little")
+    return [float(h >> 32), float(h & 0xFFFFFFFF)]
+
+
+class LayerCombinedTimerData:
+    """The live layer-time panel, ``LayerCombinedTimerData`` of the reference
+    (renderers/layer_combined_time/compute.py:44-361), over this package's layer rings.
+
+    ``profiles`` are the ``LayerProfile``s of this process, one per local engine (rank
+    ``comm.index * len(profiles) + i``).  Each tick: ``tml_layer_tick_bounds`` per local rank and
+    one small all-gather pick the safe step; ``tml_layer_tick_snapshot`` per local rank, one
+    all-gather of the ``[n_layers]`` snapshots and ``tml_layer_tick_fold`` reduce across ranks on
+    the device; the EMA caches, the ordering and the top-N / "other" rows stay on the host
+    (O(n_layers) scalars).  The device stages run on a side stream, never the training stream.
+    Layers are joined across ranks by index: every rank must profile the same ordered layer list.
+    """
+
+    def __init__(self, profiles: Sequence[Any], comm: Any = None, *, top_n_layers: int = 20,
+                 ema_alpha: float = 0.10, device: Optional[torch.device] = None,
+                 use_side_stream: bool = True) -> None:
+        self.profiles = list(profiles)
+        self.comm = comm or LocalComm()
+        self.L = len(self.profiles)
+        self._top_n = int(top_n_layers)
+        self._ema_alpha = float(ema_alpha)
+        self.names: List[str] = list(self.profiles[0].names)
+        self.device = device or torch.device("cuda", self.profiles[0].engine.device)
+        self._stream = None
+        if use_side_stream and self.device.type == "cuda":
+            self._stream = torch.cuda.Stream(device=self.device)
+        self._lib = _abi.lib()
+        self._forward_cache: Dict[str, Dict[str, Any]] = {}
+        self._backward_cache: Dict[str, Dict[str, Any]] = {}
+        self._join_status: Optional[Dict[str, Any]] = None
+        self._worst_rank_by_layer: Dict[str, int] = {}
+        self._mismatch: Optional[List[int]] = None  # ranks whose layer list differs from rank 0's
+        self._last: Optional[Dict[str, Any]] = None
+        self.last_timings_ms: Dict[str, float] = {}
+
+    @property
+    def world_size(self) -> int:
+        return self.comm.world * self.L
+
+    def compute_display_data(self) -> Dict[str, Any]:
+        """compute.py:77-109, as ``dataclasses.asdict(LayerCombinedTimerResult)``.  A tick that
+        raises returns the last result (or the empty one): the live view never takes training down."""
+        try:
+            if self._stream is not None:
+                with torch.cuda.stream(self._stream):
+                    result = self._compute_impl()
+            else:
+                result = self._compute_impl()
+        except Exception:  # noqa: BLE001
+            return self._last if self._last is not None else self._empty_result(self.world_size)
+        self._last = result
+        return result
+
+    # ------------------------------------------------------------------ device stages + exchanges
+    def _sid(self) -> int:
+        if self.device.type != "cuda":
+            return 0
+        return int(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _identity(self) -> List[int]:
+        if self._mismatch is None:
+            flat: List[float] = []
+            for p in self.profiles:
+                flat += _layer_names_hash(p.names)
+            gathered = [row[i * 2:(i + 1) * 2] for row in self.comm.all_gather_vec(flat, self.device)
+                        for i in range(self.L)]
+            self._mismatch = [r for r, h in enumerate(gathered) if h != gathered[0]]
+        return self._mismatch
+
+    def _compute_impl(self) -> Dict[str, Any]:
+        t0 = time.perf_counter()
+        W, sid, lib = self.world_size, self._sid(), self._lib
+        bad = self._identity()
+        if bad:
+            out = self._empty_result(W)
+            out["status_message"] = (f"Layer lists differ across ranks: ranks {bad} do not profile "
+                                     "the same ordered layers as rank 0.")
+            return out
+        # bounds: [newest forward step, newest backward step, has forward rows, has backward rows]
+        flat: List[float] = []
+        nf, nb, old = _abi.u64(0), _abi.u64(0), _abi.u64(0)
+        for p in self.profiles:
+            if not p.names:
+                flat += [0.0, 0.0, 0.0, 0.0]
+                continue
+            has = _abi.check(lib.tml_layer_tick_bounds(p.engine._h, C.byref(nf), C.byref(nb), C.byref(old), sid),
+                             "tml_layer_tick_bounds")
+            flat += [float(nf.value), float(nb.value), float(has & _abi.LAYER_HAS_FWD),
+                     float(has & _abi.LAYER_HAS_BWD)]
+        steps: List[int] = []  # compute.py:111-135: a rank without both tables is left out
+        for row in self.comm.all_gather_vec(flat, self.device):
+            for l in range(self.L):
+                v = row[l * 4:(l + 1) * 4]
+                if v[2] and v[3]:
+                    steps.append(min(int(v[0]), int(v[1])))
+        if not steps or not self.names:
+            return self._empty_result(W)
+        safe_step = min(steps)
+        # snapshots -> one all-gather -> the cross-rank fold
+        n = len(self.names)
+        dev = self.device
+        local = torch.empty(self.L, n * _SNAP_BYTES, dtype=torch.uint8, device=dev)
+        for l, p in enumerate(self.profiles):
+            _abi.check(lib.tml_layer_tick_snapshot(p.engine._h, int(safe_step), local[l].data_ptr(), sid),
+                       "tml_layer_tick_snapshot")
+        if self.comm.world == 1:
+            snaps = local
+        else:
+            snaps = torch.empty(W * n * _SNAP_BYTES, dtype=torch.uint8, device=dev)
+            self.comm.all_gather_into(snaps, local.view(-1))
+        out = torch.empty(n * _LAYER_ROW_DTYPE.itemsize + W * 4, dtype=torch.uint8, device=dev)
+        _abi.check(lib.tml_layer_tick_fold(self.profiles[0].engine._h, snaps.data_ptr(), W, n, out.data_ptr(), sid),
+                   "tml_layer_tick_fold")
+        host = out.cpu().numpy()
+        rows = host[:n * _LAYER_ROW_DTYPE.itemsize].view(_LAYER_ROW_DTYPE)
+        rank_flags = host[n * _LAYER_ROW_DTYPE.itemsize:].view(np.uint32)
+        self.last_timings_ms = {"device": (time.perf_counter() - t0) * 1e3}
+
+        # compute.py:87-109 on the folded rows
+        fwd_missing = [r for r in range(W) if not rank_flags[r] & _abi.LSNAP_RANK_FWD]
+        bwd_missing = [r for r in range(W) if not rank_flags[r] & _abi.LSNAP_RANK_BWD]
+        missing_ranks = sorted(set(fwd_missing) | set(bwd_missing))
+        self._join_status = {"safe_step": int(safe_step), "incomplete": bool(missing_ranks),
+                             "missing_ranks": missing_ranks, "world_size": W}
+        self._merge_cache(self._forward_cache, self._snapshot(rows, 0))
+        self._merge_cache(self._backward_cache, self._snapshot(rows, 1))
+        self._worst_rank_by_layer = {self.names[i]: w for i, w in enumerate(rows["worst_rank"].tolist()) if w >= 0}
+        result = self._build_result()
+        self.last_timings_ms["tick"] = (time.perf_counter() - t0) * 1e3
+        return result
+
+    # ------------------------------------------------------------------ host part (O(n_layers))
+    def _snapshot(self, rows: np.ndarray, d: int) -> Dict[str, Dict[str, Any]]:
+        """compute.py:189-196.  The reference fills ``layer_current`` / ``layer_peak`` rank by rank
+        (and, for the peaks, newest row first) and iterates their union as a Python set: the dicts
+        are filled here in that same first-seen order, so the set -- and every float sum taken
+        over it downstream -- iterates in the reference's order."""
+        cbit, pbit = _abi.LSNAP_CUR_FWD << d, _abi.LSNAP_PEAK_FWD << d
+        flags, names = rows["flags"], self.names
+        ci = np.flatnonzero(flags & cbit)
+        ci = ci[np.argsort(rows["cur_rank"][ci, d], kind="stable")]         # (first rank, layer)
+        pi = np.flatnonzero(flags & pbit)
+        pi = pi[np.lexsort((pi, -rows["peak_last"][pi, d].astype(np.int64),  # (first rank, newest row, layer)
+                            rows["peak_rank"][pi, d]))]
+        cur_ms, peak_ms = rows["cur_ms"][:, d].tolist(), rows["peak_ms"][:, d].tolist()
+        layer_current = {names[i]: cur_ms[i] for i in ci.tolist()}
+        layer_peak = {names[i]: peak_ms[i] for i in pi.tolist()}
+        return {k: {"current": layer_current.get(k, 0.0), "peak": layer_peak.get(k, 0.0),
+                    "on_gpu": k in layer_current}
+                for k in set(layer_current) | set(layer_peak)}
+
+    def _merge_cache(self, cache: Dict[str, Dict[str, Any]], snapshot: Dict[str, Dict[str, Any]]) -> None:
+        """compute.py:217-237: every tick, also when the safe step did not move."""
+        a = self._ema_alpha
+        for layer, v in snapshot.items():
+            cur = float(v["current"])
+            peak = float(v["peak"])
+            if layer not in cache:
+                cache[layer] = {"current": cur, "avg": cur, "peak": peak, "on_gpu": v["on_gpu"]}
+            else:
+                cache[layer]["current"] = cur
+                cache[layer]["avg"] = (1 - a) * cache[layer]["avg"] + a * cur
+                cache[layer]["peak"] = max(cache[layer]["peak"], peak)
+                cache[layer]["on_gpu"] |= v["on_gpu"]
+
+    def _build_result(self) -> Dict[str, Any]:
+        """compute.py:255-323."""
+        join = self._join_status
+        layers = set(self._forward_cache) | set(self._backward_cache)
+        rows: List[Dict[str, Any]] = []
+        total_sum = 0.0
+        for layer in layers:
+            f = self._forward_cache.get(layer, {})
+            b = self._backward_cache.get(layer, {})
+            total_cur = f.get("current", 0.0) + b.get("current", 0.0)
+            rows.append({
+                "layer": layer,
+                "forward_current": f.get("current", 0.0), "forward_avg": f.get("avg", 0.0),
+                "forward_peak": f.get("peak", 0.0),
+                "backward_current": b.get("current", 0.0), "backward_avg": b.get("avg", 0.0),
+                "backward_peak": b.get("peak", 0.0),
+                "total_current": total_cur, "total_avg": f.get("avg", 0.0) + b.get("avg", 0.0),
+                "total_peak": f.get("peak", 0.0) + b.get("peak", 0.0),
+                "pct": 0.0, "worst_rank": self._worst_rank_by_layer.get(layer),
+                "on_gpu": f.get("on_gpu", b.get("on_gpu", False)),
+            })
+            total_sum += total_cur
+        out = []
+        for r in sorted(rows, key=lambda r: r["total_avg"], reverse=True):
+            out.append({**r, "pct": (r["total_current"] / total_sum * 100.0) if total_sum else 0.0})
+        top, rest = out[: self._top_n], out[self._top_n:]
+        other = {"total_forward_current": sum(r["forward_current"] for r in rest),
+                 "total_forward_avg": sum(r["forward_avg"] for r in rest),
+                 "total_backward_current": sum(r["backward_current"] for r in rest),
+                 "total_backward_avg": sum(r["backward_avg"] for r in rest),
+                 "pct": sum(r["pct"] for r in rest)}
+        status = (f"Step snapshot incomplete at step={join['safe_step']}. Missing ranks: {join['missing_ranks']}"
+                  if join and join["incomplete"] else "Timing snapshot ready.")
+        return {"top_items": top, "all_items": out, "other": other,
+                "safe_step": join["safe_step"] if join else None,
+                "incomplete": join["incomplete"] if join else False,
+                "missing_ranks": join["missing_ranks"] if join else [],
+                "world_size": join["world_size"] if join else self.world_size,
+                "status_message": status}
+
+    @staticmethod
+    def _empty_result(world_size: int) -> Dict[str, Any]:
+        """compute.py:344-361."""
+        return {"top_items": [], "all_items": [],
+                "other": {"total_forward_current": 0.0, "total_forward_avg": 0.0,
+                          "total_backward_current": 0.0, "total_backward_avg": 0.0, "pct": 0.0},
+                "safe_step": None, "incomplete": True, "missing_ranks": list(range(world_size)),
+                "world_size": world_size, "status_message": _WAITING}

@@ -314,10 +314,25 @@ def to_reference_step_memory_combined(result: Dict[str, Any]):
     return StepMemoryCombinedResult(metrics=metrics, status_message=result["status_message"])
 
 
+def to_reference_layer_time(result: Dict[str, Any]):
+    """``live.LayerCombinedTimerData`` result -> the reference's ``LayerCombinedTimerResult``
+    (renderers/layer_combined_time/schema.py:12-73), what its layer-time renderer consumes."""
+    from traceml.renderers.layer_combined_time.schema import (LayerCombinedTimerOther, LayerCombinedTimerResult,
+                                                              LayerCombinedTimerRow)
+
+    return LayerCombinedTimerResult(
+        top_items=[LayerCombinedTimerRow(**r) for r in result["top_items"]],
+        all_items=[LayerCombinedTimerRow(**r) for r in result["all_items"]],
+        other=LayerCombinedTimerOther(**result["other"]), safe_step=result["safe_step"],
+        incomplete=result["incomplete"], missing_ranks=list(result["missing_ranks"]),
+        world_size=result["world_size"], status_message=result["status_message"])
+
+
 class ReferenceComputerAdapter:
-    """Drop-in for the ``_computer`` attribute of the kept renderers
-    (renderers/step_time/renderer.py:56, step_memory/renderer.py:60): same ``compute_cli`` /
-    ``compute_dashboard`` methods, reference dataclasses out, this package's live computer in."""
+    """Drop-in for the computer of the kept renderers (renderers/step_time/renderer.py:56,
+    step_memory/renderer.py:60: ``_computer``; layer_combined_time/renderer.py:42: ``_service``):
+    same ``compute_cli`` / ``compute_dashboard`` / ``compute_display_data`` methods, reference
+    dataclasses out, this package's live computer in."""
 
     def __init__(self, computer, convert):
         self._computer, self._convert = computer, convert
@@ -328,7 +343,11 @@ class ReferenceComputerAdapter:
     def compute_dashboard(self):
         return self._convert(self._computer.compute_dashboard())
 
+    def compute_display_data(self):
+        return self._convert(self._computer.compute_display_data())
 
-__all__ = ["to_reference_step_combined", "to_reference_step_memory_combined", "ReferenceComputerAdapter",
+
+__all__ = ["to_reference_step_combined", "to_reference_step_memory_combined", "to_reference_layer_time",
+           "ReferenceComputerAdapter",
            "build_final_summary", "reference_payloads", "reference_available", "default_identity",
            "to_reference_step_time", "to_reference_step_memory", "to_reference_process", "to_reference_system"]

@@ -1843,6 +1843,36 @@ __global__ void __launch_bounds__(256) k_bands(const __grid_constant__ BandParam
     return;
   }
   u64 lo = p.lo[kind][b], hi = p.hi[kind][b];
+  if (lo < hi && lo >= p.shard_lo && hi <= p.shard_hi) {
+    // The whole band is on this shard: its sum exactly as the reference's mean takes it (core.py:34,
+    // CPython >= 3.12 sum(): Neumaier's compensated sum, left to right, the compensation added once
+    // at the end when it is finite and non-zero), so a trend within ulps of a gate (+-8 %, the
+    // dead-band, %+.1f) gets the reference's verdict.  The CTA stages the band into shared memory
+    // and thread 0 runs the dependent chain.
+    __shared__ double s_v[1024];
+    double acc = 0.0, comp = 0.0;
+    for (u64 c = lo; c < hi; c += 1024) {
+      const u32 m = (hi - c) < 1024 ? (u32)(hi - c) : 1024u;
+      for (u32 k = threadIdx.x; k < m; k += 256) s_v[k] = v[c + k];
+      __syncthreads();
+      if (threadIdx.x == 0) {
+#pragma unroll 8
+        for (u32 k = 0; k < m; ++k) {
+          const double x = s_v[k], t = acc + x;
+          comp += fabs(acc) >= fabs(x) ? (acc - t) + x : (x - t) + acc;
+          acc = t;
+        }
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+      if (comp != 0.0 && isfinite(comp)) acc += comp;
+      out_sum[s * 3 + b] = acc;
+      out_cnt[s * 3 + b] = hi - lo;
+    }
+    return;
+  }
+  // A band split across shards: a tree here, then bands_collect's rank-order fold of the shards.
   if (lo < p.shard_lo) lo = p.shard_lo;
   if (hi > p.shard_hi) hi = p.shard_hi;
   double acc[1] = {0.0};

@@ -507,6 +507,7 @@ void unpack_align(const double* v, bool handles, Aligned* a) {
 
 // ------------------------------------------------------------------ trend band layout
 // analytics/trends/core.py:38-84 + schema.py:27-62, as traceml_b200/reduce.py:trend_layout
+// (tests/test_gpu_align_bands.py::test_build_band_layout keeps the two copies equal to the oracle's bands)
 bool trend_layout(u64 n, u64 min_points, double warmup_frac, u64 lo[3], u64 hi[3]) {
   static const double BANDS[3][2] = {{0.15, 0.25}, {0.45, 0.55}, {0.90, 1.00}};
   if (n < min_points) return false;

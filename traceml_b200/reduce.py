@@ -185,7 +185,9 @@ def _band_bounds(n: int, band) -> tuple:
 
 def trend_layout(n: int, *, min_points: int, warmup_frac: float):
     """Global series index ranges of the three trend bands, or None if the
-    series is too short (analytics/trends/core.py:51-84)."""
+    series is too short (analytics/trends/core.py:51-84).  csrc/tml_summary.cpp:trend_layout is the
+    native driver's copy: tests/test_gpu_align_bands.py::test_build_band_layout keeps both equal to
+    the oracle's bands."""
     if n < min_points:
         return None
     length = min(n, _HISTORY_LIMIT)
